@@ -1,10 +1,11 @@
 #!/usr/bin/env python
-"""bench.py - edges/sec of the Equiformer graph-attention hot path (fwd+bwd training step) on B200.
+"""bench.py - edges/sec of the Equiformer graph-attention hot path (fwd+bwd training step) on H100.
 
 Contract (one JSON line on stdout from rank 0):
-    python bench.py --gpus N --steps K --warmup W                    # sm_100a kernels behind the drop-in modules
+    python bench.py --gpus N --steps K --warmup W                    # sm_90a kernels behind the drop-in modules
     python bench.py --impl reference --gpus N --steps K --warmup W   # the oracle restatement on the host cores (CPU arm)
-    python bench.py --impl reference-gpu ...                         # the same reference-style op chain, eager torch on the B200
+    python bench.py --impl reference-gpu ...                         # the same reference-style op chain, eager torch on the GPU
+    python bench.py ... --dump-outputs DIR                           # also write the last timed step's results as DIR/*.npy
 
 Workloads (``--workload``; BASELINE.json ``configs``):
     qm9      [1] (default, the config the metric is quoted on) 128 molecules x ~18 atoms, radius 5 A, Lmax=2,
@@ -13,7 +14,8 @@ Workloads (``--workload``; BASELINE.json ``configs``):
              forces + L2-MAE loss (weights 1 / 100, scripts/train/md17/equiformer/se_l3/target@aspirin.sh:22-23) + double
              backward + AdamW
     oc20_l1  [3] 16 periodic frames x ~73 atoms x ~50 neighbours per GPU, ``l1_256_nonlinear`` (IS2RE), energy L1 loss
-    stress   [4] one periodic cell of 10 000 atoms, ~50 neighbours (E ~ 5e5), Lmax=2 model of [1]; replicas under --gpus N
+    stress   [4] one periodic cell of 5 000 atoms, ~50 neighbours (E ~ 2.5e5), Lmax=2 model of [1]; replicas under --gpus N
+             (the largest round cell whose captured training step fits the 80 GB of an H100)
 
 * ``value``    - edges/s with the step's inputs already resident in HBM when the timed region starts.
 * ``e2e``      - the same step from pinned HOST tensors: H2D copy of the inputs and D2H read of the loss inside the timed
@@ -22,7 +24,8 @@ Workloads (``--workload``; BASELINE.json ``configs``):
 * ``roofline`` - the dominant hand-written kernel family by summed device time (CUDA events around every launch of our
                  kernels in an instrumented eager pass): algorithmic bytes / time against the measured HBM copy bandwidth
                  AND, for contraction kernels, useful flops / time against the TF32 tensor roof (half the measured bf16
-                 throughput of MEASURED_PEAKS.json) - both are reported, ``bound`` names the nearer one.
+                 throughput of MEASURED_PEAKS.json, else the H100 SXM data sheet) - both are reported, ``bound`` names the
+                 nearer one.
 * ``cpu_baseline`` - the oracle (reference-style op chain, torch CPU) on a bounded sample of the same workload (N = 1 only).
 
 Multi-GPU: one process per GPU (torchrun), independent batch per rank (weak scaling), NCCL all-reduce of one flat gradient
@@ -56,8 +59,8 @@ WORKLOADS = {
     "oc20_l1": dict(metric="edges/sec fwd+bwd, OC20 IS2RE l1_256_nonlinear frames", model="graph_attention_transformer_oc20",
                     n_graphs=16, text="OC20 IS2RE synthetic frames: 16 periodic frames x ~73 atoms x ~50 neighbours per GPU, "
                                       "l1_256_nonlinear, fwd+bwd+AdamW"),
-    "stress": dict(metric="edges/sec fwd+bwd, 10k-atom periodic cell Lmax=2", model="graph_attention_transformer_nonlinear_l2",
-                   n_graphs=1, text="stress: one periodic cell of 10 000 atoms, ~50 neighbours within 5 A (E ~ 5e5), Lmax=2, "
+    "stress": dict(metric="edges/sec fwd+bwd, 5k-atom periodic cell Lmax=2", model="graph_attention_transformer_nonlinear_l2",
+                   n_graphs=1, text="stress: one periodic cell of 5 000 atoms, ~50 neighbours within 5 A (E ~ 2.5e5), Lmax=2, "
                                     "fwd+bwd+AdamW; one independent cell per GPU"),
 }
 
@@ -86,7 +89,7 @@ def make_inputs(workload: str, seed: int, n_graphs=None):
         return dict(pos=pos, batch=batch, z=z, tags=tags, cell=torch.diag_embed(cell[:, None].expand(-1, 3)).float(),
                     target=torch.randn(n, 1, generator=g))
     if workload == "stress":
-        pos, batch, z, side = S.stress_cell(n_graphs or 10000, seed=seed)
+        pos, batch, z, side = S.stress_cell(n_graphs or 5000, seed=seed)
         return dict(pos=pos, batch=batch, z=z, cell=(torch.eye(3) * side).view(1, 3, 3).float(), target=torch.randn(1, 1, generator=g))
     raise ValueError(workload)
 
@@ -99,7 +102,7 @@ def count_edges(workload: str, inp) -> int:
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region (read-only queries)."""
 
     QUERY = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
              "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -146,19 +149,7 @@ def measured_peaks():
         with open(path) as f:
             d = json.load(f)
         return float(d["hbm_gbs"]), float(d["bf16_tflops"]) / 2.0, "measured (MEASURED_PEAKS.json: hbm_gbs, bf16_tflops / 2)"
-    return 6650.0, 1125.0, "fallback (B200_PROFILING.md: 6.65 TB/s, 2.25 PFLOP/s bf16 / 2)"
-
-
-def ncu_traffic(kernel: str):
-    """dram bytes per launch of the dominant kernel from the committed ncu summary (profiles/), if present."""
-    path = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.exists(path):
-        try:
-            with open(path) as f:
-                return json.load(f).get(kernel)
-        except Exception:
-            return None
-    return None
+    return 3350.0, 989.0 / 2.0, "H100 SXM data sheet (700 W): 3.35 TB/s, 989 TFLOP/s bf16 dense / 2 - not measured"
 
 
 # --------------------------------------------------------------------------------------------------- reference arms
@@ -293,7 +284,7 @@ def run_reference(args):
     dt = (time.perf_counter() - t0) / args.steps
     value = edges / dt
     full = WORKLOADS[base]["n_graphs"]
-    where = "eager torch CUDA ops on the B200 (allow_tf32 off)" if gpu else "torch CPU fp32"
+    where = f"eager torch CUDA ops on the {torch.cuda.get_device_name()} (allow_tf32 off)" if gpu else "torch CPU fp32"
     sample = f"{n_graphs} of the {full} graphs ({edges} edges) per step, oracle op chain fwd+bwd, {where}"
     line = {"impl": args.impl, "metric": WORKLOADS[wl]["metric"], "value": value, "unit": "edges/s", "n_gpus": args.gpus,
             "steps": args.steps, "warmup": args.warmup, "ms_per_step": dt * 1e3, "higher_is_better": True,
@@ -337,8 +328,7 @@ def run_ours(args):
     if not torch.cuda.is_available():
         raise RuntimeError("bench.py needs a CUDA device: the edge path has no CPU implementation "
                            "(use --impl reference for the CPU oracle)")
-    if not _lib.LIB_PATH.exists():
-        _lib.build()
+    _lib.load()                    # the library build() left in the tree; the benchmark compiles nothing
     wl = args.workload
     rank, local, world = init_distributed("nccl")
     torch.cuda.set_device(local)
@@ -505,6 +495,8 @@ def run_ours(args):
     clocks = sampler.stop() if sampler else None
     ms_e2e, last_loss = timed(args.steps if args.stream <= 1 else max(args.steps, len(hosts)), from_host=True, profile=None,
                               stream=args.stream > 1)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last_loss, bucket.flat, opt.flat)
 
     edges_total = torch.tensor([edges_of[0]], device=dev, dtype=torch.float64)
     edges_stream = torch.tensor([edges_local], device=dev, dtype=torch.float64)
@@ -541,7 +533,7 @@ def run_ours(args):
                     "hbm": {"achieved": gbs, "peak": hbm_peak, "frac": f_hbm, "unit": "GB/s"},
                     "tensor": {"achieved_useful": tfs, "peak_tf32_dense": tf32_peak, "frac": f_tensor, "unit": "TFLOP/s",
                                "note": "useful fp32 flops; the 3xTF32 scheme issues 3 tensor-core products per useful one"},
-                    "traffic": ncu_traffic(dominant), "peak_source": peak_src,
+                    "peak_source": peak_src,
                     "bytes_per_launch": d["bytes"] / d["launches"], "us_per_launch": d["ms"] * 1e3 / d["launches"],
                     "share_of_step": d["ms"] / (ms_step * n_prof_steps), "launches_per_step": d["launches"] / n_prof_steps,
                     "runner_up": {k: entry(k) for k in sorted(own, key=lambda k: -own[k]["ms"])[1:4]},
@@ -576,10 +568,10 @@ def run_ours(args):
                        "dropout": (f"attention-weight dropout p = {args.alpha_drop} (reference default 0.2; the only stochastic op "
                                    "of the step; p = 0 keeps the run comparable with the parity tests)"),
                        "fused": (f"EQF_FUSED={ops._FUSED_MODE}: the depth-wise tensor product is produced on chip as the A operand of "
-                                 f"the tcgen05 GEMMs (K1) from {ops._FUSED_MIN_EDGES} edges per call in 'auto' mode - "
+                                 f"the wgmma GEMMs (K1) from {ops._FUSED_MIN_EDGES} edges per call in 'auto' mode - "
                                  + ("ON" if ops._FUSED and (ops._FUSED_MODE == "1" or edges_of[0] >= ops._FUSED_MIN_EDGES) else "OFF")
                                  + " for this workload"),
-                       "gemm": ("tcgen05 3xTF32, hand-written (forward / dgrad from "
+                       "gemm": ("wgmma 3xTF32, hand-written (forward / dgrad from "
                                 f"{ops._GEMM_MIN_M} rows, wgrad from {ops._WGRAD_MIN_K} reduction rows); below "
                                 "that the grouped warp-MMA 3xTF32 kernel (all degrees of a linear per launch); no cuBLAS on the path")
                                if ops.gemm_backend() == "tf32x3" else ops.gemm_backend(),
@@ -591,6 +583,7 @@ def run_ours(args):
                     "ms_per_step": ms_e2e, "h2d_bytes_per_step": h2d_bytes, "d2h_bytes_per_step": 4,
                     "distinct_batches": len(hosts), "captures": getattr(graphed, "captures", None)},
             "gpu_launches": profile.launches // max(n_prof_steps, 1),   # our kernels launched per step (instrumented pass)
+            "device": torch.cuda.get_device_name(dev), "power_limit_w": power_limit(local),
             "clocks": clocks, "roofline": roof, "cpu_baseline": cpu, "kernels": kernels,
             "loss": last_loss, "grad_bucket_bytes": bucket.nbytes,
         }
@@ -598,6 +591,46 @@ def run_ours(args):
     if world > 1:
         dist.barrier()
         dist.destroy_process_group()
+
+
+DUMP_BUDGET_BYTES = 64 << 20        # every file of one dump together
+DUMP_MAX_ELEMENTS = 4 << 20          # per flat array: 16 MB of float32, so loss + gradients + parameters stay within budget
+
+
+def dump_sample(n: int) -> torch.Tensor:
+    """The entries a dump keeps of a flat array of ``n`` > DUMP_MAX_ELEMENTS: a fixed, seeded choice, in ascending order.
+    It depends on ``n`` only, so two builds (or a reader of the dump) recompute the same indices."""
+    return torch.randperm(n, generator=torch.Generator().manual_seed(0))[:DUMP_MAX_ELEMENTS].sort().values
+
+
+def dump_outputs(out_dir: str, loss: float, grads: torch.Tensor, params: torch.Tensor) -> None:
+    """What the last timed step handed back: its loss (float64), the flat gradient of every parameter and the parameters
+    after the optimizer update (float32) as .npy files.  A flat array longer than DUMP_MAX_ELEMENTS is replaced by the
+    entries ``dump_sample`` picks, so that two builds can be compared entry for entry; all files together stay within
+    DUMP_BUDGET_BYTES."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    paths = [os.path.join(out_dir, "loss.npy")]
+    np.save(paths[0], np.array([loss], dtype=np.float64))
+    for name, t in (("grads", grads), ("params", params)):
+        flat = t.detach().float().reshape(-1).cpu()
+        if flat.numel() > DUMP_MAX_ELEMENTS:
+            flat = flat[dump_sample(flat.numel())]
+        paths.append(os.path.join(out_dir, f"{name}.npy"))
+        np.save(paths[-1], flat.numpy().astype(np.float32))
+    total = sum(os.path.getsize(p) for p in paths)
+    if total > DUMP_BUDGET_BYTES:
+        raise RuntimeError(f"--dump-outputs wrote {total} bytes, more than the {DUMP_BUDGET_BYTES} allowed")
+
+
+def power_limit(index: int):
+    """The card's power limit in W (nvidia-smi query; None when unavailable) - part of every number measured on it."""
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader,nounits", "-i", str(index)],
+                             capture_output=True, text=True, timeout=10).stdout.strip()
+        return float(out)
+    except (OSError, ValueError, subprocess.SubprocessError):
+        return None
 
 
 def main():
@@ -613,7 +646,13 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--graph", dest="graph", action="store_true", default=True)
     ap.add_argument("--no-graph", dest="graph", action="store_false")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's loss, gradients and updated parameters as DIR/*.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.dump_outputs and args.impl != "ours":
+        ap.error("--dump-outputs writes the results of the timed path of --impl ours only")
     if args.stream > 1 and args.workload != "qm9":
         ap.error("--stream is implemented for the qm9 workload")
     if args.impl in ("reference", "reference-gpu"):

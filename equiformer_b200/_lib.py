@@ -1,6 +1,6 @@
 """ctypes binding of ``libeqf_b200.so`` (C ABI declared in ``include/eqf_b200.h``).
 
-The shared library is built in-tree by :func:`build` (``nvcc -gencode arch=compute_100a,code=sm_100a``)
+The shared library is built in-tree by :func:`build` (``nvcc -gencode arch=compute_90a,code=sm_90a``)
 and loaded lazily.  There is deliberately **no fallback**: if the library is missing or a kernel entry
 point fails, the call raises - the product path never routes through a CPU or eager-torch restatement
 (the only CPU restatement lives in ``oracle/`` and is test infrastructure).
@@ -21,15 +21,13 @@ INCLUDE_DIR = PKG_DIR.parent / "include"
 LIB_PATH = PKG_DIR / "libeqf_b200.so"
 SOURCES = ("eqf_abi.cu", "eqf_dtp.cu", "eqf_dtp_vec.cu", "eqf_dtp_v3.cu", "eqf_attn.cu", "eqf_pointwise.cu", "eqf_gemm_tf32x3.cu", "eqf_graph.cu",
            "eqf_fused.cu", "eqf_edge.cu", "eqf_gemm_small.cu")
-GEMM_LIB_PATH = PKG_DIR / "libeqf_gemm.so"
-GEMM_SOURCES = ("eqf_gemm.cu",)
 
 EQF_COLSUM_COUNTERS = 16384
 EQF_MAX_BLOCKS = 8
 EQF_MAX_HEADS = 16
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17", "--shared", "-Xcompiler", "-fPIC",
 ]
 
@@ -131,7 +129,6 @@ SIGNATURES = {
                                   c_void_p, c_void_p, c_void_p]),
     "eqf_gemm_tf32x3": (c_int32, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64, c_int64, c_int32,
                                   c_void_p, c_void_p]),
-    "eqf_gemm_tf32x3_set_timeline": (None, [c_void_p]),
     "eqf_gemm_tf32x3_wgrad_slices": (c_int64, [c_int64, c_int64, c_int64]),
     "eqf_gemm_tf32x3_wgrad": (c_int32, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64, c_void_p]),
     "eqf_gemm_tf32x3_wgrad_accumulate": (c_int32, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64,
@@ -174,17 +171,6 @@ SIGNATURES = {
 }
 
 
-GEMM_SIGNATURES = {
-    "eqf_gemm_f32": (c_int32, [c_int32, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64,
-                                c_int64, c_float, c_void_p, c_int64, c_void_p]),
-    "eqf_gemm_f32_wgrad_sliced": (c_int32, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64,
-                                            c_int64, c_void_p, c_int64, c_void_p]),
-    "eqf_gemm_workspace_bytes": (c_int64, []),
-    "eqf_gemm_last_error": (c_char_p, []),
-    "eqf_gemm_config": (c_int32, [POINTER(c_int32), POINTER(c_int32), POINTER(c_int32)]),
-}
-
-
 class EqfError(RuntimeError):
     pass
 
@@ -213,14 +199,14 @@ def needs_build() -> bool:
 
 
 def build(force: bool = False, verbose: bool = False) -> Path:
-    """Compile ``csrc/*.cu`` for sm_100a into ``equiformer_b200/libeqf_b200.so`` (in-tree)."""
+    """Compile ``csrc/*.cu`` for sm_90a into ``equiformer_b200/libeqf_b200.so`` (in-tree)."""
     generate_sources()
     if not force and not needs_build():
         return LIB_PATH
     nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
     if not os.path.exists(nvcc):
         raise EqfError("nvcc not found: cannot build libeqf_b200.so")
-    # one nvcc per source file, in parallel (the plan-specialised and the tcgen05 files take a minute each), then one
+    # one nvcc per source file, in parallel (the plan-specialised files take a minute each), then one
     # link step; objects live in a scratch directory next to the library
     from concurrent.futures import ThreadPoolExecutor
     obj_dir = PKG_DIR / "build" / ("obj%d" % os.getpid())
@@ -243,7 +229,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
             if verbose:
                 print(proc.stderr)
         tmp = LIB_PATH.with_suffix(".so.tmp%d" % os.getpid())
-        link = subprocess.run([nvcc, "--shared", "-Xcompiler", "-fPIC", "-gencode", "arch=compute_100a,code=sm_100a",
+        link = subprocess.run([nvcc, "--shared", "-Xcompiler", "-fPIC", "-gencode", "arch=compute_90a,code=sm_90a",
                                "-o", str(tmp), *[str(o) for o, _ in results]], capture_output=True, text=True)
         if link.returncode != 0:
             raise EqfError("nvcc link failed:\n" + link.stdout + link.stderr)
@@ -251,76 +237,6 @@ def build(force: bool = False, verbose: bool = False) -> Path:
     finally:
         shutil.rmtree(obj_dir, ignore_errors=True)
     return LIB_PATH
-
-
-def cutlass_include_dirs():
-    """CUTLASS/CuTe header trees vendored in site-packages (Environment section of the task statement)."""
-    import importlib.util
-    for pkg, rel in (("flashinfer", "data/cutlass"), ("tilelang", "3rdparty/cutlass")):
-        spec = importlib.util.find_spec(pkg)
-        if spec is None or not spec.submodule_search_locations:
-            continue
-        root = Path(list(spec.submodule_search_locations)[0]) / rel
-        if (root / "include" / "cutlass" / "cutlass.h").exists():
-            dirs = [root / "include"]
-            if (root / "tools" / "util" / "include").exists():
-                dirs.append(root / "tools" / "util" / "include")
-            return dirs
-    raise EqfError("CUTLASS headers not found (expected under site-packages/flashinfer/data/cutlass)")
-
-
-def gemm_needs_build() -> bool:
-    if not GEMM_LIB_PATH.exists():
-        return True
-    mtime = GEMM_LIB_PATH.stat().st_mtime
-    deps = [CSRC_DIR / s for s in GEMM_SOURCES] + [INCLUDE_DIR / "eqf_b200.h"]
-    return any(p.stat().st_mtime > mtime for p in deps if p.name != "eqf_b200.h") or not GEMM_LIB_PATH.exists()
-
-
-def build_gemm(force: bool = False) -> Path:
-    """Compile the CUTLASS fast-fp32 (tcgen05) GEMM instantiations into ``libeqf_gemm.so`` (takes minutes)."""
-    if not force and not gemm_needs_build():
-        return GEMM_LIB_PATH
-    nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
-    tmp = GEMM_LIB_PATH.with_suffix(".so.tmp%d" % os.getpid())
-    inc = []
-    for d in cutlass_include_dirs():
-        inc += ["-I", str(d)]
-    cmd = [nvcc, *NVCC_FLAGS, "--expt-relaxed-constexpr", "-diag-suppress", "20012", *inc, "-I", str(INCLUDE_DIR),
-           "-o", str(tmp), *[str(CSRC_DIR / s) for s in GEMM_SOURCES]]
-    proc = subprocess.run(cmd, capture_output=True, text=True)
-    if proc.returncode != 0:
-        raise EqfError("nvcc failed (gemm):\n" + proc.stdout[-4000:] + proc.stderr[-4000:])
-    os.replace(tmp, GEMM_LIB_PATH)
-    return GEMM_LIB_PATH
-
-
-_gemm_lib = None
-
-
-def load_gemm():
-    global _gemm_lib
-    if _gemm_lib is not None:
-        return _gemm_lib
-    with _lock:
-        if _gemm_lib is not None:
-            return _gemm_lib
-        path = Path(os.environ.get("EQF_GEMM_LIB", GEMM_LIB_PATH))     # override: tuning variants (tools/gemm_microbench.py)
-        if not path.exists():
-            raise EqfError(f"{path} is missing: run __graft_entry__.build()")
-        lib = ctypes.CDLL(str(path))
-        for name, (restype, argtypes) in GEMM_SIGNATURES.items():
-            fn = getattr(lib, name)
-            fn.restype = restype
-            fn.argtypes = argtypes
-        _gemm_lib = lib
-    return _gemm_lib
-
-
-def check_gemm(rc: int, what: str) -> None:
-    if rc != 0:
-        msg = load_gemm().eqf_gemm_last_error()
-        raise EqfError(f"{what} failed (code {rc}): {msg.decode() if msg else '?'}")
 
 
 def load():
@@ -334,7 +250,7 @@ def load():
         if not LIB_PATH.exists():
             raise EqfError(
                 f"{LIB_PATH} is missing: run `python -c 'import __graft_entry__ as g; g.build()'` "
-                "(the sm_100a kernels are the only implementation of the edge path)")
+                "(the sm_90a kernels are the only implementation of the edge path)")
         lib = ctypes.CDLL(str(LIB_PATH))
         for name, (restype, argtypes) in SIGNATURES.items():
             try:

@@ -471,13 +471,13 @@ extern "C" int eqf_attn_edge_scale(const EqfHeadLayout* lay, const float* alpha,
   }
   if (vec_ok(a)) {
     long long vb = (n_edges + 7) / 8;
-    if (vb > 148LL * 16) vb = 148LL * 16;
+    if (vb > 132LL * 16) vb = 132LL * 16;
     edge_scale_vec_kernel<<<(unsigned)(vb < 1 ? 1 : vb), 256, 0, (cudaStream_t)stream>>>(
         a, alpha, reinterpret_cast<const long long*>(dst), n_edges);
     return check_cuda(cudaGetLastError(), "edge_scale_vec_kernel launch");
   }
   long long blocks = (n_edges * max_rowlen + 255) / 256;
-  if (blocks > 148LL * 32) blocks = 148LL * 32;
+  if (blocks > 132LL * 32) blocks = 132LL * 32;
   if (blocks < 1) blocks = 1;
   dim3 grid((unsigned)blocks, (unsigned)a.n_groups);
   edge_scale_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(a, alpha, reinterpret_cast<const long long*>(dst), n_edges);

@@ -1,4 +1,4 @@
-// eqf_common.cuh - shared device/host definitions for libeqf_b200.so (sm_100a).
+// eqf_common.cuh - shared device/host definitions for libeqf_b200.so (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -93,7 +93,7 @@ struct EqfPlan {
   std::vector<uint32_t> blob;   // host copy
   uint32_t* d_blob = nullptr;   // device copy
   int device = -1;
-  int sm_count = 148;
+  int sm_count = 132;
   size_t smem_bytes = 0;        // dynamic shared memory per CTA (scalar kernels)
   size_t smem_bytes_vec_fwd = 0;  // vector forward (includes the TMA weight ring)
   size_t smem_bytes_vec_bwd = 0;  // vector grad_x / grad_xw

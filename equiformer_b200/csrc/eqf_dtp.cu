@@ -1,4 +1,4 @@
-// eqf_dtp.cu - the depth-wise tensor product (DTP) contraction family for sm_100a.
+// eqf_dtp.cu - the depth-wise tensor product (DTP) contraction family for sm_90a.
 //
 // Reference work replaced: o3.TensorProduct('uvu') inside TensorProductRescale
 // (nets/tensor_product_rescale.py:33-37,126) as instantiated by DepthwiseTensorProduct
@@ -14,7 +14,7 @@
 // path is a (2l1+1)x(2l3+1) mat-vec per channel held entirely in registers.
 //
 // HBM-bound streaming kernels: per edge the forward moves 4*(D_in + D_y + W + D_out) bytes for about
-// 2*sum_p mul*(2l1+1)*(2l3+1) flops (QM9 Lmax=2: 18 340 B vs 17 kflop) - see DESIGN.md.
+// 2*sum_p mul*(2l1+1)*(2l3+1) flops (QM9 Lmax=2: 18 340 B vs 17 kflop).
 #include <mutex>
 #include <unordered_map>
 

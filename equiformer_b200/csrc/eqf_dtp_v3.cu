@@ -1,8 +1,7 @@
-// eqf_dtp_v3.cu - third-generation DTP kernels (sm_100a): software-pipelined tiles, one barrier per tile.
+// eqf_dtp_v3.cu - third-generation DTP kernels (sm_90a): software-pipelined tiles, one barrier per tile.
 //
-// What the ncu captures of the second generation showed (profiles/r1_ncu_dtp_v2.md): DRAM traffic == algorithmic bytes
-// but only ~38 % of DRAM peak; issue slots 42 % busy with FFMA only 13 % of the instructions (integer address/divide
-// overhead), barrier + long-scoreboard stalls exposed because a tile went load-y -> barrier -> fold -> barrier -> work.
+// What profiling of the second generation showed: DRAM traffic == algorithmic bytes but far from DRAM peak; FFMA a small
+// share of the issued instructions (integer address/divide overhead), barrier + long-scoreboard stalls exposed because a tile went load-y -> barrier -> fold -> barrier -> work.
 // This generation therefore
 //   * pipelines the per-tile staging: edge harmonics of tile t+2 are loaded into registers while tile t is processed,
 //     the fold M_p = C_p.y of tile t+1 runs before the work of tile t, buffers are double - ONE __syncthreads per tile;

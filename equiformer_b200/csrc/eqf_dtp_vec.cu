@@ -1,4 +1,4 @@
-// eqf_dtp_vec.cu - vectorised (128-bit per lane) DTP kernels with TMA-staged radial weights, sm_100a.
+// eqf_dtp_vec.cu - vectorised (128-bit per lane) DTP kernels with TMA-staged radial weights, sm_90a.
 //
 // Same math and tables as eqf_dtp.cu; what changes is how bytes move:
 //   * every lane owns FOUR consecutive channels: all global accesses are 16-byte LDG/STG, a warp instruction

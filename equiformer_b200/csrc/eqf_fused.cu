@@ -1,5 +1,5 @@
 // eqf_fused.cu - K1: the depth-wise tensor product produced ON CHIP as the A operand of the per-degree channel-mixing
-// GEMM that follows it (sm_100a).  Reference path: nets/graph_attention_transformer.py:487-496 -
+// GEMM that follows it (sm_90a).  Reference path: nets/graph_attention_transformer.py:487-496 -
 //   message = src[edge_src] + dst[edge_dst]; f = dtp(message, edge_attr, dtp_rad(edge_scalars)); lin(f) / sep_alpha(f)
 // (e3nn 'uvu' tensor product -> [E, 3136] in HBM -> 'uvw' einsum = cuBLAS GEMM).  Here, per output degree l3 (group):
 //
@@ -7,25 +7,22 @@
 //   M_p[e][i, k] = sum_j CG_p[i, j, k] y[e, j]   (the edge's (2 l1 + 1) x (2 l3 + 1) coupling block, channel independent)
 //
 // and f never reaches HBM.  One CTA per SM, persistent over 128-row x n_tile output tiles (rows = (edge, component)
-// pairs of ONE output degree), warp-specialised like eqf_gemm_tf32x3.cu's tensor-memory kernel:
-//   warps 0-3    epilogue      TMEM accumulator -> registers -> swizzled staging -> TMA store of C
-//   warp  4      TMA producer  weight tiles B_hi / B_lo of the k-tile (K-major planes, 128-byte rows) and, for per-edge
-//                              weights, a box of the [E, W] radial-weight matrix - one "operand slot" per k-tile
-//   warp  5      MMA issuer    tcgen05.mma.kind::tf32, A from TENSOR MEMORY, 3xTF32 (stacked [b_hi | b_lo] for N <= 64)
-//   warps 6-7    table helpers ONE ROW BLOCK AHEAD: the block's src / dst rows and harmonics into shared memory, then the
-//                              coupling blocks M_p[e] from the group's CG blocks (double-buffered, tab_ready / tab_free)
-//   warps 8-11   transform     raw A tile (shared memory) -> a_hi / a_lo in tensor memory (one thread = one row)
-//   warps 12-27  DTP producers two sets of 8 warps alternate k-tiles: gather x = A[src] + B[dst] (float4 per lane, node
-//                tables L2 resident; issued before the handshake), multiply by the radial weights, contract with M_p[e]
-//                (128-bit shared loads, dense) and write the 128 x 32 raw A tile (SWIZZLE_128B row order, conflict-free)
-// Three independent rings (v5): operand slots (TMA -> MMA commit), raw A tiles (producers -> transform loads), tensor-memory
-// A slots (transform -> MMA commit).  Register budget (896 threads x 72 at launch): setmaxnreg gives the TMA / MMA / helper
-// warpgroup 56 and the transform warpgroup 88.
-// History (profiles/r2_fused_fwd_v*, DESIGN.md section 4b): v1 computed M_p[e] with dependent GLOBAL loads of CG and y inside
-// the tile loop (~12 k cycles per tile); v2 moved the tables to two helper warps that walked the entries serially (28 us per
-// tile); v3 built them with all 16 DTP warps between two 512-thread barriers (7 k cycles per row block with the pipeline
-// drained) and tied weight tiles, raw tile and TMEM slot to ONE 5-deep ring; v4 = dense producer, cheaper table build,
-// wait hints (A/B: the producer's instruction count is not the limiter); v5 = this file.
+// pairs of ONE output degree), warp-specialised:
+//   warps 0-3, 8-11  consumers     (two warpgroups, 64 rows each) raw A tile -> registers -> a_hi / a_lo register
+//                                  fragments -> 3xTF32 wgmma against the weight tiles; accumulator in registers, stored
+//                                  to C at the end of the tile (eqf_tc.cuh)
+//   warp  4          TMA producer  weight tiles B_hi / B_lo of the k-tile (K-major planes, 128-byte rows) and, for per-edge
+//                                  weights, a box of the [E, W] radial-weight matrix - one "operand slot" per k-tile
+//   warps 6-7        table helpers ONE ROW BLOCK AHEAD: the block's src / dst rows and harmonics into shared memory, then the
+//                                  coupling blocks M_p[e] from the group's CG blocks (double-buffered, tab_ready / tab_free)
+//   warps 12-27      DTP producers two sets of 8 warps alternate k-tiles: gather x = A[src] + B[dst] (float4 per lane, node
+//                                  tables L2 resident; issued before the handshake), multiply by the radial weights, contract
+//                                  with M_p[e] (128-bit shared loads, dense) and write the 128 x 32 raw A tile (SWIZZLE_128B
+//                                  row order, conflict-free for the writers and for the consumers' fragment loads)
+// Two independent rings: operand slots (TMA -> consumers' MMAs) and raw A tiles (producers -> consumers' fragment loads).
+// Register budget (896 threads x 72 at launch): setmaxnreg gives the TMA / helper warpgroup 56 and each consumer
+// warpgroup 80; ptxas allocates the consumer within the 72 of the launch, so it holds a 64 x 64 accumulator and the
+// split fragments of half a k-tile at a time.
 #include <cuda.h>
 #include <cuda_runtime.h>
 
@@ -43,17 +40,16 @@ namespace fused {
 
 using namespace tc;
 
-constexpr int BM = 128;                 // rows per tile (UMMA M)
-constexpr int BKT = 32;                 // channels per k-tile: 128-byte rows
+constexpr int BM = 128;                 // rows per tile (two consumer warpgroups of 64)
+constexpr int BKT = kKTile;             // channels per k-tile: 128-byte rows
 constexpr int kRowBytes = BKT * 4;
-constexpr int UMMA_K = 8;
-constexpr int kStoreCols = 32;
-constexpr int kEpilogueWarps = 4, kProducerWarp = 4, kMmaWarp = 5;
+constexpr int kProducerWarp = 4;
 constexpr int kHelperWarp0 = 6, kHelperWarps = 2, kHelperThreads = kHelperWarps * 32;   // table helpers
-constexpr int kTransformWarp0 = 8, kTransformWarps = 4;
+constexpr int kConsumerWarps = 8;       // warps 0-3 and 8-11
 constexpr int kDtpWarp0 = 12, kDtpWarps = 16, kDtpSets = 2, kDtpSetWarps = kDtpWarps / kDtpSets;
-constexpr int kDtpThreads = kDtpWarps * 32, kDtpSetThreads = kDtpSetWarps * 32;
+constexpr int kDtpSetThreads = kDtpSetWarps * 32;
 constexpr int kThreads = (kDtpWarp0 + kDtpWarps) * 32;            // 896
+constexpr int kMaxBN = 64;              // output columns per tile
 constexpr int kMaxPaths = 16;
 constexpr int kMaxTileEdges = 136;      // 128 / d3 + 2 <= 130
 constexpr int kMetaInts = 2 * kMaxTileEdges;   // int32 src / dst rows of the tile's edges
@@ -80,38 +76,36 @@ struct FArgs {
   const float* w;
   const float* w_offset;
   const float* cg;
+  float* C;              // [M, N] with row stride ldc
+  long long ldc;
   long long E, M;        // edges; GEMM rows = E * d3
   int d_y, W, w_shared, d3, n_paths, m_row, K, N;
   int n_tile, n_blocks;
   long long m_blocks;
-  int dbg_skip;          // measurement aid: bit 0 skips the DTP math, bit 1 the MMAs, bit 2 the transform (garbage results);
-                         // v4 switches (results unchanged): 8 try_wait with a suspend-time hint, 16 two-instruction tf32 rounding,
-                         // 32 dense vector-load k-tile producer, 64 entry-per-thread table build, 128 gathers before the handshake
+  int dbg_skip;          // measurement aid: bit 0 skips the DTP math, bit 1 the MMAs (garbage results); bit 3 (8) turns off
+                         // the suspend-time hint of the barrier waits (results unchanged)
   long long* dbg;        // optional clock64 timeline of CTA 0: dbg[role * 2048 + n] (eqf_fused_set_timeline)
   // shared-memory layout (bytes), fixed by the host: n_op operand slots (B hi | B lo | weight box) | n_raw raw A tiles |
-  // store staging | 2 x (M rows + harmonics + node rows) | descriptors | barriers
+  // 2 x (M rows + harmonics + node rows) | descriptors | barriers
   int n_op, n_raw, op_bytes, w_tile_off, w_box_rows, tab_bytes, m_buf_floats, y_buf_floats, cg_floats;
   unsigned char kt_path[kMaxKTiles];   // path of each 32-channel k-tile, in channel order
   FPath paths[kMaxPaths];
 };
 
-// timeline of CTA 0: role 0 TMA producer, 1 MMA issuer, 2 transform (warp 8), 3 epilogue (warp 0), 4 DTP set 0 (first
-// thread: tables ready, then k-tile start / end), 5 table helper (row block start / end)
+// timeline of CTA 0: role 0 TMA producer, 1 consumer warp 0 (k-tile start / end), 3 consumer warp 0 (tile stored), 4 DTP
+// set 0 (first thread: tables ready, then k-tile start / end), 5 table helper (row block start / end)
 __device__ __forceinline__ void stamp(const FArgs& a, int role, int& n) {
   if (a.dbg != nullptr && blockIdx.x == 0 && n < 2048) a.dbg[role * 2048 + n] = clock64();
   ++n;
 }
 
-template <int BN, bool STACK>
+
+template <int BN>
 struct FSmem {
-  static constexpr int kAccCols = STACK ? 2 * BN : BN;
   static constexpr int kABytes = BM * kRowBytes;                    // raw A tile written by the DTP warps
   static constexpr int kBBytes = BN * kRowBytes;
-  static constexpr int kStoreBytes = kEpilogueWarps * 2 * 32 * kStoreCols * 4;
   static constexpr int kBarBytes = 1024;
   static constexpr int kBudget = 227 * 1024 - 1024;
-  static constexpr int kStagesTmem = (512 - 2 * kAccCols) / (2 * BKT);
-  static_assert(kStagesTmem >= 2, "accumulators leave no room for the A ring");
 };
 
 __device__ __forceinline__ float4 ld4(const float* p) { return __ldg(reinterpret_cast<const float4*>(p)); }
@@ -230,137 +224,102 @@ __device__ __forceinline__ void dtp_ktile_d1(const FArgs& a, const FPath& p, int
   }
 }
 
-template <int BN, bool STACK, int D3>
+
+template <int BN, int D3>
 __global__ void __launch_bounds__(kThreads, 1)
 dtp_gemm_fwd_kernel(const __grid_constant__ CUtensorMap map_bhi, const __grid_constant__ CUtensorMap map_blo,
-                    const __grid_constant__ CUtensorMap map_c, const __grid_constant__ CUtensorMap map_w,
-                    const __grid_constant__ FArgs a) {
-  using S = FSmem<BN, STACK>;
-  constexpr int kTmemCols = 512;
-  constexpr int kAcc = S::kAccCols;
-  constexpr int kACol0 = 2 * kAcc;                       // first TMEM column of the A staging area
-  constexpr int kTS = S::kStagesTmem > kMaxStages ? kMaxStages : S::kStagesTmem;    // a_hi / a_lo slots in tensor memory
+                    const __grid_constant__ CUtensorMap map_w, const __grid_constant__ FArgs a) {
+  using S = FSmem<BN>;
   const int n_op = a.n_op, n_raw = a.n_raw;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* op_base = smem;                                            // [n_op] x (B hi | B lo | radial-weight box)
   uint8_t* raw_base = smem + (size_t)n_op * a.op_bytes;               // [n_raw] x raw A tile
-  uint8_t* store_base = raw_base + (size_t)n_raw * S::kABytes;
-  uint8_t* tab_base = store_base + S::kStoreBytes;           // two table buffers: [m_buf_floats] M rows, harmonics, src / dst rows
+  uint8_t* tab_base = raw_base + (size_t)n_raw * S::kABytes;          // two table buffers: [m_buf_floats] M rows, harmonics, src / dst rows
   int4* mdesc = reinterpret_cast<int4*>(tab_base + 2 * a.tab_bytes);      // per M-row entry: (cg offset, y offset, d2, -)
   float* cg_s = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(mdesc) + ((a.m_row * 16 + 127) & ~127));   // the group's CG blocks
   uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(cg_s) + ((a.cg_floats * 4 + 127) & ~127));
   uint64_t* op_full = bars;                        // [8] weight tiles and the radial-weight box landed (TMA)
   uint64_t* op_empty = bars + kMaxStages;          // [8] the MMAs that read the slot's weight tiles finished
   uint64_t* raw_ready = bars + 2 * kMaxStages;     // [8] raw A tile written by the DTP set
-  uint64_t* raw_free = bars + 3 * kMaxStages;      // [8] the transform warps hold the raw tile in registers
-  uint64_t* a_ready = bars + 4 * kMaxStages;       // [8] a_hi / a_lo in tensor memory
-  uint64_t* a_free = bars + 5 * kMaxStages;        // [8] the MMAs that read the tensor-memory slot finished
-  uint64_t* tmem_full = bars + 6 * kMaxStages;     // [2]
-  uint64_t* tmem_empty = tmem_full + 2;            // [2]
-  uint64_t* tab_ready = tmem_full + 4;             // [2] tables of a row block built (helper warps)
-  uint64_t* tab_free = tmem_full + 6;              // [2] the DTP warps finished the row block
-  uint32_t* tmem_base_slot = reinterpret_cast<uint32_t*>(tmem_full + 8);
+  uint64_t* raw_free = bars + 3 * kMaxStages;      // [8] the consumers hold the raw tile in registers
+  uint64_t* tab_ready = bars + 4 * kMaxStages;     // [2] tables of a row block built (helper warps)
+  uint64_t* tab_free = tab_ready + 2;              // [2] the DTP warps finished the row block
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int k_tiles = a.K / BKT;
-  constexpr int d3 = D3;        // compile-time output degree: one kernel per degree (the all-degrees build was 142 KB of code)
+  constexpr int d3 = D3;        // compile-time output degree: one kernel per degree
   const long long n_tiles_total = a.m_blocks * a.n_blocks;
   const bool w_tma = !a.w_shared;
   const bool hint = (a.dbg_skip & 8) == 0;         // try_wait with the long suspend-time hint (bit 3 turns it off: A/B)
   auto wait = [hint](uint64_t* bar, uint32_t parity) { if (hint) mbar_wait_hint(bar, parity); else mbar_wait(bar, parity); };
 
-  if (warp == kProducerWarp && lane == 0) {
-    prefetch_map(&map_bhi); prefetch_map(&map_blo); prefetch_map(&map_c);
+  if (threadIdx.x == kProducerWarp * 32) {
+    prefetch_map(&map_bhi); prefetch_map(&map_blo);
     if (w_tma) prefetch_map(&map_w);
     for (int s = 0; s < kMaxStages; ++s) {
       mbar_init(&op_full[s], 1);
-      mbar_init(&op_empty[s], 1);
+      mbar_init(&op_empty[s], kConsumerWarps);
       mbar_init(&raw_ready[s], kDtpSetWarps);
-      mbar_init(&raw_free[s], kTransformWarps);
-      mbar_init(&a_ready[s], kTransformWarps);
-      mbar_init(&a_free[s], 1);
+      mbar_init(&raw_free[s], kConsumerWarps);
     }
     for (int b = 0; b < 2; ++b) {
-      mbar_init(&tmem_full[b], 1);
-      mbar_init(&tmem_empty[b], kEpilogueWarps);
       mbar_init(&tab_ready[b], kHelperWarps);
       mbar_init(&tab_free[b], kDtpWarps);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == kMmaWarp) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_base_slot)), "n"(kTmemCols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_base_slot;
 
-  if (warp < kEpilogueWarps) {
-    // ===================================================================================== epilogue (warpgroup 0)
-    uint32_t acc_it = 0, chunk_it = 0;
+  if (warp < 4 || (warp >= 8 && warp < kDtpWarp0)) {
+    // ===================================================================================== consumers (warpgroups 0, 2)
+    reg_alloc<80>();
+    const int row_wg = (warp < 4 ? 0 : 64) + (warp & 3) * 16;     // first of this warp's 16 rows inside the tile
+    const bool stamper = threadIdx.x == 0;
+    Ring op(n_op), raw(n_raw);
     int n_stamp = 0;
-    for (long long tile = blockIdx.x; tile < n_tiles_total; tile += gridDim.x, ++acc_it) {
+    for (long long tile = blockIdx.x; tile < n_tiles_total; tile += gridDim.x) {
       const long long mb = tile / a.n_blocks;
       const int nb = (int)(tile % a.n_blocks);
-      const int ab = acc_it & 1;
-      const uint32_t aph = (acc_it >> 1) & 1;
-      wait(&tmem_full[ab], aph);
-      if (threadIdx.x == 0) stamp(a, 3, n_stamp);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)(ab * kAcc);
-      const long long row0 = mb * BM + warp * 32;
-      const int col0 = nb * a.n_tile;
-      uint8_t* wbuf = store_base + warp * (2 * 32 * kStoreCols * 4);
-      const int n_valid = (a.N - col0) < a.n_tile ? (a.N - col0) : a.n_tile;
-      for (int c = 0; c < n_valid; c += kStoreCols, ++chunk_it) {
-        const uint32_t buf = smem_u32(wbuf + (chunk_it & 1) * (32 * kStoreCols * 4));
-        uint32_t v[32];
-        tmem_ld32(taddr + (uint32_t)c, v);
-        if constexpr (STACK) {       // add the hi*lo half of the stacked accumulator, 16 columns at a time
+      float acc[BN / 2];
 #pragma unroll
-          for (int hh = 0; hh < 2; ++hh) {
-            uint32_t v2[16];
-            tmem_ld16(taddr + (uint32_t)(BN + c + 16 * hh), v2);
-            tmem_wait_ld();
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      for (int kt = 0; kt < k_tiles; ++kt, op.next(), raw.next()) {
+        wait(&op_full[op.idx], op.ph);
+        wait(&raw_ready[raw.idx], raw.ph);
+        if (stamper) stamp(a, 1, n_stamp);
+        // the k-tile in two halves of two 8-deep k-steps: the accumulator and one half's split fragments fit the
+        // 72-register launch budget of the 896-thread CTA, so ptxas keeps the MMAs of a half asynchronous
+        const uint32_t raw_tile = smem_u32(raw_base + (size_t)raw.idx * S::kABytes);
+        const uint32_t st = smem_u32(op_base + (size_t)op.idx * a.op_bytes);
 #pragma unroll
-            for (int j = 0; j < 16; ++j) v[16 * hh + j] = __float_as_uint(__uint_as_float(v[16 * hh + j]) + __uint_as_float(v2[j]));
+        for (int half = 0; half < 2; ++half) {
+          uint32_t hi[8], lo[8];
+          load_a_split(raw_tile, row_wg, lane, hi, lo, 2 * half);
+          if (half == 1) {         // the raw tile is read: hand the slot back to the DTP warps before the last MMAs
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&raw_free[raw.idx]);
           }
-        } else {
-          tmem_wait_ld();
+          if (!(a.dbg_skip & 2)) {
+            mma_ktile_3xtf32<BN>(acc, hi, lo, st, st + S::kBBytes, 2 * half);
+            wgmma_wait<0>();
+          }
         }
-        // the buffer about to be overwritten was handed to a TMA store two chunks ago: wait until that store has read it
-        if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
         __syncwarp();
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const uint32_t dst = buf + (uint32_t)lane * 128u + (uint32_t)((j ^ (lane & 7)) << 4);
-          sts128(dst, make_float4(__uint_as_float(v[4 * j]), __uint_as_float(v[4 * j + 1]), __uint_as_float(v[4 * j + 2]),
-                                  __uint_as_float(v[4 * j + 3])));
-        }
-        fence_async_smem();
-        __syncwarp();
-        if (lane == 0 && row0 < a.M) {
-          tma_store_2d(&map_c, col0 + c, (int)row0, buf);
-          asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-        }
+        if (lane == 0) mbar_arrive(&op_empty[op.idx]);
+        if (stamper) stamp(a, 1, n_stamp);
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty[ab]);
-      if (threadIdx.x == 0) stamp(a, 3, n_stamp);
+      store_acc<BN>(acc, a.C, a.ldc, mb * BM + row_wg, a.M, nb * BN, a.N, lane, false);
+      if (stamper) stamp(a, 3, n_stamp);
     }
-    if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-  } else if (warp < kTransformWarp0) {
-    // ===================================================================================== warpgroup 1: TMA, MMA, table helpers
+  } else if (warp < 8) {
+    // ===================================================================================== warpgroup 1: TMA, table helpers
     reg_dealloc<56>();
     if (warp == kProducerWarp) {
       if (lane == 0) {
         Ring op(n_op);
         int n_stamp = 0;
-        const uint32_t tx = (uint32_t)(2 * a.n_tile * kRowBytes) + (w_tma ? (uint32_t)(a.w_box_rows * kRowBytes) : 0u);
+        const uint32_t tx = (uint32_t)(2 * S::kBBytes) + (w_tma ? (uint32_t)(a.w_box_rows * kRowBytes) : 0u);
         for (long long tile = blockIdx.x; tile < n_tiles_total; tile += gridDim.x) {
           const long long mb = tile / a.n_blocks;
           const int nb = (int)(tile % a.n_blocks);
@@ -370,8 +329,8 @@ dtp_gemm_fwd_kernel(const __grid_constant__ CUtensorMap map_bhi, const __grid_co
             stamp(a, 0, n_stamp);
             uint8_t* st = op_base + (size_t)op.idx * a.op_bytes;
             mbar_expect_tx(&op_full[op.idx], tx);
-            tma_load_2d(st, &map_bhi, kt * BKT, nb * a.n_tile, &op_full[op.idx]);
-            tma_load_2d(st + S::kBBytes, &map_blo, kt * BKT, nb * a.n_tile, &op_full[op.idx]);
+            tma_load_2d(st, &map_bhi, kt * BKT, nb * BN, &op_full[op.idx]);
+            tma_load_2d(st + S::kBBytes, &map_blo, kt * BKT, nb * BN, &op_full[op.idx]);
             if (w_tma) {
               const FPath& p = a.paths[a.kt_path[kt]];
               tma_load_2d(st + a.w_tile_off, &map_w, p.w_off + (kt * BKT - p.koff), e0, &op_full[op.idx]);
@@ -379,50 +338,7 @@ dtp_gemm_fwd_kernel(const __grid_constant__ CUtensorMap map_bhi, const __grid_co
           }
         }
       }
-    } else if (warp == kMmaWarp) {
-      if (lane == 0) {
-        const uint32_t idesc = instr_desc(a.n_tile);
-        const uint32_t idesc2 = instr_desc(2 * a.n_tile);          // STACK: [b_hi | b_lo] as one operand
-        Ring op(n_op), ts(kTS);
-        uint32_t acc_it = 0;
-        int n_stamp = 0;
-        for (long long tile = blockIdx.x; tile < n_tiles_total; tile += gridDim.x, ++acc_it) {
-          const int ab = acc_it & 1;
-          const uint32_t aph = (acc_it >> 1) & 1;
-          wait(&tmem_empty[ab], aph ^ 1);
-          tc_fence_after();
-          const uint32_t d_tmem = tmem_base + (uint32_t)(ab * kAcc);
-          for (int kt = 0; kt < k_tiles; ++kt, op.next(), ts.next()) {
-            wait(&op_full[op.idx], op.ph);
-            stamp(a, 1, n_stamp);
-            wait(&a_ready[ts.idx], ts.ph);
-            stamp(a, 1, n_stamp);
-            tc_fence_after();
-            const uint32_t st = smem_u32(op_base + (size_t)op.idx * a.op_bytes);
-            const uint64_t b_hi = smem_desc_sw128(st), b_lo = smem_desc_sw128(st + S::kBBytes);
-            const uint32_t a_hi = tmem_base + (uint32_t)(kACol0 + ts.idx * 2 * BKT), a_lo = a_hi + BKT;
-#pragma unroll
-            for (int kb = 0; kb < BKT / UMMA_K; ++kb) {
-              if (a.dbg_skip & 2) break;
-              const uint64_t adv = (uint64_t)((kb * UMMA_K * 4) >> 4);
-              const uint32_t acol = (uint32_t)(kb * UMMA_K);
-              if constexpr (STACK) {
-                umma_tf32_ts(d_tmem, a_hi + acol, b_hi + adv, idesc2, (kt > 0 || kb > 0) ? 1u : 0u);   // hi*hi | hi*lo
-                umma_tf32_ts(d_tmem, a_lo + acol, b_hi + adv, idesc, 1u);                               // + lo*hi
-              } else {
-                umma_tf32_ts(d_tmem, a_lo + acol, b_hi + adv, idesc, (kt > 0 || kb > 0) ? 1u : 0u);
-                umma_tf32_ts(d_tmem, a_hi + acol, b_lo + adv, idesc, 1u);
-                umma_tf32_ts(d_tmem, a_hi + acol, b_hi + adv, idesc, 1u);
-              }
-            }
-            umma_commit(&op_empty[op.idx]);
-            umma_commit(&a_free[ts.idx]);
-            stamp(a, 1, n_stamp);
-          }
-          umma_commit(&tmem_full[ab]);
-        }
-      }
-    } else {
+    } else if (warp >= kHelperWarp0) {
       // ------------------------------------------------------------------------------------- table helpers (warps 6, 7)
       // One row block AHEAD of the DTP warps: the block's edges (src / dst rows, harmonics) into shared memory, then the
       // coupling blocks M_p[e] = CG_p . y_e, one thread per entry q of the edge's M row (its CG column in registers)
@@ -496,52 +412,6 @@ dtp_gemm_fwd_kernel(const __grid_constant__ CUtensorMap map_bhi, const __grid_co
         if (ht == 0) stamp(a, 5, n_stamp);
       }
     }
-  } else if (warp < kDtpWarp0) {
-    // ===================================================================================== transform (warpgroup 2)
-    reg_alloc<88>();
-    const int row = (warp & 3) * 32 + lane;
-    const uint32_t lane_field = (uint32_t)((warp & 3) * 32) << 16;
-    Ring raw(n_raw), ts(kTS);
-    int n_stamp = 0;
-    const bool stamper = warp == kTransformWarp0 && lane == 0;
-    for (long long tile = blockIdx.x; tile < n_tiles_total; tile += gridDim.x) {
-      for (int kt = 0; kt < k_tiles; ++kt, raw.next(), ts.next()) {
-        wait(&raw_ready[raw.idx], raw.ph);
-        if (stamper) stamp(a, 2, n_stamp);
-        float hi[BKT], lo[BKT];
-        {
-          const uint32_t rbase = smem_u32(raw_base + (size_t)raw.idx * S::kABytes) + (uint32_t)row * (uint32_t)kRowBytes;
-          float4 v[8];
-#pragma unroll
-          for (int c = 0; c < 8; ++c) v[c] = lds128(rbase + (uint32_t)((c ^ (row & 7)) << 4));
-#pragma unroll
-          for (int c = 0; c < 8; ++c) { hi[4 * c] = v[c].x; hi[4 * c + 1] = v[c].y; hi[4 * c + 2] = v[c].z; hi[4 * c + 3] = v[c].w; }
-        }
-        // the raw tile is in registers: hand the slot back to the DTP warps before the conversion (the arrive's release
-        // orders the loads above before it; __syncwarp extends that to the other lanes)
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&raw_free[raw.idx]);
-        wait(&a_free[ts.idx], ts.ph ^ 1);
-        tc_fence_after();
-        if (!(a.dbg_skip & 4)) {
-          if (!(a.dbg_skip & 16)) {
-#pragma unroll
-            for (int j = 0; j < BKT; ++j) { const float xv = hi[j]; hi[j] = tf32_rn_fast(xv); lo[j] = xv - hi[j]; }
-          } else {
-#pragma unroll
-            for (int j = 0; j < BKT; ++j) { const float xv = hi[j]; hi[j] = tf32_rn(xv); lo[j] = xv - hi[j]; }
-          }
-          const uint32_t acol = tmem_base + lane_field + (uint32_t)(kACol0 + ts.idx * 2 * BKT);
-          tmem_st32(acol, hi);
-          tmem_st32(acol + BKT, lo);
-          tmem_wait_st();
-        }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&a_ready[ts.idx]);
-        if (stamper) stamp(a, 2, n_stamp);
-      }
-    }
   } else {
     // ===================================================================================== DTP producers (warpgroups 3-6)
     const int dt = threadIdx.x - kDtpWarp0 * 32;          // 0 .. 511
@@ -585,18 +455,12 @@ dtp_gemm_fwd_kernel(const __grid_constant__ CUtensorMap map_bhi, const __grid_co
       if (lane == 0) mbar_arrive(&tab_free[b]);           // this warp no longer reads the row block's tables
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == kMmaWarp) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(kTmemCols) : "memory");
-  }
 }
 
 // ---------------------------------------------------------------------------------------------- one group to HBM
 // The same producer for an output group whose linear is too WIDE to fuse (N > 128 columns: every column tile would
 // recompute the product): write f_g[e, k, :K] to HBM (the 0e group of the QM9 model is 224 of the 3136 floats per edge) and
-// let the wide tcgen05 GEMM read it.  One CTA = 32 edges: coupling blocks of its edges in shared memory, then the
+// let the wide wgmma GEMM read it.  One CTA = 32 edges: coupling blocks of its edges in shared memory, then the
 // group's k-tiles with the thread layout of dtp_ktile (8 lanes x float4 per edge).
 template <int D1, int D3>
 __device__ __forceinline__ void group_ktile(const FArgs& a, const FPath& p, int ch0, int el, int c8, long long e,
@@ -676,19 +540,16 @@ __global__ void split_transpose_kernel(const float* __restrict__ w, long long ld
     const float v = w[k * ldw + n];
     const float h = tf32_rn(v);
     hi[i] = h;
-    lo[i] = v - h;
+    lo[i] = tf32_rn(v - h);
   }
 }
 
-template <int BN, bool STACK, int D3>
-static int launch_fwd_d3(const CUtensorMap& mh, const CUtensorMap& ml, const CUtensorMap& mc, const CUtensorMap& mw, FArgs& a,
-                      cudaStream_t s) {
-  using S = FSmem<BN, STACK>;
-  // shared-memory layout: operand slots (B hi | B lo | radial-weight box) | raw A tiles | store staging | 2 table buffers |
-  // descriptors | barriers.  The rings are independent: an operand slot is held from its TMA to the MMAs that read the
-  // weight tiles, a raw tile only from the DTP warps' stores to the transform warps' loads, a tensor-memory A slot from
-  // the transform's stores to the MMAs (v3 tied all three to ONE 5-deep ring whose round trip - TMA from HBM, producer,
-  // transform, MMA - was ~7 k cycles: 1.4 k cycles per k-tile before any arithmetic).
+template <int BN, int D3>
+static int launch_fwd_d3(const CUtensorMap& mh, const CUtensorMap& ml, const CUtensorMap& mw, FArgs& a, cudaStream_t s) {
+  using S = FSmem<BN>;
+  // shared-memory layout: operand slots (B hi | B lo | radial-weight box) | raw A tiles | 2 table buffers | descriptors |
+  // barriers.  The rings are independent: an operand slot is held from its TMA to the MMAs that read the weight tiles,
+  // a raw tile only from the DTP warps' stores to the consumers' fragment loads.
   const int n_e_max = BM / a.d3 + 2;
   a.w_box_rows = a.w_shared ? 0 : n_e_max;
   a.w_tile_off = 2 * S::kBBytes;
@@ -698,7 +559,7 @@ static int launch_fwd_d3(const CUtensorMap& mh, const CUtensorMap& ml, const CUt
   a.cg_floats = 0;
   for (int i = 0; i < a.n_paths; ++i) a.cg_floats += a.paths[i].d1 * a.paths[i].d2 * a.d3;
   a.tab_bytes = ((a.m_buf_floats + a.y_buf_floats) * 4 + kMetaInts * 4 + 127) & ~127;
-  const int fixed = S::kStoreBytes + 2 * a.tab_bytes + ((a.m_row * 16 + 127) & ~127) + ((a.cg_floats * 4 + 127) & ~127) + S::kBarBytes;
+  const int fixed = 2 * a.tab_bytes + ((a.m_row * 16 + 127) & ~127) + ((a.cg_floats * 4 + 127) & ~127) + S::kBarBytes;
   int n_raw = 0, n_op = 0;
   for (int r = 4; r >= 2 && n_raw == 0; --r) {             // prefer 4 raw tiles (two per DTP set) if >= r operand slots remain
     const int o = (S::kBudget - fixed - r * S::kABytes) / a.op_bytes;
@@ -713,7 +574,7 @@ static int launch_fwd_d3(const CUtensorMap& mh, const CUtensorMap& ml, const CUt
   {
     std::lock_guard<std::mutex> lock(mtx);
     if (total > attr_bytes) {
-      cudaError_t e = cudaFuncSetAttribute(dtp_gemm_fwd_kernel<BN, STACK, D3>, cudaFuncAttributeMaxDynamicSharedMemorySize, total);
+      cudaError_t e = cudaFuncSetAttribute(dtp_gemm_fwd_kernel<BN, D3>, cudaFuncAttributeMaxDynamicSharedMemorySize, total);
       if (e != cudaSuccess) return check_cuda(e, "dtp_gemm_fwd smem attribute");
       attr_bytes = total;
     }
@@ -721,18 +582,17 @@ static int launch_fwd_d3(const CUtensorMap& mh, const CUtensorMap& ml, const CUt
   const int sms = device_sms();
   const long long tiles = a.m_blocks * a.n_blocks;
   const int grid = (int)(tiles < sms ? tiles : sms);
-  dtp_gemm_fwd_kernel<BN, STACK, D3><<<grid, kThreads, total, s>>>(mh, ml, mc, mw, a);
+  dtp_gemm_fwd_kernel<BN, D3><<<grid, kThreads, total, s>>>(mh, ml, mw, a);
   return check_cuda(cudaGetLastError(), "dtp_gemm_fwd_kernel launch");
 }
 
-template <int BN, bool STACK>
-static int launch_fwd(const CUtensorMap& mh, const CUtensorMap& ml, const CUtensorMap& mc, const CUtensorMap& mw, FArgs& a,
-                      cudaStream_t s) {
+template <int BN>
+static int launch_fwd(const CUtensorMap& mh, const CUtensorMap& ml, const CUtensorMap& mw, FArgs& a, cudaStream_t s) {
   switch (a.d3) {
-    case 1: return launch_fwd_d3<BN, STACK, 1>(mh, ml, mc, mw, a, s);
-    case 3: return launch_fwd_d3<BN, STACK, 3>(mh, ml, mc, mw, a, s);
-    case 5: return launch_fwd_d3<BN, STACK, 5>(mh, ml, mc, mw, a, s);
-    default: return launch_fwd_d3<BN, STACK, 7>(mh, ml, mc, mw, a, s);
+    case 1: return launch_fwd_d3<BN, 1>(mh, ml, mw, a, s);
+    case 3: return launch_fwd_d3<BN, 3>(mh, ml, mw, a, s);
+    case 5: return launch_fwd_d3<BN, 5>(mh, ml, mw, a, s);
+    default: return launch_fwd_d3<BN, 7>(mh, ml, mw, a, s);
   }
 }
 
@@ -829,6 +689,7 @@ static int fill_fargs(const EqfPlan* plan, const EqfEdgeOperands* op, int64_t n_
   a.y = op->y; a.w = op->w; a.w_offset = op->w_offset; a.w_shared = op->w_shared;
   if (a.w_shared && a.w_offset != nullptr) { set_error(std::string(who) + ": w_offset needs per-edge weights"); return EQF_ERR_INVALID; }
   a.cg = reinterpret_cast<const float*>(plan->d_blob + h.off_cg);
+  a.C = nullptr; a.ldc = 0;
   a.E = n_edges; a.M = n_edges * a.d3; a.d_y = h.d_y; a.W = h.w_numel; a.N = 0;
   if (a.M > 0x7fffffffLL) { set_error(std::string(who) + ": too many rows"); return EQF_ERR_UNSUPPORTED; }
   a.n_tile = a.n_blocks = 0; a.m_blocks = 0;
@@ -888,26 +749,22 @@ extern "C" int eqf_dtp_linear_fwd(const EqfPlan* plan, const EqfEdgeOperands* op
   float* lo = split + N * K;
   {
     const long long n = N * K;
-    const unsigned blocks = (unsigned)((n + 255) / 256 < 1184 ? (n + 255) / 256 : 1184);
+    const unsigned blocks = (unsigned)((n + 255) / 256 < 1056 ? (n + 255) / 256 : 1056);
     split_transpose_kernel<<<blocks, 256, 0, s>>>(Wt, ldw, hi, lo, N, K);
   }
   if ((rc = check_cuda(cudaGetLastError(), "split_transpose_kernel launch")) != EQF_OK) return rc;
-  // column tiles: stacked [b_hi | b_lo] operand for outputs of exactly 32 / 64 columns, else tiles of <= 128 columns
-  const bool stack = (N == 32 || N == 64);
-  const int n_blocks = (int)((N + 127) / 128);
-  const int n_tile = n_blocks == 1 ? (int)((N + 15) & ~15LL) : 128;
+  // column tiles of at most 64 (the consumers' accumulators live in registers): every tile recomputes the product
+  const int n_blocks = (int)((N + kMaxBN - 1) / kMaxBN);
+  const int n_tile = (n_blocks == 1 && N <= 32) ? 32 : kMaxBN;
   a.n_tile = n_tile; a.n_blocks = n_blocks; a.m_blocks = (a.M + BM - 1) / BM;
-  CUtensorMap mh, ml, mc, mw;
+  a.C = C; a.ldc = ldc;
+  CUtensorMap mh, ml, mw;
   if ((rc = make_map_2d(&mh, hi, N, K, K, n_tile, BKT)) != EQF_OK) return rc;
   if ((rc = make_map_2d(&ml, lo, N, K, K, n_tile, BKT)) != EQF_OK) return rc;
-  if ((rc = make_map_2d(&mc, C, a.M, N, ldc, 32, kStoreCols)) != EQF_OK) return rc;
-  mw = mc;    // placeholder when the weights are shared (never dereferenced)
+  mw = mh;    // placeholder when the weights are shared (never dereferenced)
   // per-edge radial weights: [E, W] row-major, a box of (128 / d3 + 2) edges x 32 channels per k-tile, rows back to back
   if (!a.w_shared && (rc = make_map_2d(&mw, a.w, n_edges, h.w_numel, h.w_numel, BM / a.d3 + 2, BKT, MapKind::kLinear)) != EQF_OK)
     return rc;
-  if (stack && n_tile == 32) return launch_fwd<32, true>(mh, ml, mc, mw, a, s);
-  if (stack && n_tile == 64) return launch_fwd<64, true>(mh, ml, mc, mw, a, s);
-  if (n_tile <= 32) return launch_fwd<32, false>(mh, ml, mc, mw, a, s);
-  if (n_tile <= 64) return launch_fwd<64, false>(mh, ml, mc, mw, a, s);
-  return launch_fwd<128, false>(mh, ml, mc, mw, a, s);
+  if (n_tile == 32) return launch_fwd<32>(mh, ml, mw, a, s);
+  return launch_fwd<64>(mh, ml, mw, a, s);
 }

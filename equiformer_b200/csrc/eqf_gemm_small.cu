@@ -1,10 +1,9 @@
-// eqf_gemm_small.cu - grouped fp32 GEMM for the SMALL products of the path (sm_100a, CUDA cores, exact fp32 FMA).
+// eqf_gemm_small.cu - grouped fp32 GEMM for the SMALL products of the path (sm_90a, CUDA cores, exact fp32 FMA).
 //
 // Node-level linears (nets/graph_attention_transformer.py:430-431 merge_src / merge_dst, :515 proj, the FeedForwardNetwork's
 // two FCTPs, nets/tensor_product_rescale.py LinearRS) are one [atoms * (2l+1), mul_in] x [mul_in, mul_out] product per degree:
-// 2 324 atoms x {1, 3, 5} rows against 128 / 64 / 32 channels - 30 to 80 MFLOP each.  Round 1 handed every one of them to
-// cuBLAS (its SIMT SGEMM: ~180 launches of 5-8 us per step); the tcgen05 kernels need M >= 16 k rows to pay for their
-// prologue.  Here ONE launch carries all degrees of a linear (and, in the backward, the data gradients AND the weight
+// 2 324 atoms x {1, 3, 5} rows against 128 / 64 / 32 channels - 30 to 80 MFLOP each: one cuBLAS call per degree would
+// mean ~180 small launches per step, and the wgmma kernels need M >= 16 k rows to pay for their prologue.  Here ONE launch carries all degrees of a linear (and, in the backward, the data gradients AND the weight
 // gradients of all degrees): a table of up to EQF_GROUP_MAX problems
 //     C_i[M, N] (+)= alpha_i * sum_k A_i(m, k) B_i(k, n)
 // whose operands are addressed through (contiguous-along-k | contiguous-along-m/n) flags, so the same tile code serves
@@ -155,10 +154,9 @@ __global__ void __launch_bounds__(kThreadsG) grouped_gemm_kernel(const __grid_co
 // ---------------------------------------------------------------------------------------------- warp-MMA variant
 // The same tiles on the tensor cores' warp-level path (mma.sync m16n8k8, tf32 inputs, fp32 accumulate) with the 3xTF32
 // split done in registers: a = a_hi + a_lo, b = b_hi + b_lo, acc += a_lo b_hi + a_hi b_lo + a_hi b_hi (the error of the
-// dropped a_lo b_lo term is ~2^-22 relative, like the tcgen05 kernels of eqf_gemm_tf32x3.cu).  The CUDA-core kernel
-// above is bound by FMA issue (a 64 x 64 x 128 tile is 16 k warp-FMAs: 2.2 us alone on an SM); here a k-step of 8 costs a
+// dropped a_lo b_lo term is ~2^-22 relative, like the wgmma kernels of eqf_gemm_tf32x3.cu).  The CUDA-core kernel
+// above is bound by FMA issue (a 64 x 64 x 128 tile is 16 k warp-FMAs); here a k-step of 8 costs a
 // warp 24 MMAs + 16 shared loads + 48 split instructions for its 32 x 32 sub-tile instead of 256 FMAs + 32 loads.
-// tcgen05 is not worth its prologue at this size (measured: 8.7 us vs 5.5 us for cuBLAS on 2 324 x 128 x 128).
 // 128 threads = 4 warps (2 x 2) per 64 x 64 tile; operands in shared memory in whichever orientation makes the global
 // load a 128-bit access AND the fragment loads conflict-free: k-contiguous operands as [row][16 + 4], the others as
 // [k][64 + 8].
@@ -215,8 +213,7 @@ __device__ __forceinline__ void mma_tile(const Prob& p, int tm, int tn, int spli
     for (int j = 0; j < 4; ++j)
 #pragma unroll
       for (int c = 0; c < 4; ++c) acc[i][j][c] = 0.f;
-  // kMmaStages-deep cp.async ring: with one chunk of register prefetch every 16-deep chunk cost a full L2 round trip (8.8 us
-  // for the 157 MFLOP forward of a node-level linear, of which ~6 us were eight exposed load latencies)
+  // kMmaStages-deep cp.async ring: with one chunk of register prefetch every 16-deep chunk costs a full L2 round trip
   const int n_chunks = (k_end - k_begin + BK - 1) / BK;
 #pragma unroll
   for (int s = 0; s < kMmaStages - 1; ++s) {
@@ -328,7 +325,7 @@ extern "C" int eqf_gemm_grouped(const EqfGemmProblem* problems, int32_t n, void*
   Args g;
   g.n = 0;
   int tiles = 0;
-  int sms = 148, dev = 0;
+  int sms = 132, dev = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   for (int i = 0; i < n; ++i) {

@@ -1,26 +1,19 @@
-// eqf_gemm_tf32x3.cu - hand-written tcgen05 GEMM for the per-degree channel-mixing linears (sm_100a).
+// eqf_gemm_tf32x3.cu - hand-written warpgroup-MMA (wgmma) GEMMs for the per-degree channel-mixing linears (sm_90a).
 //
-//   C[M, N] = A[M, K] * Bt[N, K]^T        fp32 in HBM, fp32-level accuracy, M = edges x (2l+1) rows (tall), K, N <= ~1000
+//   forward / data gradient   C[M, N] = A[M, K] * Bt[N, K]^T        M = edges x (2l+1) rows (tall), K, N <= ~1000
+//   weight gradient           W[K1, N] = A[R, K1]^T G[R, N]         reduction over the R rows, tiny output
 //
-// The linears after each depth-wise tensor product (LinearRS, nets/tensor_product_rescale.py:165-174; in the reference
-// an e3nn 'uvw' einsum -> cuBLAS SGEMM) are skinny: tens of thousands of rows, K and N of a few hundred.  The CUTLASS
-// 9xBF16 collective (eqf_gemm.cu) keeps the tensor pipe 33 % busy on them: every value is split three ways by a
-// transform warp-group and the TMEM accumulator is promoted to registers every other k-block.  This kernel uses the
-// 3xTF32 scheme instead:
-//   a = a_hi + a_lo,  a_hi = a rounded to nearest tf32 (19 bits), a_lo = a - a_hi (exact),
-//   a*b ~= a_lo*b_hi + a_hi*b_lo + a_hi*b_hi          (the dropped a_lo*b_lo term is 2^-24 relative)
-// The transform warps rewrite the TMA-written A tile in place with a_hi and write a_lo next to it (masking the raw
-// bits instead - what the MMA does to a raw fp32 operand - is biased and cost 10x in accuracy at K ~ 1000); the
-// weights' hi / lo planes are split once per call by a tiny kernel; all three products accumulate in one TMEM
-// accumulator over the whole K loop - no promotion.
+// fp32 in HBM, fp32-level accuracy through the 3xTF32 split of eqf_tc.cuh (the weights' hi / lo planes are split once per
+// call by a tiny kernel; the A operand is split in registers and fed to wgmma as its register fragment).
 //
-// One CTA per SM, persistent over 128 x BN output tiles, warp-specialised:
-//   warps 0-3  epilogue   (tcgen05.ld TMEM -> registers -> st.global; warp w owns TMEM lanes 32w..32w+31)
-//   warp  4    TMA producer (one lane): A raw tile, B hi tile, B lo tile per 32-wide k-tile (128-byte rows, SWIZZLE_128B)
-//   warp  5    MMA issuer (one lane): 4 k-blocks x 3 tcgen05.mma.kind::tf32 per k-tile; owns the TMEM allocation
-//   warps 6-9  transform: A_lo tile from the A raw tile (in shared memory, same swizzled positions)
-// Pipelines: smem ring (full / lo_ready / empty mbarriers) and a double-buffered TMEM accumulator (tmem_full / tmem_empty),
-// so the epilogue of tile i overlaps the main loop of tile i+1.
+// Forward: one CTA per 128 x BN output tile, three warpgroups:
+//   warpgroup 0      TMA producer (one thread): A tile [128 x 32] and the B hi / lo tiles [BN x 32] of each k-tile
+//                    (128-byte rows, SWIZZLE_128B) into a ring of shared-memory stages (full / empty mbarriers)
+//   warpgroups 1, 2  consumers, 64 rows each: A fragments from shared memory -> hi / lo in registers -> 3 wgmma per
+//                    8-deep k-step and 64-column chunk into a k-tile accumulator, added to the running sum in registers
+// Weight gradient: the same roles over the CTA's slice of the R rows.  Both operands are "MN-major" (the reduction runs
+// along the strided dimension), which tf32 wgmma cannot read from shared memory: A^T is read as register fragments
+// straight from its swizzled TMA boxes, and the consumers transpose + split each G tile into K-major hi / lo tiles first.
 #include <cuda.h>
 #include <cuda_runtime.h>
 
@@ -30,956 +23,105 @@
 #include <string>
 
 #include "eqf_common.cuh"
+#include "eqf_tc.cuh"
 
 namespace eqf {
 namespace tf32x3 {
 
-#ifndef EQF_TF32X3_BK
-#define EQF_TF32X3_BK 16
-#endif
-constexpr int BM = 128;              // rows per tile (UMMA M)
-constexpr int BK = EQF_TF32X3_BK;    // fp32 per k-tile row: 32 -> 128-byte rows (SWIZZLE_128B), 16 -> 64-byte rows (SWIZZLE_64B)
+using namespace tc;
+
+constexpr int BM = 128;                   // output rows per CTA: two consumer warpgroups of 64
+constexpr int BK = kKTile;                // reduction depth per stage (128-byte rows)
 constexpr int kRowBytes = BK * 4;
-constexpr int UMMA_K = 8;            // tf32 MMA depth
-constexpr int kStoreCols = 32;       // epilogue chunk: 32 columns = 128-byte rows in the staging buffers (SWIZZLE_128B)
-static_assert(BK == 16 || BK == 32, "BK must be 16 or 32");
-constexpr int kThreads = 320;
-constexpr int kEpilogueWarps = 4, kProducerWarp = 4, kMmaWarp = 5, kTransformWarp0 = 6, kTransformWarps = 4;
-constexpr int kTransformThreads = kTransformWarps * 32;
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t done;
-  do {
-    asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                 : "=r"(done) : "r"(smem_u32(bar)), "r"(parity) : "memory");
-  } while (!done);
-}
-// the same wait with the suspend-time hint CUTLASS passes: the warp sleeps in hardware until the phase completes instead
-// of returning after the short default limit and being re-issued (one polling lane per warp + __syncwarp was measured
-// SLOWER than all lanes waiting: profiles/r2_v4_ab_*.jsonl)
-__device__ __forceinline__ void mbar_wait_hint(uint64_t* bar, uint32_t parity) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "WAIT_%=:\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1, %2;\n\t"
-      "@p bra DONE_%=;\n\t"
-      "bra WAIT_%=;\n\t"
-      "DONE_%=:\n\t}"
-      ::"r"(smem_u32(bar)), "r"(parity), "r"(0x989680u) : "memory");
-}
-__device__ __forceinline__ void mbar_wait_x(uint64_t* bar, uint32_t parity, bool hinted) {
-  if (hinted) mbar_wait_hint(bar, parity); else mbar_wait(bar, parity);
-}
-__device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
-  asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
-               ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {   // arrives on `bar` once every MMA issued so far has finished
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// K-major operand tile in shared memory: rows of kRowBytes, 8-row groups 8*kRowBytes apart, swizzle span = row length
-// (cute UMMA::SmemDescriptor: start>>4 | LBO(=1)<<16 | SBO<<32 | version(=1)<<46 | layout<<61; SWIZZLE_128B = 2, _64B = 4)
-__device__ __forceinline__ uint64_t smem_desc(uint32_t addr) {
-  constexpr uint64_t sbo = (8 * kRowBytes) >> 4;
-  constexpr uint64_t layout = (BK == 32) ? 2 : 4;
-  return (uint64_t)((addr >> 4) & 0x3FFF) | (1ull << 16) | (sbo << 32) | (1ull << 46) | (layout << 61);
-}
-// kind::tf32, fp32 accumulate, K-major A and B, M = 128, N = n  (cute UMMA::InstrDescriptor)
-__device__ __forceinline__ uint32_t instr_desc(int n) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-}
-__device__ __forceinline__ void umma_tf32(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-
-// round to nearest tf32 (10-bit mantissa), low 13 bits zero: an unbiased split, unlike masking the raw bits
-__device__ __forceinline__ float tf32_rn(float x) {
-  uint32_t r;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
-  return __uint_as_float(r);
-}
-
-// the same rounding (nearest, ties away from zero) in two integer instructions: cvt.rna.tf32.f32 compiles to five on
-// sm_100a (it also keeps NaN payloads; here a NaN still reaches the product through lo = x - hi = NaN)
-__device__ __forceinline__ float tf32_rn_fast(float x) {
-  return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xffffe000u);
-}
-
-__device__ __forceinline__ float4 lds128(uint32_t addr) {
-  float4 v;
-  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
-  return v;
-}
-__device__ __forceinline__ void sts128(uint32_t addr, const float4& v) {
-  asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
-}
-
-// x -> (hi, lo): hi = x rounded to tf32 written back in place (the MMA truncates its fp32 operand, so it must be
-// handed the rounded value explicitly), lo = x - hi written `lo_offset` bytes further
-__device__ __forceinline__ void split_store(uint32_t addr, uint32_t lo_offset, const float4& v, bool fast = false) {
-  float4 h, r;
-  if (fast) { h.x = tf32_rn_fast(v.x); h.y = tf32_rn_fast(v.y); h.z = tf32_rn_fast(v.z); h.w = tf32_rn_fast(v.w); }
-  else { h.x = tf32_rn(v.x); h.y = tf32_rn(v.y); h.z = tf32_rn(v.z); h.w = tf32_rn(v.w); }
-  r.x = v.x - h.x; r.y = v.y - h.y; r.z = v.z - h.z; r.w = v.w - h.w;
-  sts128(addr, h);
-  sts128(addr + lo_offset, r);
-}
-
-__device__ __forceinline__ uint8_t* stage_base_of(uint8_t* smem, int s, int stage_bytes) { return smem + (size_t)s * stage_bytes; }
-
-struct Params {
-  float* C;
-  long long M, N, K, ldc;
-  int n_tile;        // columns per output tile (multiple of 16, <= BN)
-  int n_blocks;      // ceil(N / n_tile)
-  long long m_blocks;
-  long long* dbg;    // optional timeline of CTA 0 (clock64 stamps), see tools/tf32x3_timeline.py
-  int dbg_skip;      // measurement aid (EQF_TF32X3_DBG_SKIP): bit 0 skips the transform math, bit 1 the MMAs - results are
-                     // garbage then; what remains is the load / synchronisation skeleton.  Bit 3 (8) turns OFF the
-                     // suspend-time hint of the barrier waits, bit 4 (16) the two-instruction tf32 rounding (A/B switches of
-                     // tools/v4_ab.py; the results do not change)
-};
-
-// dbg layout: role r in {0 producer, 1 mma, 2 transform, 3 epilogue}: dbg[r * 1024 + n] = n-th stamp of that role
-__device__ __forceinline__ void stamp(const Params& p, int role, int& n) {
-  if (p.dbg != nullptr && blockIdx.x == 0 && n < 1024) p.dbg[role * 1024 + n] = clock64();
-  ++n;
-}
+constexpr int kThreads = 384;
+constexpr int kConsumerWarps = 8, kConsumerThreads = kConsumerWarps * 32;
+constexpr int kSmemBudget = 227 * 1024;
+constexpr int kMaxStages = 8;
 
 template <int BN>
 struct Smem {
   static constexpr int kABytes = BM * kRowBytes;
   static constexpr int kBBytes = BN * kRowBytes;
-  static constexpr int kStageBytes = 2 * kABytes + 2 * kBBytes;       // A hi | A lo | B hi | B lo
-  static constexpr int kStoreBytes = kEpilogueWarps * 2 * 32 * kStoreCols * 4;   // per warp: 2 buffers of 32 rows x 128 B
-  static constexpr int kBarrierBytes = 1024;
-  static constexpr int kBudget = 227 * 1024 - 1024 /* alignment slack */;
-  static constexpr int kStagesRaw = (kBudget - kStoreBytes - kBarrierBytes) / kStageBytes;
-  static constexpr int kStages = kStagesRaw > 8 ? 8 : kStagesRaw;
+  static constexpr int kStageBytes = kABytes + 2 * kBBytes;       // A raw | B hi | B lo
+  static constexpr int kStagesRaw = (kSmemBudget - 2048) / kStageBytes;
+  static constexpr int kStages = kStagesRaw > kMaxStages ? kMaxStages : kStagesRaw;
   static_assert(kStages >= 2, "tile does not fit shared memory");
-  static constexpr int kTotal = kStages * kStageBytes + kStoreBytes + kBarrierBytes + 1024;
+  static constexpr int kTotal = kStages * kStageBytes + 1024 /* barriers */ + 1024 /* alignment slack */;
+};
+
+struct Params {
+  float* C;
+  long long M, ldc;
+  int N, K;
 };
 
 template <int BN>
 __global__ void __launch_bounds__(kThreads, 1)
 gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_bhi,
-                   const __grid_constant__ CUtensorMap map_blo, const __grid_constant__ CUtensorMap map_c, Params p) {
+                   const __grid_constant__ CUtensorMap map_blo, Params p) {
   using S = Smem<BN>;
   constexpr int kStages = S::kStages;
-  constexpr int kTmemCols = (2 * BN <= 32) ? 32 : (2 * BN <= 64) ? 64 : (2 * BN <= 128) ? 128 : (2 * BN <= 256) ? 256 : 512;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* stage_base = smem;
-  uint8_t* store_base = smem + kStages * S::kStageBytes;     // epilogue staging (1024-byte aligned)
-  uint64_t* bars = reinterpret_cast<uint64_t*>(store_base + S::kStoreBytes);
-  uint64_t* full = bars;                       // [kStages] TMA landed
-  uint64_t* lo_ready = bars + kStages;         // [kStages] A_lo written
-  uint64_t* empty = bars + 2 * kStages;        // [kStages] MMAs reading the stage have finished
-  uint64_t* tmem_full = bars + 3 * kStages;    // [2]
-  uint64_t* tmem_empty = bars + 3 * kStages + 2;  // [2]
-  uint32_t* tmem_base_slot = reinterpret_cast<uint32_t*>(bars + 3 * kStages + 4);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + kStages * S::kStageBytes);
+  uint64_t* empty = full + kStages;
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const long long k_tiles = (p.K + BK - 1) / BK;
-  const long long n_tiles_total = p.m_blocks * p.n_blocks;
-
-  if (warp == kProducerWarp && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_a)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_bhi)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_blo)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_c)) : "memory");
-    for (int s = 0; s < kStages; ++s) {
-      mbar_init(&full[s], 1);
-      mbar_init(&lo_ready[s], kTransformWarps);
-      mbar_init(&empty[s], 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&tmem_full[a], 1);
-      mbar_init(&tmem_empty[a], kEpilogueWarps);
-    }
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2;
+  const long long m0 = (long long)blockIdx.x * BM;
+  const int n0 = blockIdx.y * BN;
+  const int k_tiles = (p.K + BK - 1) / BK;
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < kStages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], kConsumerWarps); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == kMmaWarp) {   // whole warp: TMEM allocation
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_base_slot)), "n"(kTmemCols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_base_slot;
 
-  if (warp == kProducerWarp) {
-    // ===================================================================================== TMA producer
-    if (lane == 0) {
-      uint32_t it = 0;
-      int n_stamp = 0;
-      const uint32_t tx = (uint32_t)(S::kABytes + 2 * p.n_tile * kRowBytes);
-      for (long long tile = blockIdx.x; tile < n_tiles_total; tile += gridDim.x) {
-        const long long mb = tile / p.n_blocks;
-        const int nb = (int)(tile % p.n_blocks);
-        for (long long kt = 0; kt < k_tiles; ++kt, ++it) {
-          const int s = it % kStages;
-          const uint32_t ph = (it / kStages) & 1;
-          mbar_wait_x(&empty[s], ph ^ 1, (p.dbg_skip & 8) == 0);
-          stamp(p, 0, n_stamp);
-          uint8_t* st = stage_base + (size_t)s * S::kStageBytes;
-          mbar_expect_tx(&full[s], tx);
-          tma_load_2d(st, &map_a, (int)(kt * BK), (int)(mb * BM), &full[s]);
-          tma_load_2d(st + 2 * S::kABytes, &map_bhi, (int)(kt * BK), nb * p.n_tile, &full[s]);
-          tma_load_2d(st + 2 * S::kABytes + S::kBBytes, &map_blo, (int)(kt * BK), nb * p.n_tile, &full[s]);
-        }
-      }
-    }
-  } else if (warp == kMmaWarp) {
-    // ===================================================================================== MMA issuer
-    if (lane == 0) {
-      const uint32_t idesc = instr_desc(p.n_tile);
-      uint32_t it = 0, acc_it = 0;
-      int n_stamp = 0;
-      for (long long tile = blockIdx.x; tile < n_tiles_total; tile += gridDim.x, ++acc_it) {
-        const int a = acc_it & 1;
-        const uint32_t aph = (acc_it >> 1) & 1;
-        mbar_wait_x(&tmem_empty[a], aph ^ 1, (p.dbg_skip & 8) == 0);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(a * BN);
-        for (long long kt = 0; kt < k_tiles; ++kt, ++it) {
-          const int s = it % kStages;
-          const uint32_t ph = (it / kStages) & 1;
-          mbar_wait_x(&full[s], ph, (p.dbg_skip & 8) == 0);
-          stamp(p, 1, n_stamp);
-          mbar_wait_x(&lo_ready[s], ph, (p.dbg_skip & 8) == 0);
-          stamp(p, 1, n_stamp);
-          tc_fence_after();
-          const uint32_t st = smem_u32(stage_base + (size_t)s * S::kStageBytes);
-          const uint64_t a_hi = smem_desc(st), a_lo = smem_desc(st + S::kABytes);
-          const uint64_t b_hi = smem_desc(st + 2 * S::kABytes), b_lo = smem_desc(st + 2 * S::kABytes + S::kBBytes);
-#pragma unroll
-          for (int kb = 0; kb < BK / UMMA_K; ++kb) {
-            const uint64_t adv = (uint64_t)((kb * UMMA_K * 4) >> 4);     // 32 bytes per k-block inside the swizzled row
-            umma_tf32(d_tmem, a_lo + adv, b_hi + adv, idesc, (kt > 0 || kb > 0) ? 1u : 0u);
-            umma_tf32(d_tmem, a_hi + adv, b_lo + adv, idesc, 1u);
-            umma_tf32(d_tmem, a_hi + adv, b_hi + adv, idesc, 1u);
-          }
-          umma_commit(&empty[s]);                    // frees the smem stage once these MMAs have read it
-          stamp(p, 1, n_stamp);
-        }
-        umma_commit(&tmem_full[a]);                  // accumulator complete
-      }
-    }
-  } else if (warp >= kTransformWarp0) {
-    // ===================================================================================== transform: A -> (A_hi, A_lo)
-    const int t = threadIdx.x - kTransformWarp0 * 32;   // 0..127
-    uint32_t it = 0;
-    int n_stamp = 0;
-    for (long long tile = blockIdx.x; tile < n_tiles_total; tile += gridDim.x) {
-      for (long long kt = 0; kt < k_tiles; ++kt, ++it) {
-        const int s = it % kStages;
-        const uint32_t ph = (it / kStages) & 1;
-        mbar_wait_x(&full[s], ph, (p.dbg_skip & 8) == 0);
-        if (t == 0) stamp(p, 2, n_stamp);
-        // loads are batched ahead of the stores (explicit ld/st.shared: with generic pointers the compiler serialised
-        // load -> use -> store and the transform, not the tensor pipe, set the pace)
-        const uint32_t st_addr = smem_u32(stage_base + (size_t)s * S::kStageBytes);
-        {   // A tile: BM rows
-          const uint32_t raw_addr = st_addr + (uint32_t)t * 16u;
-          constexpr int kPer = (BM * BK / 4) / kTransformThreads;
-          float4 v[kPer];
-#pragma unroll
-          for (int i = 0; i < kPer; ++i) v[i] = lds128(raw_addr + (uint32_t)i * (kTransformThreads * 16));
-#pragma unroll
-          for (int i = 0; i < kPer; ++i) split_store(raw_addr + (uint32_t)i * (kTransformThreads * 16), S::kABytes, v[i], (p.dbg_skip & 16) == 0);
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to the MMA's async proxy
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&lo_ready[s]);
-        if (t == 0) stamp(p, 2, n_stamp);
+  if (wg == 0) {
+    reg_dealloc<40>();
+    if (threadIdx.x == 0) {
+      prefetch_map(&map_a); prefetch_map(&map_bhi); prefetch_map(&map_blo);
+      for (int kt = 0; kt < k_tiles; ++kt) {
+        const int s = kt % kStages;
+        mbar_wait_hint(&empty[s], ((kt / kStages) & 1) ^ 1);
+        uint8_t* st = smem + s * S::kStageBytes;
+        mbar_expect_tx(&full[s], (uint32_t)S::kStageBytes);
+        tma_load_2d(st, &map_a, kt * BK, (int)m0, &full[s]);
+        tma_load_2d(st + S::kABytes, &map_bhi, kt * BK, n0, &full[s]);
+        tma_load_2d(st + S::kABytes + S::kBBytes, &map_blo, kt * BK, n0, &full[s]);
       }
     }
   } else {
-    // ===================================================================================== epilogue (warps 0-3)
-    uint32_t acc_it = 0, chunk_it = 0;
-    int n_stamp = 0;
-    for (long long tile = blockIdx.x; tile < n_tiles_total; tile += gridDim.x, ++acc_it) {
-      const long long mb = tile / p.n_blocks;
-      const int nb = (int)(tile % p.n_blocks);
-      const int a = acc_it & 1;
-      const uint32_t aph = (acc_it >> 1) & 1;
-      mbar_wait_x(&tmem_full[a], aph, (p.dbg_skip & 8) == 0);
-      if (threadIdx.x == 0) stamp(p, 3, n_stamp);
-      tc_fence_after();
-      // TMEM -> registers -> swizzled staging rows (this warp's 32 rows x 32 columns) -> TMA store; two staging buffers
-      // per warp so the store of chunk c overlaps the TMEM read of chunk c+1.  (Direct st.global of a thread's own row
-      // made every warp store touch 32 different lines: 13-15k cycles per tile, more than the main loop.)
-      const uint32_t taddr = tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)(a * BN);
-      const int row0 = (int)(mb * BM) + warp * 32;
-      const int col0 = nb * p.n_tile;
-      uint8_t* wbuf = store_base + warp * (2 * 32 * kStoreCols * 4);
-      const int n_valid = (p.N - col0) < p.n_tile ? (int)(p.N - col0) : p.n_tile;   // columns of this tile that exist
-      for (int c = 0; c < n_valid; c += kStoreCols, ++chunk_it) {
-        const uint32_t buf = smem_u32(wbuf + (chunk_it & 1) * (32 * kStoreCols * 4));
-        uint32_t v[32];
-        asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-            "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-            : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-              "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-              "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-              "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-            : "r"(taddr + (uint32_t)c));
-        // the buffer about to be overwritten was handed to a TMA store two chunks ago: wait until that store has read it
-        if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-        __syncwarp();
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+    reg_alloc<232>();
+    const int row_wg = (wg - 1) * 64 + (warp & 3) * 16;      // first of this warp's 16 rows inside the tile
+    float acc[BN / 2], part[BN / 2];       // running sum, this k-tile's tensor-core sum
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {       // 16-byte chunk j of this lane's 128-byte row, SWIZZLE_128B position
-          const uint32_t dst = buf + (uint32_t)lane * 128u + (uint32_t)((j ^ (lane & 7)) << 4);
-          sts128(dst, make_float4(__uint_as_float(v[4 * j]), __uint_as_float(v[4 * j + 1]), __uint_as_float(v[4 * j + 2]),
-                                  __uint_as_float(v[4 * j + 3])));
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        __syncwarp();
-        if (lane == 0) {
-          asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%1, %2}], [%3];"
-                       ::"l"(reinterpret_cast<uint64_t>(&map_c)), "r"(col0 + c), "r"(row0), "r"(buf) : "memory");
-          asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-        }
-      }
-      tc_fence_before();
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    for (int kt = 0; kt < k_tiles; ++kt) {
+      const int s = kt % kStages;
+      mbar_wait_hint(&full[s], (kt / kStages) & 1);
+      const uint32_t st = smem_u32(smem + s * S::kStageBytes);
+      uint32_t hi[16], lo[16];
+      load_a_split(st, row_wg, lane, hi, lo);
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) part[i] = 0.f;
+      mma_ktile_3xtf32<BN>(part, hi, lo, st + S::kABytes, st + S::kABytes + S::kBBytes);
+      wgmma_wait<0>();
       __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty[a]);
-      if (threadIdx.x == 0) stamp(p, 3, n_stamp);
+      if (lane == 0) mbar_arrive(&empty[s]);
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[i] += part[i];
     }
-    if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // all of this warp's stores have landed
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == kMmaWarp) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(kTmemCols) : "memory");
+    store_acc<BN>(acc, p.C, p.ldc, m0 + row_wg, p.M, n0, p.N, lane, false);
   }
 }
 
-// ================================================================================================ narrow outputs: A from TMEM
-// For N <= 128 the loop above is bound by shared-memory traffic per k-tile (TMA writes, the transform's read + two
-// writes of the A tile, and every MMA re-reading its 128-row A operand), not by the tensor pipe or HBM.  This variant
-// keeps the split A operand in TMEM: the transform warps read the TMA-written A tile once (one thread = one row),
-// split it in registers and tcgen05.st the hi / lo parts into TMEM columns; the MMAs take A from TMEM and only the small
-// weight tiles from shared memory.  TMEM: 2 accumulators x BN columns + kStages x 2 x BK columns of A.
-namespace ts {
-
-constexpr int BKT = 32;                      // k-tile of this variant: 128-byte rows (SWIZZLE_128B) - with 64-byte rows the
-constexpr int kRowBytesT = BKT * 4;          // TMA engine's per-row cost, not HBM, paced the tall-skinny A stream
-
-__device__ __forceinline__ uint64_t smem_desc_sw128(uint32_t addr) {
-  return (uint64_t)((addr >> 4) & 0x3FFF) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-}
-
-// STACK (n_tile == BN <= 64): the hi and lo weight tiles are adjacent in shared memory, so ONE MMA with N' = 2 BN
-// computes a_hi*b_hi and a_hi*b_lo side by side (accumulator columns [0, BN) and [BN, 2 BN)), a second one adds a_lo*b_hi
-// to the first half; the epilogue adds the halves.  Two MMAs per k-block instead of three: with outputs this narrow the
-// tensor pipe is bound by the number of MMA instructions, not by their size (skipping the MMAs: 68 -> 44 us on
-// [162 800, 352] -> 32, while skipping the transform only gains 8 us).
-template <int BN, bool STACK>
-struct TSmem {
-  static constexpr int kAccCols = STACK ? 2 * BN : BN;              // TMEM columns per accumulator buffer
-  static constexpr int kABytes = BM * kRowBytesT;                   // raw A tile (TMA)
-  static constexpr int kBBytes = BN * kRowBytesT;
-  static constexpr int kStageBytes = kABytes + 2 * kBBytes;         // A raw | B hi | B lo
-  static constexpr int kStoreBytes = kEpilogueWarps * 2 * 32 * kStoreCols * 4;
-  static constexpr int kBudget = 227 * 1024 - 1024;
-  static constexpr int kStagesSmem = (kBudget - kStoreBytes - 1024) / kStageBytes;
-  static constexpr int kStagesTmem = (512 - 2 * kAccCols) / (2 * BKT);
-  static constexpr int kStagesMin = kStagesSmem < kStagesTmem ? kStagesSmem : kStagesTmem;
-  static constexpr int kStages = kStagesMin > 8 ? 8 : kStagesMin;
-  static_assert(kStages >= 2, "tile does not fit");
-  static constexpr int kTotal = kStages * kStageBytes + kStoreBytes + 1024 + 1024;
-};
-
-__device__ __forceinline__ void umma_tf32_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const float* v) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      ::"r"(taddr), "f"(v[0]), "f"(v[1]), "f"(v[2]), "f"(v[3]), "f"(v[4]), "f"(v[5]), "f"(v[6]), "f"(v[7]), "f"(v[8]),
-        "f"(v[9]), "f"(v[10]), "f"(v[11]), "f"(v[12]), "f"(v[13]), "f"(v[14]), "f"(v[15]), "f"(v[16]), "f"(v[17]),
-        "f"(v[18]), "f"(v[19]), "f"(v[20]), "f"(v[21]), "f"(v[22]), "f"(v[23]), "f"(v[24]), "f"(v[25]), "f"(v[26]),
-        "f"(v[27]), "f"(v[28]), "f"(v[29]), "f"(v[30]), "f"(v[31]) : "memory");
-}
-
-template <int BN, bool STACK>
-__global__ void __launch_bounds__(kThreads, 1)
-gemm_tf32x3_ts_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_bhi,
-                      const __grid_constant__ CUtensorMap map_blo, const __grid_constant__ CUtensorMap map_c, Params p) {
-  using S = TSmem<BN, STACK>;
-  constexpr int kStages = S::kStages;
-  constexpr int kTmemCols = 512;
-  constexpr int kAcc = S::kAccCols;
-  constexpr int kACol0 = 2 * kAcc;                       // first TMEM column of the A staging area
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* stage_base = smem;
-  uint8_t* store_base = smem + kStages * S::kStageBytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(store_base + S::kStoreBytes);
-  uint64_t* full = bars;
-  uint64_t* a_ready = bars + kStages;          // A hi / lo of the stage are in TMEM
-  uint64_t* empty = bars + 2 * kStages;
-  uint64_t* tmem_full = bars + 3 * kStages;
-  uint64_t* tmem_empty = bars + 3 * kStages + 2;
-  uint32_t* tmem_base_slot = reinterpret_cast<uint32_t*>(bars + 3 * kStages + 4);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const long long k_tiles = (p.K + BKT - 1) / BKT;
-  const long long n_tiles_total = p.m_blocks * p.n_blocks;
-
-  if (warp == kProducerWarp && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_a)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_bhi)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_blo)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_c)) : "memory");
-    for (int s = 0; s < kStages; ++s) {
-      mbar_init(&full[s], 1);
-      mbar_init(&a_ready[s], kTransformWarps);
-      mbar_init(&empty[s], 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&tmem_full[a], 1);
-      mbar_init(&tmem_empty[a], kEpilogueWarps);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == kMmaWarp) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_base_slot)), "n"(kTmemCols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_base_slot;
-
-  if (warp == kProducerWarp) {
-    if (lane == 0) {
-      uint32_t it = 0;
-      int n_stamp = 0;
-      const uint32_t tx = (uint32_t)(S::kABytes + 2 * p.n_tile * kRowBytesT);
-      for (long long tile = blockIdx.x; tile < n_tiles_total; tile += gridDim.x) {
-        const long long mb = tile / p.n_blocks;
-        const int nb = (int)(tile % p.n_blocks);
-        for (long long kt = 0; kt < k_tiles; ++kt, ++it) {
-          const int s = it % kStages;
-          const uint32_t ph = (it / kStages) & 1;
-          mbar_wait_x(&empty[s], ph ^ 1, (p.dbg_skip & 8) == 0);
-          stamp(p, 0, n_stamp);
-          uint8_t* st = stage_base + (size_t)s * S::kStageBytes;
-          mbar_expect_tx(&full[s], tx);
-          tma_load_2d(st, &map_a, (int)(kt * BKT), (int)(mb * BM), &full[s]);
-          tma_load_2d(st + S::kABytes, &map_bhi, (int)(kt * BKT), nb * p.n_tile, &full[s]);
-          tma_load_2d(st + S::kABytes + S::kBBytes, &map_blo, (int)(kt * BKT), nb * p.n_tile, &full[s]);
-        }
-      }
-    }
-  } else if (warp == kMmaWarp) {
-    if (lane == 0) {
-      const uint32_t idesc = instr_desc(p.n_tile);
-      const uint32_t idesc2 = instr_desc(2 * p.n_tile);          // STACK: [b_hi | b_lo] as one operand
-      uint32_t it = 0, acc_it = 0;
-      int n_stamp = 0;
-      for (long long tile = blockIdx.x; tile < n_tiles_total; tile += gridDim.x, ++acc_it) {
-        const int a = acc_it & 1;
-        const uint32_t aph = (acc_it >> 1) & 1;
-        mbar_wait_x(&tmem_empty[a], aph ^ 1, (p.dbg_skip & 8) == 0);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(a * kAcc);
-        for (long long kt = 0; kt < k_tiles; ++kt, ++it) {
-          const int s = it % kStages;
-          const uint32_t ph = (it / kStages) & 1;
-          mbar_wait_x(&full[s], ph, (p.dbg_skip & 8) == 0);          // the weight tiles (and the raw A tile) have landed
-          stamp(p, 1, n_stamp);
-          mbar_wait_x(&a_ready[s], ph, (p.dbg_skip & 8) == 0);       // A hi / lo are in TMEM
-          stamp(p, 1, n_stamp);
-          tc_fence_after();
-          const uint32_t st = smem_u32(stage_base + (size_t)s * S::kStageBytes);
-          const uint64_t b_hi = smem_desc_sw128(st + S::kABytes), b_lo = smem_desc_sw128(st + S::kABytes + S::kBBytes);
-          const uint32_t a_hi = tmem_base + (uint32_t)(kACol0 + s * 2 * BKT), a_lo = a_hi + BKT;
-#pragma unroll
-          for (int kb = 0; kb < BKT / UMMA_K; ++kb) {
-            if (p.dbg_skip & 2) break;
-            const uint64_t adv = (uint64_t)((kb * UMMA_K * 4) >> 4);
-            const uint32_t acol = (uint32_t)(kb * UMMA_K);
-            if constexpr (STACK) {
-              umma_tf32_ts(d_tmem, a_hi + acol, b_hi + adv, idesc2, (kt > 0 || kb > 0) ? 1u : 0u);   // hi*hi | hi*lo
-              umma_tf32_ts(d_tmem, a_lo + acol, b_hi + adv, idesc, 1u);                               // + lo*hi
-            } else {
-              umma_tf32_ts(d_tmem, a_lo + acol, b_hi + adv, idesc, (kt > 0 || kb > 0) ? 1u : 0u);
-              umma_tf32_ts(d_tmem, a_hi + acol, b_lo + adv, idesc, 1u);
-              umma_tf32_ts(d_tmem, a_hi + acol, b_hi + adv, idesc, 1u);
-            }
-          }
-          umma_commit(&empty[s]);
-          stamp(p, 1, n_stamp);
-        }
-        umma_commit(&tmem_full[a]);
-      }
-    }
-  } else if (warp >= kTransformWarp0) {
-    // one thread = one row of the A tile (TMEM lane = 32 * (warp % 4) + lane); the row's eight 16-byte chunks sit at
-    // SWIZZLE_128B positions chunk ^ (row & 7)
-    const int row = (warp & 3) * 32 + lane;
-    const uint32_t lane_field = (uint32_t)((warp & 3) * 32) << 16;
-    uint32_t it = 0;
-    int n_stamp = 0;
-    const bool stamper = (threadIdx.x == kTransformWarp0 * 32);
-    for (long long tile = blockIdx.x; tile < n_tiles_total; tile += gridDim.x) {
-      for (long long kt = 0; kt < k_tiles; ++kt, ++it) {
-        const int s = it % kStages;
-        const uint32_t ph = (it / kStages) & 1;
-        mbar_wait_x(&full[s], ph, (p.dbg_skip & 8) == 0);
-        if (stamper) stamp(p, 2, n_stamp);
-        if (p.dbg_skip & 1) {
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&a_ready[s]);
-          continue;
-        }
-        const uint32_t rbase = smem_u32(stage_base + (size_t)s * S::kStageBytes) + (uint32_t)row * (uint32_t)kRowBytesT;
-        float hi[BKT], lo[BKT];
-        float4 v[8];
-#pragma unroll
-        for (int c = 0; c < 8; ++c) v[c] = lds128(rbase + (uint32_t)((c ^ (row & 7)) << 4));
-#pragma unroll
-        for (int c = 0; c < 8; ++c) {
-          const float x[4] = {v[c].x, v[c].y, v[c].z, v[c].w};
-#pragma unroll
-          for (int q = 0; q < 4; ++q) hi[4 * c + q] = x[q];
-        }
-        if (!(p.dbg_skip & 16)) {
-#pragma unroll
-          for (int j = 0; j < BKT; ++j) { const float x = hi[j]; hi[j] = tf32_rn_fast(x); lo[j] = x - hi[j]; }
-        } else {
-#pragma unroll
-          for (int j = 0; j < BKT; ++j) { const float x = hi[j]; hi[j] = tf32_rn(x); lo[j] = x - hi[j]; }
-        }
-        const uint32_t acol = tmem_base + lane_field + (uint32_t)(kACol0 + s * 2 * BKT);
-        tmem_st32(acol, hi);
-        tmem_st32(acol + BKT, lo);
-        asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&a_ready[s]);
-        if (stamper) stamp(p, 2, n_stamp);
-      }
-    }
-  } else {
-    uint32_t acc_it = 0, chunk_it = 0;
-    int n_stamp = 0;
-    for (long long tile = blockIdx.x; tile < n_tiles_total; tile += gridDim.x, ++acc_it) {
-      const long long mb = tile / p.n_blocks;
-      const int nb = (int)(tile % p.n_blocks);
-      const int a = acc_it & 1;
-      const uint32_t aph = (acc_it >> 1) & 1;
-      mbar_wait_x(&tmem_full[a], aph, (p.dbg_skip & 8) == 0);
-      if (threadIdx.x == 0) stamp(p, 3, n_stamp);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)(a * kAcc);
-      const int row0 = (int)(mb * BM) + warp * 32;
-      const int col0 = nb * p.n_tile;
-      uint8_t* wbuf = store_base + warp * (2 * 32 * kStoreCols * 4);
-      const int n_valid = (p.N - col0) < p.n_tile ? (int)(p.N - col0) : p.n_tile;   // columns of this tile that exist
-      for (int c = 0; c < n_valid; c += kStoreCols, ++chunk_it) {
-        const uint32_t buf = smem_u32(wbuf + (chunk_it & 1) * (32 * kStoreCols * 4));
-        uint32_t v[32];
-        asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-            "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-            : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-              "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-              "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-              "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-            : "r"(taddr + (uint32_t)c));
-        uint32_t v2[32];
-        if constexpr (STACK) {     // the hi*lo half of the stacked accumulator
-          asm volatile(
-              "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-              "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-              : "=r"(v2[0]), "=r"(v2[1]), "=r"(v2[2]), "=r"(v2[3]), "=r"(v2[4]), "=r"(v2[5]), "=r"(v2[6]), "=r"(v2[7]),
-                "=r"(v2[8]), "=r"(v2[9]), "=r"(v2[10]), "=r"(v2[11]), "=r"(v2[12]), "=r"(v2[13]), "=r"(v2[14]), "=r"(v2[15]),
-                "=r"(v2[16]), "=r"(v2[17]), "=r"(v2[18]), "=r"(v2[19]), "=r"(v2[20]), "=r"(v2[21]), "=r"(v2[22]), "=r"(v2[23]),
-                "=r"(v2[24]), "=r"(v2[25]), "=r"(v2[26]), "=r"(v2[27]), "=r"(v2[28]), "=r"(v2[29]), "=r"(v2[30]), "=r"(v2[31])
-              : "r"(taddr + (uint32_t)(BN + c)));
-        }
-        if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-        __syncwarp();
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        if constexpr (STACK) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(__uint_as_float(v[j]) + __uint_as_float(v2[j]));
-        }
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const uint32_t dst = buf + (uint32_t)lane * 128u + (uint32_t)((j ^ (lane & 7)) << 4);
-          sts128(dst, make_float4(__uint_as_float(v[4 * j]), __uint_as_float(v[4 * j + 1]), __uint_as_float(v[4 * j + 2]),
-                                  __uint_as_float(v[4 * j + 3])));
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        __syncwarp();
-        if (lane == 0) {
-          asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%1, %2}], [%3];"
-                       ::"l"(reinterpret_cast<uint64_t>(&map_c)), "r"(col0 + c), "r"(row0), "r"(buf) : "memory");
-          asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty[a]);
-      if (threadIdx.x == 0) stamp(p, 3, n_stamp);
-    }
-    if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == kMmaWarp) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(kTmemCols) : "memory");
-  }
-}
-
-}  // namespace ts
-
-// ================================================================================================ CTA-pair variant
-// The stacked narrow-output kernel above is bound by the NUMBER of MMA instructions (about 100 cycles each whatever
-// their width).  Here two CTAs of a cluster (one TPC) share each instruction: tcgen05.mma.cta_group::2 with M = 256 -
-// CTA r owns rows [256 t + 128 r, +128) of the tile (its A hi / lo in its own TMEM, its accumulator rows in its own
-// TMEM) and supplies HALF of the weight operand's columns from its own shared memory:
-//   MMA 1  a_hi x [b_hi | b_lo]   N' = 2 BN   CTA 0 holds b_hi (columns [0, BN)), CTA 1 holds b_lo ([BN, 2 BN))   region Y
-//   MMA 2  a_lo x  b_hi           N  = BN     CTA 0 holds b_hi rows [0, BN/2), CTA 1 rows [BN/2, BN)             region X
-// so one instruction pair covers 256 rows instead of 128 and each SM reads half the weight bytes per row.
-// Only the leader (rank 0) issues MMAs; its commits are multicast to both CTAs' `empty` / `tmem_full` barriers; the
-// transform and epilogue warps of both CTAs arrive on the LEADER's `a_ready` / `tmem_empty` barriers (mapa + remote arrive).
-//
-// MEASURED (profiles/r1_tf32x3_cta_pair_*.txt): bit-identical to the single-CTA kernel, and 9-11 % SLOWER
-// ([162 800, 352] -> 32: 70.5 vs 64.7 us; [97 680, 384] -> 64: 56.1 vs 50.3 us), so it stays opt-in (EQF_TF32X3_2SM=1).
-// The timeline shows why: an M = 256 pair instruction occupies the issue slot of the one leader thread for the same
-// ~85 cycles as an M = 128 one, but it is the ONLY issuer for two SMs - instructions per row halve and so do the
-// issuers, nothing is gained - while the shapes' real floor is the A stream (load skeleton alone: 46 of 65 us).  What a
-// pair does save, weight bytes read from shared memory per SM, is not what limits a 32- or 64-column output.
-namespace ts2 {
-
-using ts::BKT;
-using ts::kRowBytesT;
-
-template <int BN>
-struct T2Smem {
-  static constexpr int kAccCols = 2 * BN;
-  static constexpr int kABytes = BM * kRowBytesT;
-  static constexpr int kYBytes = BN * kRowBytesT;
-  static constexpr int kXBytes = (BN / 2) * kRowBytesT;
-  static constexpr int kStageBytes = kABytes + kYBytes + kXBytes;
-  static_assert(kYBytes % 1024 == 0 && kXBytes % 1024 == 0, "operand regions must keep the 1024-byte swizzle alignment");
-  static constexpr int kStoreBytes = kEpilogueWarps * 2 * 32 * kStoreCols * 4;
-  static constexpr int kBudget = 227 * 1024 - 1024;
-  static constexpr int kStagesSmem = (kBudget - kStoreBytes - 1024) / kStageBytes;
-  static constexpr int kStagesTmem = (512 - 2 * kAccCols) / (2 * BKT);
-  static constexpr int kStagesMin = kStagesSmem < kStagesTmem ? kStagesSmem : kStagesTmem;
-  static constexpr int kStages = kStagesMin > 8 ? 8 : kStagesMin;
-  static_assert(kStages >= 2, "tile does not fit");
-  static constexpr int kTotal = kStages * kStageBytes + kStoreBytes + 1024 + 1024;
-};
-
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// arrive on the barrier at the same shared-memory offset in CTA `rank` of the cluster
-__device__ __forceinline__ void mbar_arrive_on(uint64_t* bar, uint32_t rank) {
-  uint32_t remote;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(bar)), "r"(rank));
-  // plain arrive (as cutlass::arch::ClusterBarrier::arrive(cta_id)): with .release.cluster the compiler emits
-  // MEMBAR.ALL.GPU in front of it - ~3 000 cycles per k-tile, which made the first version 2x SLOWER than one CTA.
-  // What the leader's MMA consumes was made visible by other means: the operand tiles by the TMA's own completion on
-  // this CTA's barrier, the tensor-memory stores by tcgen05.wait::st + fence::before_thread_sync.
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
-}
-__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {
-  uint32_t done;
-  do {
-    asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                 : "=r"(done) : "r"(smem_u32(bar)), "r"(parity) : "memory");
-  } while (!done);
-}
-// arrives on `bar` in BOTH CTAs once every MMA issued so far has finished
-__device__ __forceinline__ void umma_commit_pair(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(smem_u32(bar)), "h"((uint16_t)3) : "memory");
-}
-__device__ __forceinline__ void umma_tf32_ts_pair(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::tf32 [%0], [%1], %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// kind::tf32, fp32 accumulate, K-major A and B, M = 256 (the pair), N = n
-__device__ __forceinline__ uint32_t instr_desc_pair(int n) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(256 >> 4) << 24);
-}
-
-template <int BN>
-__global__ void __launch_bounds__(kThreads, 1)
-gemm_tf32x3_ts2_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_bhi,
-                       const __grid_constant__ CUtensorMap map_blo, const __grid_constant__ CUtensorMap map_bhalf,
-                       const __grid_constant__ CUtensorMap map_c, Params p) {
-  using S = T2Smem<BN>;
-  constexpr int kStages = S::kStages;
-  constexpr int kTmemCols = 512;
-  constexpr int kAcc = S::kAccCols;
-  constexpr int kACol0 = 2 * kAcc;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* stage_base = smem;
-  uint8_t* store_base = smem + kStages * S::kStageBytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(store_base + S::kStoreBytes);
-  uint64_t* full = bars;                        // local: this CTA's TMA loads of the stage have landed
-  uint64_t* a_ready = bars + kStages;           // leader's copy counts the transform warps of BOTH CTAs
-  uint64_t* empty = bars + 2 * kStages;         // both copies: multicast commit
-  uint64_t* tmem_full = bars + 3 * kStages;     // both copies: multicast commit
-  uint64_t* tmem_empty = bars + 3 * kStages + 2;   // leader's copy counts the epilogue warps of BOTH CTAs
-  uint32_t* tmem_base_slot = reinterpret_cast<uint32_t*>(bars + 3 * kStages + 4);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const long long k_tiles = (p.K + BKT - 1) / BKT;
-  const long long m2_blocks = (p.M + 2 * BM - 1) / (2 * BM);
-  const long long n_tiles_total = m2_blocks * p.n_blocks;
-  const long long first_tile = blockIdx.x >> 1, tile_step = gridDim.x >> 1;
-
-  if (warp == kProducerWarp && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_a)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_bhi)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_blo)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_bhalf)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_c)) : "memory");
-    for (int s = 0; s < kStages; ++s) {
-      mbar_init(&full[s], 1);
-      mbar_init(&a_ready[s], 2 * kTransformWarps);
-      mbar_init(&empty[s], 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&tmem_full[a], 1);
-      mbar_init(&tmem_empty[a], 2 * kEpilogueWarps);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == kMmaWarp) {     // the same warp of both CTAs allocates (and later frees) the pair's tensor memory
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_base_slot)), "n"(kTmemCols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  cluster_sync_all();        // barrier inits and the allocation are visible to the peer before anything arrives remotely
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_base_slot;
-
-  if (warp == kProducerWarp) {
-    if (lane == 0) {
-      uint32_t it = 0;
-      int n_stamp = 0;
-      const int half = p.n_tile >> 1;
-      const uint32_t tx = (uint32_t)(S::kABytes + (p.n_tile + half) * kRowBytesT);
-      const CUtensorMap* map_y = rank == 0 ? &map_bhi : &map_blo;
-      for (long long tile = first_tile; tile < n_tiles_total; tile += tile_step) {
-        const long long mb2 = tile / p.n_blocks;
-        const int nb = (int)(tile % p.n_blocks);
-        const int row0 = (int)(mb2 * 2 * BM) + (int)rank * BM;
-        for (long long kt = 0; kt < k_tiles; ++kt, ++it) {
-          const int s = it % kStages;
-          const uint32_t ph = (it / kStages) & 1;
-          mbar_wait_x(&empty[s], ph ^ 1, (p.dbg_skip & 8) == 0);
-          stamp(p, 0, n_stamp);
-          uint8_t* st = stage_base + (size_t)s * S::kStageBytes;
-          mbar_expect_tx(&full[s], tx);
-          tma_load_2d(st, &map_a, (int)(kt * BKT), row0, &full[s]);
-          tma_load_2d(st + S::kABytes, map_y, (int)(kt * BKT), nb * p.n_tile, &full[s]);
-          tma_load_2d(st + S::kABytes + S::kYBytes, &map_bhalf, (int)(kt * BKT), nb * p.n_tile + (int)rank * half, &full[s]);
-        }
-      }
-    }
-  } else if (warp == kMmaWarp) {
-    if (lane == 0 && rank == 0) {
-      const uint32_t idesc = instr_desc_pair(p.n_tile);
-      const uint32_t idesc2 = instr_desc_pair(2 * p.n_tile);
-      uint32_t it = 0, acc_it = 0;
-      int n_stamp = 0;
-      for (long long tile = first_tile; tile < n_tiles_total; tile += tile_step, ++acc_it) {
-        const int a = acc_it & 1;
-        const uint32_t aph = (acc_it >> 1) & 1;
-        mbar_wait_cluster(&tmem_empty[a], aph ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(a * kAcc);
-        for (long long kt = 0; kt < k_tiles; ++kt, ++it) {
-          const int s = it % kStages;
-          const uint32_t ph = (it / kStages) & 1;
-          mbar_wait_x(&full[s], ph, (p.dbg_skip & 8) == 0);
-          stamp(p, 1, n_stamp);
-          mbar_wait_cluster(&a_ready[s], ph);      // both CTAs: operand tiles landed, A hi / lo in tensor memory
-          stamp(p, 1, n_stamp);
-          tc_fence_after();
-          const uint32_t st = smem_u32(stage_base + (size_t)s * S::kStageBytes);
-          const uint64_t b_y = ts::smem_desc_sw128(st + S::kABytes), b_x = ts::smem_desc_sw128(st + S::kABytes + S::kYBytes);
-          const uint32_t a_hi = tmem_base + (uint32_t)(kACol0 + s * 2 * BKT), a_lo = a_hi + BKT;
-#pragma unroll
-          for (int kb = 0; kb < BKT / UMMA_K; ++kb) {
-            if (p.dbg_skip & 2) break;
-            const uint64_t adv = (uint64_t)((kb * UMMA_K * 4) >> 4);
-            const uint32_t acol = (uint32_t)(kb * UMMA_K);
-            umma_tf32_ts_pair(d_tmem, a_hi + acol, b_y + adv, idesc2, (kt > 0 || kb > 0) ? 1u : 0u);   // hi*hi | hi*lo
-            umma_tf32_ts_pair(d_tmem, a_lo + acol, b_x + adv, idesc, 1u);                               // + lo*hi
-          }
-          umma_commit_pair(&empty[s]);
-          stamp(p, 1, n_stamp);
-        }
-        umma_commit_pair(&tmem_full[a]);
-      }
-    }
-  } else if (warp >= kTransformWarp0) {
-    const int row = (warp & 3) * 32 + lane;
-    const uint32_t lane_field = (uint32_t)((warp & 3) * 32) << 16;
-    uint32_t it = 0;
-    int n_stamp = 0;
-    const bool stamper = (threadIdx.x == kTransformWarp0 * 32);
-    for (long long tile = first_tile; tile < n_tiles_total; tile += tile_step) {
-      for (long long kt = 0; kt < k_tiles; ++kt, ++it) {
-        const int s = it % kStages;
-        const uint32_t ph = (it / kStages) & 1;
-        mbar_wait_x(&full[s], ph, (p.dbg_skip & 8) == 0);
-        if (stamper) stamp(p, 2, n_stamp);
-        if (!(p.dbg_skip & 1)) {
-          const uint32_t rbase = smem_u32(stage_base + (size_t)s * S::kStageBytes) + (uint32_t)row * (uint32_t)kRowBytesT;
-          float hi[BKT], lo[BKT];
-          float4 v[8];
-#pragma unroll
-          for (int c = 0; c < 8; ++c) v[c] = lds128(rbase + (uint32_t)((c ^ (row & 7)) << 4));
-#pragma unroll
-          for (int c = 0; c < 8; ++c) {
-            const float x[4] = {v[c].x, v[c].y, v[c].z, v[c].w};
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              hi[4 * c + q] = tf32_rn(x[q]);
-              lo[4 * c + q] = x[q] - hi[4 * c + q];
-            }
-          }
-          const uint32_t acol = tmem_base + lane_field + (uint32_t)(kACol0 + s * 2 * BKT);
-          ts::tmem_st32(acol, hi);
-          ts::tmem_st32(acol + BKT, lo);
-          asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-        }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive_on(&a_ready[s], 0);
-        if (stamper) stamp(p, 2, n_stamp);
-      }
-    }
-  } else {
-    uint32_t acc_it = 0, chunk_it = 0;
-    int n_stamp = 0;
-    for (long long tile = first_tile; tile < n_tiles_total; tile += tile_step, ++acc_it) {
-      const long long mb2 = tile / p.n_blocks;
-      const int nb = (int)(tile % p.n_blocks);
-      const int a = acc_it & 1;
-      const uint32_t aph = (acc_it >> 1) & 1;
-      mbar_wait_x(&tmem_full[a], aph, (p.dbg_skip & 8) == 0);
-      if (threadIdx.x == 0) stamp(p, 3, n_stamp);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)(a * kAcc);
-      const long long row0 = mb2 * 2 * BM + (long long)rank * BM + warp * 32;
-      const int col0 = nb * p.n_tile;
-      uint8_t* wbuf = store_base + warp * (2 * 32 * kStoreCols * 4);
-      const int n_valid = (p.N - col0) < p.n_tile ? (int)(p.N - col0) : p.n_tile;
-      for (int c = 0; c < n_valid; c += kStoreCols, ++chunk_it) {
-        const uint32_t buf = smem_u32(wbuf + (chunk_it & 1) * (32 * kStoreCols * 4));
-        uint32_t v[32], v2[32];
-        asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-            "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-            : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-              "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-              "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-              "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-            : "r"(taddr + (uint32_t)c));
-        asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-            "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-            : "=r"(v2[0]), "=r"(v2[1]), "=r"(v2[2]), "=r"(v2[3]), "=r"(v2[4]), "=r"(v2[5]), "=r"(v2[6]), "=r"(v2[7]),
-              "=r"(v2[8]), "=r"(v2[9]), "=r"(v2[10]), "=r"(v2[11]), "=r"(v2[12]), "=r"(v2[13]), "=r"(v2[14]), "=r"(v2[15]),
-              "=r"(v2[16]), "=r"(v2[17]), "=r"(v2[18]), "=r"(v2[19]), "=r"(v2[20]), "=r"(v2[21]), "=r"(v2[22]), "=r"(v2[23]),
-              "=r"(v2[24]), "=r"(v2[25]), "=r"(v2[26]), "=r"(v2[27]), "=r"(v2[28]), "=r"(v2[29]), "=r"(v2[30]), "=r"(v2[31])
-            : "r"(taddr + (uint32_t)(BN + c)));
-        if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-        __syncwarp();
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(__uint_as_float(v[j]) + __uint_as_float(v2[j]));
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const uint32_t dst = buf + (uint32_t)lane * 128u + (uint32_t)((j ^ (lane & 7)) << 4);
-          sts128(dst, make_float4(__uint_as_float(v[4 * j]), __uint_as_float(v[4 * j + 1]), __uint_as_float(v[4 * j + 2]),
-                                  __uint_as_float(v[4 * j + 3])));
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        __syncwarp();
-        if (lane == 0 && row0 < p.M) {
-          asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%1, %2}], [%3];"
-                       ::"l"(reinterpret_cast<uint64_t>(&map_c)), "r"(col0 + c), "r"((int)row0), "r"(buf) : "memory");
-          asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_on(&tmem_empty[a], 0);
-      if (threadIdx.x == 0) stamp(p, 3, n_stamp);
-    }
-    if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-  }
-
-  tc_fence_before();
-  cluster_sync_all();        // nobody leaves (or frees tensor memory) while the peer can still arrive here
-  if (warp == kMmaWarp) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(kTmemCols) : "memory");
-  }
-}
-
-}  // namespace ts2
-
-// hi / lo planes of the (small) weight operand: hi = w rounded to tf32, lo = w - hi
+// hi / lo planes of the (small) weight operand: hi = w rounded to tf32, lo = w - hi rounded to tf32
 __global__ void split_kernel(const float* __restrict__ w, float* __restrict__ hi, float* __restrict__ lo, long long n) {
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     const float v = w[i];
     const float h = tf32_rn(v);
     hi[i] = h;
-    lo[i] = v - h;
+    lo[i] = tf32_rn(v - h);
   }
 }
 
@@ -992,302 +134,159 @@ __global__ void split_transpose_kernel(const float* __restrict__ w, long long ld
     const float v = w[k * ldw + n];
     const float h = tf32_rn(v);
     hi[i] = h;
-    lo[i] = v - h;
+    lo[i] = tf32_rn(v - h);
   }
 }
 
-// ---------------------------------------------------------------------------------------------- host side
-typedef CUresult (*EncodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static EncodeTiled encode_fn() {
-  static EncodeTiled fn = [] {
-    void* f = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &f, cudaEnableDefault, &q) != cudaSuccess) f = nullptr;
-    return reinterpret_cast<EncodeTiled>(f);
-  }();
-  return fn;
-}
-
-// 2-D fp32 tensor [rows, cols] with row stride ld (elements), box = [box_rows, box_cols], swizzle span = box row bytes
-// (64 or 128), zero fill out of bounds (loads) / clipping (stores)
-static int make_map(CUtensorMap* map, const float* base, long long rows, long long cols, long long ld, int box_rows,
-                    int box_cols, bool atom_32b = false, bool linear = false) {
-  EncodeTiled enc = encode_fn();
-  if (enc == nullptr) { set_error("cuTensorMapEncodeTiled is not available from the driver"); return EQF_ERR_CUDA; }
-  cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)ld * sizeof(float)};
-  cuuint32_t box[2] = {(cuuint32_t)box_cols, (cuuint32_t)box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  // atom_32b: 32-byte chunks swizzled within the 128-byte span - the only layout the MMA accepts for MN-major tf32 operands
-  // linear: rows of the box land back to back, unswizzled (read by threads, never by the MMA)
-  const CUtensorMapSwizzle sw = linear ? CU_TENSOR_MAP_SWIZZLE_NONE
-                                : atom_32b ? CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B
-                                : (box_cols * 4 == 128) ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
-  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled failed (code " + std::to_string((int)r) + ")"); return EQF_ERR_CUDA; }
-  return EQF_OK;
-}
-
 template <int BN>
-static int launch(const CUtensorMap& ma, const CUtensorMap& mh, const CUtensorMap& ml, const CUtensorMap& mc,
-                  const Params& p, cudaStream_t s) {
+static int launch(const CUtensorMap& ma, const CUtensorMap& mh, const CUtensorMap& ml, const Params& p, long long m_blocks,
+                  int n_blocks, cudaStream_t s) {
   static std::once_flag once;
   static cudaError_t attr_err = cudaSuccess;
   std::call_once(once, [] {
     attr_err = cudaFuncSetAttribute(gemm_tf32x3_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Smem<BN>::kTotal);
   });
   if (attr_err != cudaSuccess) return check_cuda(attr_err, "gemm_tf32x3 smem attribute");
-  int sms = 148;
-  int dev = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  const long long tiles = p.m_blocks * p.n_blocks;
-  const int grid = (int)(tiles < sms ? tiles : sms);
-  gemm_tf32x3_kernel<BN><<<grid, kThreads, Smem<BN>::kTotal, s>>>(ma, mh, ml, mc, p);
+  gemm_tf32x3_kernel<BN><<<dim3((unsigned)m_blocks, (unsigned)n_blocks), kThreads, Smem<BN>::kTotal, s>>>(ma, mh, ml, p);
   return check_cuda(cudaGetLastError(), "gemm_tf32x3_kernel launch");
 }
 
-
 // ================================================================================================ weight gradient
-//   W[K1, N] = A[R, K1]^T G[R, N]        (reduction over the R = edges x (2l+1) rows; tiny output)
-// Both operands are "MN-major" for the MMA (the non-reduction dimension is the contiguous one in HBM): a tile is a
-// row of TMA boxes [BKR reduction rows x 32 columns] (128-byte rows, swizzle 128B_ATOM_32B), i.e. canonical UMMA
-// MN-major atoms of 4 rows x 128 bytes; LBO = distance between the 32-column blocks, SBO = distance between atoms.
-// grid = (output tiles of 128 x n_tile) x (row slices): every CTA reduces its slice of rows into one TMEM accumulator
-// and writes a partial [K1, N] block; the caller sums the partials over slices (eqf_colsum).  Same warp roles and
-// 3xTF32 split as the forward kernel; here the transform warps split both operand tiles.
 namespace wg {
 
-#ifndef EQF_WGRAD_BKR
-#define EQF_WGRAD_BKR 32
-#endif
-constexpr int BKR = EQF_WGRAD_BKR;            // reduction rows per stage (k-blocks of 8)
-constexpr int kBlockBytes = BKR * 128;        // one [BKR x 32] box
-constexpr int kMBlocks = BM / 32;             // 4 boxes for the 128 output rows
+constexpr int BKR = BK;                   // reduction rows per stage
+constexpr int kBoxBytes = BKR * 128;      // one [BKR rows x 32 columns] box of A, SWIZZLE_128B
+constexpr int kMaxBN = 128;
 
 struct WParams {
-  long long R, rows_per_slice;
-  int n_tile, n_tiles;                        // output columns per CTA (multiple of 32), number of column tiles
-  int reduce;                                 // 1: TMA reduce-add into W[K1, N] (map_p is 2-D); 0: store partial[slice]
-  int dbg_skip;                               // measurement aid: bit 0 skips the transform, bit 1 the MMAs (garbage results)
+  float* out;
+  long long R, rows_per_slice, K1;
+  int N;
+  int reduce;                             // 1: atomic adds into W[K1, N]; 0: store partial[slice]
 };
 
 template <int BN>
 struct WSmem {
-  static constexpr int kABytes = kMBlocks * kBlockBytes;           // 8 KB
-  static constexpr int kGBytes = (BN / 32) * kBlockBytes;
-  static constexpr int kRaw = kABytes + kGBytes;                   // hi (raw) part of a stage; the lo part follows
-  static constexpr int kStageBytes = 2 * kRaw;
-  static constexpr int kStoreBytes = kEpilogueWarps * 2 * 32 * kStoreCols * 4;
-  static constexpr int kBudget = 227 * 1024 - 1024;
-  static constexpr int kStagesRaw = (kBudget - kStoreBytes - 1024) / kStageBytes;
-  static constexpr int kStages = kStagesRaw > 8 ? 8 : kStagesRaw;
-  static constexpr int kTotal = kStages * kStageBytes + kStoreBytes + 1024 + 1024;
+  static constexpr int kABytes = (BM / 32) * kBoxBytes;           // A: four [BKR x 32] boxes (the CTA's 128 columns of K1)
+  static constexpr int kGRawBytes = BKR * BN * 4;                 // G: [BKR x BN] unswizzled rows
+  static constexpr int kGBytes = BN * kRowBytes;                  // G^T hi / lo: [BN x BKR] K-major, SWIZZLE_128B
+  static constexpr int kStageBytes = kABytes + kGRawBytes + 2 * kGBytes;
+  static constexpr int kStagesRaw = (kSmemBudget - 2048) / kStageBytes;
+  static constexpr int kStages = kStagesRaw > kMaxStages ? kMaxStages : kStagesRaw;
+  static_assert(kStages >= 2, "tile does not fit shared memory");
+  static constexpr int kTotal = kStages * kStageBytes + 1024 + 1024;
 };
 
-// MN-major tf32 operands exist only in the SWIZZLE_128B_BASE32B layout (cute: Layout_MN_SW128_32B_Atom, TMA swizzle
-// 128B_ATOM_32B): atoms of 4 reduction rows x 128 bytes; SBO = distance between the 4-row atoms (512 B), LBO = distance
-// between the 32-column blocks; one MMA (K = 8) spans two atoms.
-__device__ __forceinline__ uint64_t smem_desc_mn(uint32_t addr) {
-  constexpr uint64_t lbo = kBlockBytes >> 4, sbo = 512 >> 4;
-  return (uint64_t)((addr >> 4) & 0x3FFF) | (lbo << 16) | (sbo << 32) | (1ull << 46) | (1ull << 61);
-}
-__device__ __forceinline__ uint32_t instr_desc_mn(int n) {    // as instr_desc, with A and B MN-major (bits 15, 16)
-  return (1u << 4) | (2u << 7) | (2u << 10) | (1u << 15) | (1u << 16) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
+// register fragments of A^T (rows = columns m of A, reduction = rows r of A) from the four swizzled boxes of a stage
+__device__ __forceinline__ void load_at_split(uint32_t tile, int row0, int lane, uint32_t (&hi)[16], uint32_t (&lo)[16]) {
+  const int g = row0 + (lane >> 2), t = lane & 3;
+#pragma unroll
+  for (int kb = 0; kb < BKR / 8; ++kb) {
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const int m = g + ((q & 1) ? 8 : 0);
+      const int r = kb * 8 + t + ((q & 2) ? 4 : 0);
+      const int c = m & 31;
+      const uint32_t addr = tile + (uint32_t)(m >> 5) * kBoxBytes + (uint32_t)r * 128u + (uint32_t)((((c >> 2) ^ (r & 7)) << 4) + (c & 3) * 4);
+      const float x = lds32(addr);
+      const float h = tf32_rn_fast(x);
+      hi[kb * 4 + q] = __float_as_uint(h);
+      lo[kb * 4 + q] = __float_as_uint(tf32_rn_fast(x - h));
+    }
+  }
 }
 
 template <int BN>
 __global__ void __launch_bounds__(kThreads, 1)
-wgrad_tf32x3_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_g,
-                    const __grid_constant__ CUtensorMap map_p, WParams p) {
+wgrad_tf32x3_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_g, WParams p) {
   using S = WSmem<BN>;
   constexpr int kStages = S::kStages;
-  constexpr int kTmemCols = BN <= 32 ? 32 : BN <= 64 ? 64 : BN <= 128 ? 128 : 256;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* store_base = smem + kStages * S::kStageBytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(store_base + S::kStoreBytes);
-  uint64_t* full = bars;
-  uint64_t* lo_ready = bars + kStages;
-  uint64_t* empty = bars + 2 * kStages;
-  uint64_t* tmem_full = bars + 3 * kStages;
-  uint32_t* tmem_base_slot = reinterpret_cast<uint32_t*>(bars + 3 * kStages + 1);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + kStages * S::kStageBytes);
+  uint64_t* empty = full + kStages;
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int mt = blockIdx.x / p.n_tiles, nt = blockIdx.x % p.n_tiles;
-  const long long r0 = (long long)blockIdx.y * p.rows_per_slice;
-  long long rows = p.R - r0;
-  if (rows > p.rows_per_slice) rows = p.rows_per_slice;
-  const int k_tiles = (int)((rows + BKR - 1) / BKR);       // >= 1 (host guarantees non-empty slices)
-  const int g_blocks = p.n_tile / 32;
-
-  if (warp == kProducerWarp && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_a)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_g)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_p)) : "memory");
-    for (int s = 0; s < kStages; ++s) {
-      mbar_init(&full[s], 1);
-      mbar_init(&lo_ready[s], kTransformWarps);
-      mbar_init(&empty[s], 1);
-    }
-    mbar_init(tmem_full, 1);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wgi = warp >> 2;
+  const int m0 = blockIdx.x * BM;
+  const int n0 = blockIdx.y * BN;
+  const long long r_begin = (long long)blockIdx.z * p.rows_per_slice;
+  long long r_end = r_begin + p.rows_per_slice;
+  if (r_end > p.R) r_end = p.R;
+  const int k_tiles = (int)((r_end - r_begin + BKR - 1) / BKR);    // rows_per_slice % BKR == 0: slices never overlap
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < kStages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], kConsumerWarps); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == kMmaWarp) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_base_slot)), "n"(kTmemCols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_base_slot;
 
-  if (warp == kProducerWarp) {
-    if (lane == 0) {
-      const uint32_t tx = (uint32_t)((kMBlocks + g_blocks) * kBlockBytes);
+  if (wgi == 0) {
+    reg_dealloc<40>();
+    if (threadIdx.x == 0) {
+      prefetch_map(&map_a); prefetch_map(&map_g);
       for (int kt = 0; kt < k_tiles; ++kt) {
         const int s = kt % kStages;
-        const uint32_t ph = (kt / kStages) & 1;
-        mbar_wait_x(&empty[s], ph ^ 1, (p.dbg_skip & 8) == 0);
-        uint8_t* st = stage_base_of(smem, s, S::kStageBytes);
-        mbar_expect_tx(&full[s], tx);
-        const int row = (int)(r0 + (long long)kt * BKR);
-        for (int j = 0; j < kMBlocks; ++j) tma_load_2d(st + j * kBlockBytes, &map_a, mt * BM + 32 * j, row, &full[s]);
-        for (int j = 0; j < g_blocks; ++j)
-          tma_load_2d(st + S::kABytes + j * kBlockBytes, &map_g, nt * p.n_tile + 32 * j, row, &full[s]);
-      }
-    }
-  } else if (warp == kMmaWarp) {
-    if (lane == 0) {
-      const uint32_t idesc = instr_desc_mn(p.n_tile);
-      for (int kt = 0; kt < k_tiles; ++kt) {
-        const int s = kt % kStages;
-        const uint32_t ph = (kt / kStages) & 1;
-        mbar_wait_x(&full[s], ph, (p.dbg_skip & 8) == 0);
-        mbar_wait_x(&lo_ready[s], ph, (p.dbg_skip & 8) == 0);
-        tc_fence_after();
-        const uint32_t st = smem_u32(stage_base_of(smem, s, S::kStageBytes));
+        mbar_wait_hint(&empty[s], ((kt / kStages) & 1) ^ 1);
+        uint8_t* st = smem + s * S::kStageBytes;
+        const int r = (int)(r_begin + (long long)kt * BKR);
+        mbar_expect_tx(&full[s], (uint32_t)(S::kABytes + S::kGRawBytes));
 #pragma unroll
-        for (int kb = 0; kb < BKR / UMMA_K; ++kb) {
-          if (p.dbg_skip & 2) break;
-          const uint32_t off = (uint32_t)kb * 1024u;              // next 8-row group inside every 32-column block
-          const uint64_t a_hi = smem_desc_mn(st + off), g_hi = smem_desc_mn(st + S::kABytes + off);
-          const uint64_t a_lo = smem_desc_mn(st + S::kRaw + off), g_lo = smem_desc_mn(st + S::kRaw + S::kABytes + off);
-          umma_tf32(tmem_base, a_lo, g_hi, idesc, (kt > 0 || kb > 0) ? 1u : 0u);
-          umma_tf32(tmem_base, a_hi, g_lo, idesc, 1u);
-          umma_tf32(tmem_base, a_hi, g_hi, idesc, 1u);
-        }
-        umma_commit(&empty[s]);
+        for (int b = 0; b < BM / 32; ++b) tma_load_2d(st + b * kBoxBytes, &map_a, m0 + 32 * b, r, &full[s]);
+        tma_load_2d(st + S::kABytes, &map_g, n0, r, &full[s]);
       }
-      umma_commit(tmem_full);
-    }
-  } else if (warp >= kTransformWarp0) {
-    const int t = threadIdx.x - kTransformWarp0 * 32;
-    const int n_piece = (kMBlocks + g_blocks) * kBlockBytes / 16;     // 16-byte pieces of the raw part (A then G)
-    for (int kt = 0; kt < k_tiles; ++kt) {
-      const int s = kt % kStages;
-      const uint32_t ph = (kt / kStages) & 1;
-      mbar_wait_x(&full[s], ph, (p.dbg_skip & 8) == 0);
-      const uint32_t st = smem_u32(stage_base_of(smem, s, S::kStageBytes));
-      for (int base = (p.dbg_skip & 1) ? n_piece : 0; base < n_piece; base += 4 * kTransformThreads) {
-        float4 v[4];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const int idx = base + i * kTransformThreads + t;
-          if (idx < n_piece) v[i] = lds128(st + (uint32_t)idx * 16u);
-        }
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const int idx = base + i * kTransformThreads + t;
-          if (idx < n_piece) split_store(st + (uint32_t)idx * 16u, S::kRaw, v[i], (p.dbg_skip & 16) == 0);
-        }
-      }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&lo_ready[s]);
     }
   } else {
-    // epilogue: partial[slice][mt * 128 + row][nt * n_tile + col]
-    mbar_wait_x(tmem_full, 0, (p.dbg_skip & 8) == 0);
-    tc_fence_after();
-    const uint32_t taddr = tmem_base + ((uint32_t)(warp * 32) << 16);
-    uint8_t* wbuf = store_base + warp * (2 * 32 * kStoreCols * 4);
-    uint32_t chunk_it = 0;
-    for (int c = 0; c < p.n_tile; c += kStoreCols, ++chunk_it) {
-      const uint32_t buf = smem_u32(wbuf + (chunk_it & 1) * (32 * kStoreCols * 4));
-      uint32_t v[32];
-      asm volatile(
-          "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-          "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-          : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-            "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-            "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-            "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-          : "r"(taddr + (uint32_t)c));
-      if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-      __syncwarp();
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+    reg_alloc<232>();
+    const int ct = threadIdx.x - 128;                          // 0 .. 255
+    const int row_wg = (wgi - 1) * 64 + (warp & 3) * 16;
+    float acc[BN / 2], part[BN / 2];       // running sum, this k-tile's tensor-core sum
 #pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const uint32_t dst = buf + (uint32_t)lane * 128u + (uint32_t)((j ^ (lane & 7)) << 4);
-        sts128(dst, make_float4(__uint_as_float(v[4 * j]), __uint_as_float(v[4 * j + 1]), __uint_as_float(v[4 * j + 2]),
-                                __uint_as_float(v[4 * j + 3])));
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    for (int kt = 0; kt < k_tiles; ++kt) {
+      const int s = kt % kStages;
+      mbar_wait_hint(&full[s], (kt / kStages) & 1);
+      const uint32_t st = smem_u32(smem + s * S::kStageBytes);
+      const uint32_t g_raw = st + S::kABytes, g_hi = g_raw + S::kGRawBytes, g_lo = g_hi + S::kGBytes;
+      // G tile [BKR][BN] -> G^T hi / lo [BN][BKR]: item (n, 4 reduction rows) = one 16-byte chunk of each plane
+      for (int i = ct; i < BN * (BKR / 4); i += kConsumerThreads) {
+        const int n = i % BN, rq = i / BN;
+        float4 v;
+        v.x = lds32(g_raw + (uint32_t)((4 * rq + 0) * BN + n) * 4u);
+        v.y = lds32(g_raw + (uint32_t)((4 * rq + 1) * BN + n) * 4u);
+        v.z = lds32(g_raw + (uint32_t)((4 * rq + 2) * BN + n) * 4u);
+        v.w = lds32(g_raw + (uint32_t)((4 * rq + 3) * BN + n) * 4u);
+        float4 h;
+        h.x = tf32_rn_fast(v.x); h.y = tf32_rn_fast(v.y); h.z = tf32_rn_fast(v.z); h.w = tf32_rn_fast(v.w);
+        const uint32_t off = (uint32_t)n * 128u + (uint32_t)((rq ^ (n & 7)) << 4);
+        sts128(g_hi + off, h);
+        sts128(g_lo + off, make_float4(tf32_rn_fast(v.x - h.x), tf32_rn_fast(v.y - h.y), tf32_rn_fast(v.z - h.z),
+                                       tf32_rn_fast(v.w - h.w)));
       }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+      fence_async_smem();
+      named_barrier(1, kConsumerThreads);
+      uint32_t hi[16], lo[16];
+      load_at_split(st, row_wg, lane, hi, lo);
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) part[i] = 0.f;
+      mma_ktile_3xtf32<BN>(part, hi, lo, g_hi, g_lo);
+      wgmma_wait<0>();
       __syncwarp();
-      if (lane == 0) {
-        if (p.reduce) {   // element-wise fp32 add in L2: the slices' contributions meet in W itself, no partial buffer
-          asm volatile("cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.bulk_group [%0, {%1, %2}], [%3];"
-                       ::"l"(reinterpret_cast<uint64_t>(&map_p)), "r"(nt * p.n_tile + c), "r"(mt * BM + warp * 32), "r"(buf)
-                       : "memory");
-        } else {
-          asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%1, %2, %3}], [%4];"
-                       ::"l"(reinterpret_cast<uint64_t>(&map_p)), "r"(nt * p.n_tile + c), "r"(mt * BM + warp * 32),
-                         "r"((int)blockIdx.y), "r"(buf) : "memory");
-        }
-        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-      }
+      if (lane == 0) mbar_arrive(&empty[s]);
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[i] += part[i];
     }
-    if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-    tc_fence_before();
+    float* out = p.reduce ? p.out : p.out + (long long)blockIdx.z * p.K1 * p.N;
+    store_acc<BN>(acc, out, p.N, m0 + row_wg, p.K1, n0, p.N, lane, p.reduce != 0);
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == kMmaWarp) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(kTmemCols) : "memory");
-  }
-}
-
-// partial[slices][K1][N] (packed): 3-D map, box = [1, 32 rows, 32 columns]
-static int make_map3(CUtensorMap* map, const float* base, long long slices, long long K1, long long N) {
-  EncodeTiled enc = encode_fn();
-  if (enc == nullptr) { set_error("cuTensorMapEncodeTiled is not available from the driver"); return EQF_ERR_CUDA; }
-  cuuint64_t dims[3] = {(cuuint64_t)N, (cuuint64_t)K1, (cuuint64_t)slices};
-  cuuint64_t strides[2] = {(cuuint64_t)N * sizeof(float), (cuuint64_t)N * K1 * sizeof(float)};
-  cuuint32_t box[3] = {(cuuint32_t)kStoreCols, 32, 1};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(base), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled (3-D) failed (code " + std::to_string((int)r) + ")"); return EQF_ERR_CUDA; }
-  return EQF_OK;
 }
 
 struct Shape { int n_tile, n_tiles, m_tiles; long long slices, rows_per_slice; };
 
 static Shape plan(long long R, long long K1, long long N) {
   Shape sh;
-  sh.n_tiles = (int)((N + 255) / 256);
-  sh.n_tile = sh.n_tiles == 1 ? (int)((N + 31) & ~31LL) : 256;
+  sh.n_tiles = (int)((N + kMaxBN - 1) / kMaxBN);
+  sh.n_tile = sh.n_tiles == 1 ? (int)((N + 31) & ~31LL) : kMaxBN;
   sh.m_tiles = (int)((K1 + BM - 1) / BM);
-  int sms = 148, dev = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  const long long sms = device_sms();
   long long slices = sms / ((long long)sh.m_tiles * sh.n_tiles);     // one wave of CTAs (one CTA per SM)
   if (slices < 1) slices = 1;
   long long rps = (R + slices - 1) / slices;
@@ -1299,308 +298,25 @@ static Shape plan(long long R, long long K1, long long N) {
 }
 
 template <int BN>
-static int launch(const CUtensorMap& ma, const CUtensorMap& mg, const CUtensorMap& mp, const WParams& p, const Shape& sh,
-                  cudaStream_t s) {
+static int launch(const CUtensorMap& ma, const CUtensorMap& mg, const WParams& p, const Shape& sh, cudaStream_t s) {
   static std::once_flag once;
   static cudaError_t attr_err = cudaSuccess;
   std::call_once(once, [] {
     attr_err = cudaFuncSetAttribute(wgrad_tf32x3_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, WSmem<BN>::kTotal);
   });
   if (attr_err != cudaSuccess) return check_cuda(attr_err, "wgrad_tf32x3 smem attribute");
-  dim3 grid((unsigned)(sh.m_tiles * sh.n_tiles), (unsigned)sh.slices);
-  wgrad_tf32x3_kernel<BN><<<grid, kThreads, WSmem<BN>::kTotal, s>>>(ma, mg, mp, p);
+  dim3 grid((unsigned)sh.m_tiles, (unsigned)sh.n_tiles, (unsigned)sh.slices);
+  wgrad_tf32x3_kernel<BN><<<grid, kThreads, WSmem<BN>::kTotal, s>>>(ma, mg, p);
   return check_cuda(cudaGetLastError(), "wgrad_tf32x3_kernel launch");
 }
 
-
-// ------------------------------------------------------------------------------------------------ narrow outputs
-// N <= 64: the A^T operand goes through TENSOR memory instead of shared memory.  The kernel above splits both tiles in
-// shared memory (20 KB read + 40 KB written per 32-row stage) and every MMA re-reads its A tiles from there - shared-memory
-// bandwidth, not HBM, bounded it.  Here the A tile lands unswizzled ([32 rows][128 columns]); transform thread k1 reads
-// its COLUMN (a warp reads 32 consecutive floats per row: conflict-free), splits it in registers and stores hi / lo as
-// 32 + 32 columns of its tensor-memory lane - the transpose costs nothing, and that is the K-major layout an MMA takes
-// its A operand from.  Only the small G tile is split in shared memory, hi and lo blocks back to back so that
-// [g_hi | g_lo] is ONE MN-major operand of N' = 2 n columns (stacked as in ts::):
-//   MMA 1  a_hi x [g_hi | g_lo]   -> accumulator columns [0, n) and [n, 2n)
-//   MMA 2  a_lo x  g_hi           -> added to [0, n);   the epilogue adds the halves.
-template <int BN>
-struct WTSmem {
-  static constexpr int kABytes = BKR * BM * 4;                     // raw A tile, 512-byte rows
-  static constexpr int kGBytes = (BN / 32) * kBlockBytes;          // G hi; G lo follows
-  static constexpr int kStageBytes = kABytes + 2 * kGBytes;
-  static constexpr int kAcc = 2 * BN;
-  static constexpr int kStoreBytes = kEpilogueWarps * 2 * 32 * kStoreCols * 4;
-  static constexpr int kBudget = 227 * 1024 - 1024;
-  static constexpr int kStagesSmem = (kBudget - kStoreBytes - 1024) / kStageBytes;
-  static constexpr int kStagesTmem = (512 - kAcc) / (2 * BKR);
-  static constexpr int kStagesMin = kStagesSmem < kStagesTmem ? kStagesSmem : kStagesTmem;
-  static constexpr int kStages = kStagesMin > 8 ? 8 : kStagesMin;
-  static_assert(kStages >= 2, "tile does not fit");
-  static constexpr int kTotal = kStages * kStageBytes + kStoreBytes + 1024 + 1024;
-};
-
-// A from tensor memory (K-major by construction), B MN-major
-__device__ __forceinline__ uint32_t instr_desc_ts_mn(int n) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | (1u << 16) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-}
-
-template <int BN>
-__global__ void __launch_bounds__(kThreads, 1)
-wgrad_tf32x3_ts_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_g,
-                       const __grid_constant__ CUtensorMap map_p, WParams p) {
-  static_assert(BKR == 32, "one tcgen05.st.x32 per half");
-  using S = WTSmem<BN>;
-  constexpr int kStages = S::kStages;
-  constexpr int kTmemCols = 512;
-  constexpr int kACol0 = S::kAcc;
-  constexpr int g_blocks = BN / 32;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* store_base = smem + kStages * S::kStageBytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(store_base + S::kStoreBytes);
-  uint64_t* full = bars;
-  uint64_t* a_ready = bars + kStages;
-  uint64_t* empty = bars + 2 * kStages;
-  uint64_t* tmem_full = bars + 3 * kStages;
-  uint32_t* tmem_base_slot = reinterpret_cast<uint32_t*>(bars + 3 * kStages + 1);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int mt = blockIdx.x;                  // one column tile (n_tile == BN)
-  const long long r0 = (long long)blockIdx.y * p.rows_per_slice;
-  long long rows = p.R - r0;
-  if (rows > p.rows_per_slice) rows = p.rows_per_slice;
-  const int k_tiles = (int)((rows + BKR - 1) / BKR);
-
-  if (warp == kProducerWarp && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_a)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_g)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_p)) : "memory");
-    for (int s = 0; s < kStages; ++s) {
-      mbar_init(&full[s], 1);
-      mbar_init(&a_ready[s], kTransformWarps);
-      mbar_init(&empty[s], 1);
-    }
-    mbar_init(tmem_full, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == kMmaWarp) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_base_slot)), "n"(kTmemCols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_base_slot;
-
-  if (warp == kProducerWarp) {
-    if (lane == 0) {
-      const uint32_t tx = (uint32_t)(S::kABytes + S::kGBytes);
-      for (int kt = 0; kt < k_tiles; ++kt) {
-        const int s = kt % kStages;
-        const uint32_t ph = (kt / kStages) & 1;
-        mbar_wait_x(&empty[s], ph ^ 1, (p.dbg_skip & 8) == 0);
-        uint8_t* st = stage_base_of(smem, s, S::kStageBytes);
-        mbar_expect_tx(&full[s], tx);
-        const int row = (int)(r0 + (long long)kt * BKR);
-        tma_load_2d(st, &map_a, mt * BM, row, &full[s]);
-        for (int j = 0; j < g_blocks; ++j) tma_load_2d(st + S::kABytes + j * kBlockBytes, &map_g, 32 * j, row, &full[s]);
-      }
-    }
-  } else if (warp == kMmaWarp) {
-    if (lane == 0) {
-      const uint32_t idesc = instr_desc_ts_mn(BN), idesc2 = instr_desc_ts_mn(2 * BN);
-      for (int kt = 0; kt < k_tiles; ++kt) {
-        const int s = kt % kStages;
-        const uint32_t ph = (kt / kStages) & 1;
-        mbar_wait_x(&a_ready[s], ph, (p.dbg_skip & 8) == 0);
-        tc_fence_after();
-        const uint32_t st = smem_u32(stage_base_of(smem, s, S::kStageBytes));
-        const uint32_t a_hi = tmem_base + (uint32_t)(kACol0 + s * 2 * BKR), a_lo = a_hi + BKR;
-#pragma unroll
-        for (int kb = 0; kb < BKR / UMMA_K; ++kb) {
-          if (p.dbg_skip & 2) break;
-          const uint64_t g = smem_desc_mn(st + S::kABytes + (uint32_t)kb * 1024u);    // [g_hi | g_lo], next 8-row group
-          const uint32_t acol = (uint32_t)(kb * UMMA_K);
-          ts::umma_tf32_ts(tmem_base, a_hi + acol, g, idesc2, (kt > 0 || kb > 0) ? 1u : 0u);
-          ts::umma_tf32_ts(tmem_base, a_lo + acol, g, idesc, 1u);
-        }
-        umma_commit(&empty[s]);
-      }
-      umma_commit(tmem_full);
-    }
-  } else if (warp >= kTransformWarp0) {
-    const int t = threadIdx.x - kTransformWarp0 * 32;          // index for the G pieces
-    const int col = (warp & 3) * 32 + lane;                    // column of the A tile = tensor-memory lane (a warp owns
-    const uint32_t lane_field = (uint32_t)((warp & 3) * 32) << 16;   // the lane quarter 32 (warp % 4))
-    constexpr int n_piece = g_blocks * kBlockBytes / 16;
-    for (int kt = 0; kt < k_tiles; ++kt) {
-      const int s = kt % kStages;
-      const uint32_t ph = (kt / kStages) & 1;
-      mbar_wait_x(&full[s], ph, (p.dbg_skip & 8) == 0);
-      const uint32_t st = smem_u32(stage_base_of(smem, s, S::kStageBytes));
-      if (!(p.dbg_skip & 1)) {
-        const uint32_t gbase = st + S::kABytes;
-        float4 v[n_piece / kTransformThreads];
-#pragma unroll
-        for (int i = 0; i < n_piece / kTransformThreads; ++i) v[i] = lds128(gbase + (uint32_t)(i * kTransformThreads + t) * 16u);
-#pragma unroll
-        for (int i = 0; i < n_piece / kTransformThreads; ++i)
-          split_store(gbase + (uint32_t)(i * kTransformThreads + t) * 16u, S::kGBytes, v[i], (p.dbg_skip & 16) == 0);
-        float hi[BKR], lo[BKR];
-#pragma unroll
-        for (int r = 0; r < BKR; ++r) {
-          float x;
-          asm volatile("ld.shared.f32 %0, [%1];" : "=f"(x) : "r"(st + (uint32_t)(r * BM * 4 + col * 4)));
-          hi[r] = (p.dbg_skip & 16) ? tf32_rn(x) : tf32_rn_fast(x);
-          lo[r] = x - hi[r];
-        }
-        const uint32_t acol = tmem_base + lane_field + (uint32_t)(kACol0 + s * 2 * BKR);
-        ts::tmem_st32(acol, hi);
-        ts::tmem_st32(acol + BKR, lo);
-        asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-      }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&a_ready[s]);
-    }
-  } else {
-    mbar_wait_x(tmem_full, 0, (p.dbg_skip & 8) == 0);
-    tc_fence_after();
-    const uint32_t taddr = tmem_base + ((uint32_t)(warp * 32) << 16);
-    uint8_t* wbuf = store_base + warp * (2 * 32 * kStoreCols * 4);
-    uint32_t chunk_it = 0;
-    for (int c = 0; c < BN; c += kStoreCols, ++chunk_it) {
-      const uint32_t buf = smem_u32(wbuf + (chunk_it & 1) * (32 * kStoreCols * 4));
-      uint32_t v[32], v2[32];
-      asm volatile(
-          "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-          "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-          : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-            "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-            "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-            "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-          : "r"(taddr + (uint32_t)c));
-      asm volatile(
-          "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-          "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-          : "=r"(v2[0]), "=r"(v2[1]), "=r"(v2[2]), "=r"(v2[3]), "=r"(v2[4]), "=r"(v2[5]), "=r"(v2[6]), "=r"(v2[7]),
-            "=r"(v2[8]), "=r"(v2[9]), "=r"(v2[10]), "=r"(v2[11]), "=r"(v2[12]), "=r"(v2[13]), "=r"(v2[14]), "=r"(v2[15]),
-            "=r"(v2[16]), "=r"(v2[17]), "=r"(v2[18]), "=r"(v2[19]), "=r"(v2[20]), "=r"(v2[21]), "=r"(v2[22]), "=r"(v2[23]),
-            "=r"(v2[24]), "=r"(v2[25]), "=r"(v2[26]), "=r"(v2[27]), "=r"(v2[28]), "=r"(v2[29]), "=r"(v2[30]), "=r"(v2[31])
-          : "r"(taddr + (uint32_t)(BN + c)));
-      if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-      __syncwarp();
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-      for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(__uint_as_float(v[j]) + __uint_as_float(v2[j]));
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const uint32_t dst = buf + (uint32_t)lane * 128u + (uint32_t)((j ^ (lane & 7)) << 4);
-        sts128(dst, make_float4(__uint_as_float(v[4 * j]), __uint_as_float(v[4 * j + 1]), __uint_as_float(v[4 * j + 2]),
-                                __uint_as_float(v[4 * j + 3])));
-      }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) {
-        if (p.reduce) {
-          asm volatile("cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.bulk_group [%0, {%1, %2}], [%3];"
-                       ::"l"(reinterpret_cast<uint64_t>(&map_p)), "r"(c), "r"(mt * BM + warp * 32), "r"(buf) : "memory");
-        } else {
-          asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%1, %2, %3}], [%4];"
-                       ::"l"(reinterpret_cast<uint64_t>(&map_p)), "r"(c), "r"(mt * BM + warp * 32), "r"((int)blockIdx.y), "r"(buf)
-                       : "memory");
-        }
-        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-      }
-    }
-    if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-    tc_fence_before();
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == kMmaWarp) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(kTmemCols) : "memory");
-  }
-}
-
-template <int BN>
-static int launch_ts(const CUtensorMap& ma, const CUtensorMap& mg, const CUtensorMap& mp, const WParams& p, const Shape& sh,
-                     cudaStream_t s) {
-  static std::once_flag once;
-  static cudaError_t attr_err = cudaSuccess;
-  std::call_once(once, [] {
-    attr_err = cudaFuncSetAttribute(wgrad_tf32x3_ts_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, WTSmem<BN>::kTotal);
-  });
-  if (attr_err != cudaSuccess) return check_cuda(attr_err, "wgrad_tf32x3_ts smem attribute");
-  dim3 grid((unsigned)sh.m_tiles, (unsigned)sh.slices);
-  wgrad_tf32x3_ts_kernel<BN><<<grid, kThreads, WTSmem<BN>::kTotal, s>>>(ma, mg, mp, p);
-  return check_cuda(cudaGetLastError(), "wgrad_tf32x3_ts_kernel launch");
-}
-
 }  // namespace wg
-template <int BN, bool STACK>
-static int launch_ts(const CUtensorMap& ma, const CUtensorMap& mh, const CUtensorMap& ml, const CUtensorMap& mc,
-                     const Params& p, cudaStream_t s) {
-  static std::once_flag once;
-  static cudaError_t attr_err = cudaSuccess;
-  std::call_once(once, [] {
-    attr_err = cudaFuncSetAttribute(ts::gemm_tf32x3_ts_kernel<BN, STACK>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    ts::TSmem<BN, STACK>::kTotal);
-  });
-  if (attr_err != cudaSuccess) return check_cuda(attr_err, "gemm_tf32x3_ts smem attribute");
-  int sms = 148, dev = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  const long long tiles = p.m_blocks * p.n_blocks;
-  const int grid = (int)(tiles < sms ? tiles : sms);
-  ts::gemm_tf32x3_ts_kernel<BN, STACK><<<grid, kThreads, ts::TSmem<BN, STACK>::kTotal, s>>>(ma, mh, ml, mc, p);
-  return check_cuda(cudaGetLastError(), "gemm_tf32x3_ts_kernel launch");
-}
-
-// CTA-pair launch: clusters of two CTAs, one cluster per TPC
-template <int BN>
-static int launch_ts2(const CUtensorMap& ma, const CUtensorMap& mh, const CUtensorMap& ml, const CUtensorMap& mhalf,
-                      const CUtensorMap& mc, const Params& p, cudaStream_t s) {
-  static std::once_flag once;
-  static cudaError_t attr_err = cudaSuccess;
-  std::call_once(once, [] {
-    attr_err = cudaFuncSetAttribute(ts2::gemm_tf32x3_ts2_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    ts2::T2Smem<BN>::kTotal);
-  });
-  if (attr_err != cudaSuccess) return check_cuda(attr_err, "gemm_tf32x3_ts2 smem attribute");
-  int sms = 148, dev = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  const long long tiles = ((p.M + 2 * BM - 1) / (2 * BM)) * p.n_blocks;
-  const long long pairs = tiles < sms / 2 ? tiles : sms / 2;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)(2 * pairs));
-  cfg.blockDim = dim3(kThreads);
-  cfg.dynamicSmemBytes = ts2::T2Smem<BN>::kTotal;
-  cfg.stream = s;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  return check_cuda(cudaLaunchKernelEx(&cfg, ts2::gemm_tf32x3_ts2_kernel<BN>, ma, mh, ml, mhalf, mc, p),
-                    "gemm_tf32x3_ts2_kernel launch");
-}
-
 }  // namespace tf32x3
 }  // namespace eqf
 
 using namespace eqf;
 
-static long long* g_tf32x3_dbg = nullptr;
-// debugging aid: device buffer of 4 * 1024 int64 that receives CTA 0's clock64 timeline on the next launches (NULL = off)
-extern "C" void eqf_gemm_tf32x3_set_timeline(long long* device_buffer) { g_tf32x3_dbg = device_buffer; }
-
-// C[M, N] = A[M, K] (row-major, lda) x W, 3xTF32 on tcgen05.  The weight operand is either Bt[N, K] (b_is_kn = 0, row
+// C[M, N] = A[M, K] (row-major, lda) x W, 3xTF32 on wgmma.  The weight operand is either Bt[N, K] (b_is_kn = 0, row
 // stride ldb >= K: data gradient, W = Bt^T) or B[K, N] (b_is_kn = 1, row stride ldb >= N: forward, W = B).  `split` is
 // device scratch of 2 * N * K floats for its hi / lo planes.  Pointers 16-byte aligned, K, lda, ldc multiples of 4.
 extern "C" int eqf_gemm_tf32x3(const float* A, const float* Bt, float* C, int64_t M, int64_t N, int64_t K, int64_t lda,
@@ -1614,60 +330,39 @@ extern "C" int eqf_gemm_tf32x3(const float* A, const float* Bt, float* C, int64_
     set_error("eqf_gemm_tf32x3: operands must be 16-byte aligned, K and leading dimensions multiples of 4");
     return EQF_ERR_INVALID;
   }
+  if (K > 0x7fffffffLL || N > 0x7fffffffLL) { set_error("eqf_gemm_tf32x3: K / N too large"); return EQF_ERR_UNSUPPORTED; }
   cudaStream_t s = (cudaStream_t)stream;
-  // hi / lo planes of the weights, packed [N, K] (loading precomputed planes costs L2 bandwidth; splitting the raw
-  // tile in shared memory instead was tried and lost: the transform's shared-memory traffic became the limiter)
   float* hi = split;
   float* lo = split + N * K;
   {
     const long long n = N * K;
-    const unsigned blocks = (unsigned)((n + 255) / 256 < 1184 ? (n + 255) / 256 : 1184);
+    const unsigned blocks = (unsigned)((n + 255) / 256 < 1056 ? (n + 255) / 256 : 1056);
     if (b_is_kn) split_transpose_kernel<<<blocks, 256, 0, s>>>(Bt, ldb, hi, lo, N, K);
     else if (ldb == K) split_kernel<<<blocks, 256, 0, s>>>(Bt, hi, lo, n);
     else { set_error("eqf_gemm_tf32x3: Bt must be packed (ldb == K)"); return EQF_ERR_UNSUPPORTED; }
   }
   int rc = check_cuda(cudaGetLastError(), "split_kernel launch");
   if (rc != EQF_OK) return rc;
-  // column tiles: one tile of round_up(N, 16) columns when N <= 256 (out-of-range weight rows load as zeros,
-  // out-of-range columns are clipped by the TMA store), else
-  const int n_blocks = (int)((N + 255) / 256);
-  // several column tiles: as even as possible in multiples of 32 (the store chunk), e.g. 384 -> 192 + 192, 352 -> 192 + 160
-  const int n_tile = n_blocks == 1 ? (int)((N + 15) & ~15LL) : (int)((((N + n_blocks - 1) / n_blocks) + 31) & ~31LL);
+  // column tiles: as even as possible, at most 128 columns (two register accumulators per thread), rounded up to the
+  // instantiated widths
+  const long long n_split = (N + 127) / 128;
+  const long long per = (N + n_split - 1) / n_split;
+  const int bn = per <= 32 ? 32 : per <= 64 ? 64 : per <= 96 ? 96 : 128;
+  const int n_blocks = (int)((N + bn - 1) / bn);
+  const long long m_blocks = (M + BM - 1) / BM;
   Params p;
-  p.C = C; p.M = M; p.N = N; p.K = K; p.ldc = ldc; p.n_tile = n_tile; p.n_blocks = (int)((N + n_tile - 1) / n_tile);
-  p.m_blocks = (M + BM - 1) / BM;
-  p.dbg = g_tf32x3_dbg;
-  { const char* e = std::getenv("EQF_TF32X3_DBG_SKIP"); p.dbg_skip = e ? std::atoi(e) : 0; }
-  CUtensorMap ma, mh, ml, mc;
-  if ((rc = make_map(&ma, A, M, K, lda, BM, BK)) != EQF_OK) return rc;
-  if ((rc = make_map(&mh, hi, N, K, K, n_tile, BK)) != EQF_OK) return rc;
-  if ((rc = make_map(&ml, lo, N, K, K, n_tile, BK)) != EQF_OK) return rc;
-  if ((rc = make_map(&mc, C, M, N, ldc, 32, kStoreCols)) != EQF_OK) return rc;
-  // narrow outputs: A operand from TMEM, 128-byte k-tiles (EQF_TF32X3_TS=0 selects the shared-memory variant everywhere)
-  static const bool use_ts = [] { const char* e = std::getenv("EQF_TF32X3_TS"); return e == nullptr || e[0] != '0'; }();
-  if (use_ts && n_tile <= 128) {
-    if ((rc = make_map(&ma, A, M, K, lda, BM, ts::BKT)) != EQF_OK) return rc;
-    if ((rc = make_map(&mh, hi, N, K, K, n_tile, ts::BKT)) != EQF_OK) return rc;
-    if ((rc = make_map(&ml, lo, N, K, K, n_tile, ts::BKT)) != EQF_OK) return rc;
-    static const bool stack = [] { const char* e = std::getenv("EQF_TF32X3_STACK"); return e == nullptr || e[0] != '0'; }();
-    // CTA-pair variant (EQF_TF32X3_2SM=1; off by default): one M = 256 instruction pair per 256 rows
-    const char* pair_env = std::getenv("EQF_TF32X3_2SM");
-    if (stack && pair_env != nullptr && pair_env[0] == '1' && (n_tile == 32 || n_tile == 64) && N == n_tile) {
-      CUtensorMap mhalf;
-      if ((rc = make_map(&mhalf, hi, N, K, K, n_tile / 2, ts::BKT)) != EQF_OK) return rc;
-      return n_tile == 32 ? launch_ts2<32>(ma, mh, ml, mhalf, mc, p, s) : launch_ts2<64>(ma, mh, ml, mhalf, mc, p, s);
-    }
-    if (stack && n_tile == 32) return launch_ts<32, true>(ma, mh, ml, mc, p, s);
-    if (stack && n_tile == 64) return launch_ts<64, true>(ma, mh, ml, mc, p, s);
-    if (n_tile <= 32) return launch_ts<32, false>(ma, mh, ml, mc, p, s);
-    if (n_tile <= 64) return launch_ts<64, false>(ma, mh, ml, mc, p, s);
-    return launch_ts<128, false>(ma, mh, ml, mc, p, s);
+  p.C = C; p.M = M; p.ldc = ldc; p.N = (int)N; p.K = (int)K;
+  CUtensorMap ma, mh, ml;
+  if ((rc = make_map_2d(&ma, A, M, K, lda, BM, BK)) != EQF_OK) return rc;
+  if ((rc = make_map_2d(&mh, hi, N, K, K, bn, BK)) != EQF_OK) return rc;
+  if ((rc = make_map_2d(&ml, lo, N, K, K, bn, BK)) != EQF_OK) return rc;
+  switch (bn) {
+    case 32: return launch<32>(ma, mh, ml, p, m_blocks, n_blocks, s);
+    case 64: return launch<64>(ma, mh, ml, p, m_blocks, n_blocks, s);
+    case 96: return launch<96>(ma, mh, ml, p, m_blocks, n_blocks, s);
+    default: return launch<128>(ma, mh, ml, p, m_blocks, n_blocks, s);
   }
-  if (n_tile <= 64) return launch<64>(ma, mh, ml, mc, p, s);
-  if (n_tile <= 128) return launch<128>(ma, mh, ml, mc, p, s);
-  return launch<256>(ma, mh, ml, mc, p, s);
 }
-
 
 // number of row slices eqf_gemm_tf32x3_wgrad will use (= leading dimension of its `partial` scratch [slices, K1, N])
 extern "C" int64_t eqf_gemm_tf32x3_wgrad_slices(int64_t R, int64_t K1, int64_t N) {
@@ -1684,38 +379,26 @@ static int wgrad_impl(const float* A, const float* G, float* out, bool reduce, i
     set_error(std::string(who) + ": operands must be 16-byte aligned, dimensions multiples of 4");
     return EQF_ERR_INVALID;
   }
-  if (R > 0x7fffffffLL) { set_error(std::string(who) + ": too many rows"); return EQF_ERR_UNSUPPORTED; }
+  if (R > 0x7fffffffLL || K1 > 0x7fffffffLL || N > 0x7fffffffLL) {
+    set_error(std::string(who) + ": too many rows");
+    return EQF_ERR_UNSUPPORTED;
+  }
   const wg::Shape sh = wg::plan(R, K1, N);
   wg::WParams p;
-  p.R = R; p.rows_per_slice = sh.rows_per_slice; p.n_tile = sh.n_tile; p.n_tiles = sh.n_tiles; p.reduce = reduce ? 1 : 0;
-  { const char* e = std::getenv("EQF_TF32X3_DBG_SKIP"); p.dbg_skip = e ? std::atoi(e) : 0; }
-  CUtensorMap ma, mg, mp;
+  p.out = out; p.R = R; p.rows_per_slice = sh.rows_per_slice; p.K1 = K1; p.N = (int)N; p.reduce = reduce ? 1 : 0;
+  CUtensorMap ma, mg;
   int rc;
-  if ((rc = make_map(&ma, A, R, K1, lda, wg::BKR, 32, true)) != EQF_OK) return rc;
-  if ((rc = make_map(&mg, G, R, N, ldg, wg::BKR, 32, true)) != EQF_OK) return rc;
+  if ((rc = make_map_2d(&ma, A, R, K1, lda, wg::BKR, 32)) != EQF_OK) return rc;
+  if ((rc = make_map_2d(&mg, G, R, N, ldg, wg::BKR, sh.n_tile, MapKind::kLinear)) != EQF_OK) return rc;
   cudaStream_t s = (cudaStream_t)stream;
-  if (reduce) {
-    if ((rc = check_cuda(cudaMemsetAsync(out, 0, (size_t)K1 * N * sizeof(float), s), "wgrad memset")) != EQF_OK) return rc;
-    if ((rc = make_map(&mp, out, K1, N, N, 32, kStoreCols)) != EQF_OK) return rc;
-  } else {
-    if ((rc = wg::make_map3(&mp, out, sh.slices, K1, N)) != EQF_OK) return rc;
-  }
-  // narrow outputs: A^T through tensor memory (wg::wgrad_tf32x3_ts_kernel; EQF_TF32X3_WGRAD_TS=0 keeps the
-  // shared-memory kernel): 89.9 -> 60.1 us on [162 800, 352]^T x 32, 63.0 -> 43.5 us on [97 680, 384]^T x 64
-  const char* wts = std::getenv("EQF_TF32X3_WGRAD_TS");
-  // EQF_TF32X3_WGRAD_TS=2 extends it to 128 columns (4 stages fit tensor memory there) - built, NOT yet measured or
-  // covered by the GPU tests: next round's first experiment (tools/tf32x3_wgrad_ts_check.py has the cases)
-  const int ts_max = (wts != nullptr && wts[0] == '2') ? 128 : 64;
-  if ((wts == nullptr || wts[0] != '0') && sh.n_tiles == 1 && sh.n_tile <= ts_max) {
-    if ((rc = make_map(&ma, A, R, K1, lda, wg::BKR, BM, false, true)) != EQF_OK) return rc;
-    if (sh.n_tile == 32) return wg::launch_ts<32>(ma, mg, mp, p, sh, s);
-    if (sh.n_tile == 64) return wg::launch_ts<64>(ma, mg, mp, p, sh, s);
-    return wg::launch_ts<128>(ma, mg, mp, p, sh, s);
-  }
-  if (sh.n_tile <= 32) return wg::launch<32>(ma, mg, mp, p, sh, s);
-  if (sh.n_tile <= 64) return wg::launch<64>(ma, mg, mp, p, sh, s);
-  if (sh.n_tile <= 128) return wg::launch<128>(ma, mg, mp, p, sh, s);
-  return wg::launch<256>(ma, mg, mp, p, sh, s);
+  // W is zeroed and every slice's CTA adds its contribution (the order of the slices' additions is not fixed, so the last
+  // bits may differ between runs - like the atomic scatter of the reference)
+  if (reduce && (rc = check_cuda(cudaMemsetAsync(out, 0, (size_t)K1 * N * sizeof(float), s), "wgrad memset")) != EQF_OK)
+    return rc;
+  if (sh.n_tile <= 32) return wg::launch<32>(ma, mg, p, sh, s);
+  if (sh.n_tile <= 64) return wg::launch<64>(ma, mg, p, sh, s);
+  if (sh.n_tile <= 96) return wg::launch<96>(ma, mg, p, sh, s);
+  return wg::launch<128>(ma, mg, p, sh, s);
 }
 
 // partial[s] = A[rows of slice s, :K1]^T G[rows of slice s, :N]  for every slice s; the weight gradient is the sum over s
@@ -1725,9 +408,8 @@ extern "C" int eqf_gemm_tf32x3_wgrad(const float* A, const float* G, float* part
   return wgrad_impl(A, G, partial, false, R, K1, N, lda, ldg, stream, "eqf_gemm_tf32x3_wgrad");
 }
 
-// W[K1, N] (packed) = A^T G directly: W is zeroed and every slice's CTA adds its contribution with a TMA reduce-add
-// (fp32 adds in L2; the order of the slices' additions is not fixed, so the last bits may differ between runs - like
-// the atomic scatter of the reference).  One launch + one memset instead of partials + column sum.
+// W[K1, N] (packed) = A^T G directly: W is zeroed and every slice's CTA adds its contribution with fp32 atomics.
+// One launch + one memset instead of partials + column sum.
 extern "C" int eqf_gemm_tf32x3_wgrad_accumulate(const float* A, const float* G, float* W, int64_t R, int64_t K1, int64_t N,
                                                 int64_t lda, int64_t ldg, void* stream) {
   return wgrad_impl(A, G, W, true, R, K1, N, lda, ldg, stream, "eqf_gemm_tf32x3_wgrad_accumulate");

@@ -1,9 +1,9 @@
-// eqf_pointwise.cu - fused per-edge pointwise kernels around the GEMMs of the attention path (sm_100a).
+// eqf_pointwise.cu - fused per-edge pointwise kernels around the GEMMs of the attention path (sm_90a).
 //
 // Reference work replaced:
 //   * RadialProfile's hidden layers (nets/radial_func.py:24-35): LayerNorm -> SiLU on [E, 64] after each Linear -
-//     eager: native_layer_norm + silu (+ in backward layer_norm_backward whose gamma/beta reduction alone cost 240 us
-//     per call on B200, profiles/r1_launches_all_kernels_v2.csv) -> ln_silu_{fwd,bwd}_kernel, one warp per row;
+//     eager: native_layer_norm + silu (+ in backward layer_norm_backward with its separate gamma/beta reduction)
+//     -> ln_silu_{fwd,bwd}_kernel, one warp per row;
 //   * the middle of GraphAttention.forward (nets/graph_attention_transformer.py:492-495,506-507): bias adds, the Gate
 //     (SiLU on scalars, sigmoid gates x gated irreps, e3nn normalize2mom constants) and the attention logits
 //     (SmoothLeakyReLU . alpha_dot) -> gate_logits_{fwd,bwd}_kernel, one warp per edge;
@@ -22,7 +22,7 @@ __device__ __forceinline__ float sigmoidf_(float x) { return 1.f / (1.f + expf(-
 // ------------------------------------------------------------------------------------------------ LayerNorm + SiLU
 // y = silu(z), z = (x - mean) * rstd * gamma + beta ; C <= 32 * kMaxPerLane, one warp per row.  The kernels are
 // instantiated for 2 / 4 / 8 columns per lane: at C = 64 (the radial MLP) the 8-column version carried 102 registers
-// for six live arrays it did not need - 2 CTAs per SM and a latency-bound 42 us per call (profiles launch list).
+// for six live arrays it did not need - 2 CTAs per SM and a latency-bound kernel.
 constexpr int kMaxPerLane = 8;
 
 template <int PER>
@@ -127,7 +127,7 @@ __global__ void __launch_bounds__(256) ln_silu_bwd_kernel(const float* __restric
 }
 
 // C == 64 (the radial MLP): half a warp per row, one float4 per lane - two rows in flight per warp, a quarter of the
-// memory instructions and 4-step reductions; the generic kernels above spent 18-23 us per call on latency.
+// memory instructions and 4-step reductions; the generic kernels above are latency bound at this width.
 __device__ __forceinline__ float hsum16(float v) {
 #pragma unroll
   for (int o = 8; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -552,8 +552,7 @@ static bool gate_vec_ok(const GateArgs& a) {
 
 // ------------------------------------------------------------------------------------------------ column sum
 // out[c] = sum_r x[r, c]: bias / offset gradients (sum over all edges), reduction of per-CTA partial rows and of the
-// sliced weight-gradient partials.  torch's reduce_kernel ran these at 1-2 TB/s (a single CTA for the narrow ones):
-// 201 launches, 4.1 ms of a 27 ms step (profiles/r1_launches_final.csv).  Threads run along the columns (coalesced,
+// sliced weight-gradient partials (torch's reduce_kernel runs the narrow ones on a single CTA).  Threads run along the columns (coalesced,
 // float4 when aligned), rows are split over blockIdx.y; the last CTA to finish a column tile adds the partial rows in
 // a fixed order (deterministic) and resets the tile's counter, so the buffer is reusable without a memset.
 template <int VEC>
@@ -644,7 +643,7 @@ __global__ void __launch_bounds__(256) colsum_kernel(const float* __restrict__ x
 
 static void colsum_shape(long long rows, long long cols, int vec, long long& tiles, long long& splits) {
   tiles = (cols + 32 * vec - 1) / (32 * vec);
-  splits = (148LL * 4) / tiles;                     // ~4 CTAs per SM in flight ...
+  splits = (132LL * 4) / tiles;                     // ~4 CTAs per SM in flight ...
   const long long max_splits = (rows + 63) / 64;    // ... each with at least 64 rows (8 per row group)
   if (splits > max_splits) splits = max_splits;
   if (splits > 256) splits = 256;                   // bounds the final pass (32 partial rows per row group)
@@ -761,7 +760,7 @@ __global__ void __launch_bounds__(256) eln_bwd_kernel(ELNArgs a) {
 
 static int eln_grid(long long rows, int n_entries = 1) {
   long long blocks = (rows * n_entries + 7) / 8;
-  if (blocks > 148LL * 4) blocks = 148LL * 4;
+  if (blocks > 132LL * 4) blocks = 132LL * 4;
   return (int)(blocks < 1 ? 1 : blocks);
 }
 
@@ -783,7 +782,7 @@ static int fill_eln(const EqfNormLayout* lay, ELNArgs& a) {
 
 static int pointwise_grid(long long rows) {
   long long blocks = (rows + 7) / 8;
-  const long long cap = 148LL * 8;
+  const long long cap = 132LL * 8;
   if (blocks > cap) blocks = cap;
   return (int)(blocks < 1 ? 1 : blocks);
 }

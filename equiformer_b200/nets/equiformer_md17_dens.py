@@ -5,7 +5,7 @@ spherical harmonics scaled by ``|F| / sqrt(3)`` and added to the node embeddings
 reads the scalar channels of a wider equivariant feature (``512x0e+256x1e+128x2e``); a ``GraphAttention`` head
 (``denoising_pos_head``, output ``1x1e``) predicts the position noise of the corrupted atoms, returned in place of their
 forces.  Same constructor arguments, attribute / ``state_dict`` names and ``forward(data)`` contract; every edge-level op
-is the hot path of this package (planar blocks, sm_100a kernels, closed autograd families for the ``create_graph`` forces).
+is the hot path of this package (planar blocks, sm_90a kernels, closed autograd families for the ``create_graph`` forces).
 """
 from __future__ import annotations
 

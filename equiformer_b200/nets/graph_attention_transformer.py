@@ -6,7 +6,7 @@ is the body of the per-edge hot path (``GraphAttention.forward``, reference ``:4
 
 * edge tensors stay in the planar (channel-innermost, one buffer per degree) layout from the merge linears to
   the aggregated node output; the head reshapes ``Vec2AttnHeads`` / ``AttnHeads2Vec`` become index arithmetic;
-* both depth-wise tensor products run on the sm_100a kernels of ``csrc/eqf_dtp.cu`` (forward, and the hand
+* both depth-wise tensor products run on the sm_90a kernels of ``csrc/eqf_dtp.cu`` (forward, and the hand
   derived gradient family, twice differentiable);
 * softmax over destination segments and the attention-weighted scatter run on ``csrc/eqf_attn.cu`` over the
   destination-sorted edge list (no atomics);

@@ -4,7 +4,7 @@ boundary conditions, 84 atom types plus a tag embedding (0 sub-surface, 1 surfac
 Same constructor arguments, attribute / ``state_dict`` names and ``forward(data)`` contract as the reference
 (``:72-117``, ``:296-380``); ``data`` is any object with ``pos, batch, atomic_numbers, tags, cell`` (+ ``edge_index,
 cell_offsets`` when ``otf_graph=False``).  What the reference gets from ``ocpmodels`` - ``radius_graph_pbc`` and
-``get_pbc_distances`` (``:267-302``) - is ``equiformer_b200.graph.radius_graph_pbc`` here: two sm_100a kernels around one
+``get_pbc_distances`` (``:267-302``) - is ``equiformer_b200.graph.radius_graph_pbc`` here: two sm_90a kernels around one
 prefix sum, destination-sorted, same pair / image order and the same distance masks.  The energy head is the feed-forward
 one of the shipped IS2RE configurations; the auxiliary-task and attention heads (``use_auxiliary_task``,
 ``use_attention_head``), learned node attributes and atom-pair edge attributes are outside the benchmarked path and raise.

@@ -22,9 +22,8 @@ def hoist_first_layers(modules, x: torch.Tensor):
     embedding's on the same ``[E, number_of_basis]`` embedding - 7 per QM9 step: 7 products ``[E, 128] x [128, 64]`` that each
     re-read the input, 7 data-gradient products whose results are summed, 7 weight-gradient reductions over all edges.
     Stacking the weights gives one ``[E, 128] x [128, 7 * 64]`` product each way; the modules pick their column block up in
-    ``forward`` (same parameters, same ``state_dict``).  Returns the modules it served.  Measured on one box: QM9 step
-    14.72 -> 14.58 ms, OC20 22.27 -> 22.17 ms; the MD17 energy + force step (2 100 edges, second-order graph) got SLOWER, 41.7 ->
-    45.4 ms, so the MD17 / DeNS models do not hoist (profiles/r2_bench_*_hoist*_c23.json)."""
+    ``forward`` (same parameters, same ``state_dict``).  Returns the modules it served.  The QM9 and OC20 steps gain from
+    it; the MD17 energy + force step (2 100 edges, second-order graph) got slower, so the MD17 / DeNS models do not hoist."""
     from .. import ops
     if not _HOIST or not ops.fused_ok(x) or x.dim() != 2:
         return []

@@ -2,7 +2,7 @@
 
 Same classes, constructor arguments, attributes (``.tp``, ``.irreps_*``, ``.slices_sqrt_k``, ``.bias``) and
 ``state_dict`` keys as the reference; the tensor product underneath is
-:class:`equiformer_b200.o3.TensorProduct`, i.e. the sm_100a depth-wise kernels for ``'uvu'`` and planar
+:class:`equiformer_b200.o3.TensorProduct`, i.e. the sm_90a depth-wise kernels for ``'uvu'`` and planar
 per-degree GEMMs for the scalar-``in2`` ``'uvw'`` case.
 
 Behaviour restated from the reference (not copied):

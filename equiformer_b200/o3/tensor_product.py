@@ -4,7 +4,7 @@ Same constructor surface as ``e3nn.o3.TensorProduct`` (0.4.4) for the two instru
 reference instantiates through ``TensorProductRescale`` (``nets/tensor_product_rescale.py:33-37``):
 
 * weighted ``'uvu'`` with multiplicity-1 second operand - the depth-wise tensor product; executed by
-  the sm_100a kernels in ``csrc/eqf_dtp.cu`` (no other implementation exists here);
+  the sm_90a kernels in ``csrc/eqf_dtp.cu`` (no other implementation exists here);
 * weighted ``'uvw'`` whose second operand is scalar (``1x0e`` node attributes / the constant 1 of
   ``LinearRS``) - a per-degree dense channel mix, executed as row-major GEMMs on planar blocks.
 
@@ -167,7 +167,7 @@ class TensorProduct(torch.nn.Module):
 
     # ------------------------------------------------------------------ planar entry points
     def planar_depthwise(self, xs, y, weight=None):
-        """Planar DTP: in1 blocks ``[E, 2l+1, mul]`` -> output groups ``[E, 2l+1, K]`` (sm_100a kernels)."""
+        """Planar DTP: in1 blocks ``[E, 2l+1, mul]`` -> output groups ``[E, 2l+1, K]`` (sm_90a kernels)."""
         from .. import ops
         w = self._get_weights(weight)
         return ops.depthwise_tensor_product(self.plan, xs, y, w)

@@ -1,4 +1,4 @@
-"""Autograd operators over the sm_100a edge kernels (``libeqf_b200.so``).
+"""Autograd operators over the sm_90a edge kernels (``libeqf_b200.so``).
 
 Two closed families (every derivative of a member is another member, so ``create_graph=True`` -
 the MD17 force path, ``nets/graph_attention_transformer_md17.py:318-325`` - works to any order):
@@ -30,7 +30,7 @@ from .plan import DtpPlan
 def _require_cuda(t: torch.Tensor, name: str) -> torch.Tensor:
     if not t.is_cuda:
         raise _lib.EqfError(
-            f"{name} lives on {t.device}: the equiformer_b200 edge kernels are CUDA-only (sm_100a); "
+            f"{name} lives on {t.device}: the equiformer_b200 edge kernels are CUDA-only (sm_90a); "
             "there is no CPU fallback on the product path")
     if t.dtype != torch.float32:
         raise _lib.EqfError(f"{name} must be float32 (the reference trains in fp32), got {t.dtype}")
@@ -561,10 +561,9 @@ def depthwise_tensor_product_gathered(plan: DtpPlan, graph: "Graph", As, Bs, y, 
 # ----------------------------------------------------------------------------- K1: DTP fused into the per-degree linear
 
 # EQF_FUSED: "1" fused forward everywhere, "0" the round-1 pipeline (DTP -> [E, 3136] in HBM -> GEMMs), "auto" (default) by
-# size.  MEASURED (profiles/r2_fused_fwd_*): the fused forward keeps the [E, 3136] products out of HBM and out of the saved
-# activations - the 10 k-atom periodic cell (E = 5e5) trains under CUDA-graph capture in 224 ms / step with it and runs out
-# of the 180 GB without - but its producer warps are latency bound (gathers + per-k-tile handshakes: 157 vs 124 us on the
-# Lmax = 2 group of the QM9 batch), so below _FUSED_MIN_EDGES the faster unfused pipeline is kept.
+# size.  The fused forward keeps the [E, 3136] products out of HBM and out of the saved activations - what lets large
+# periodic cells (E ~ 5e5) train at all - but its producer warps are latency bound (gathers + per-k-tile handshakes), so
+# below _FUSED_MIN_EDGES the unfused pipeline is kept.
 _FUSED_MODE = os.environ.get("EQF_FUSED", "auto")
 _FUSED = _FUSED_MODE != "0"
 _FUSED_MIN_EDGES = int(os.environ.get("EQF_FUSED_MIN_EDGES", "200000"))
@@ -593,7 +592,7 @@ def dtp_linear_ok(plan: DtpPlan, y: torch.Tensor, w: torch.Tensor) -> bool:
 
 def dtp_linear_fwd_raw(plan: DtpPlan, group: int, xs, y, w, Wt: torch.Tensor, gather=None, w_offset=None) -> torch.Tensor:
     """``C[e, k, :] = DTP_group(x, y; w)[e, k, :] @ Wt`` with the tensor product produced on chip as the A operand of the
-    tcgen05 GEMM (``eqf_dtp_linear_fwd``): ``[E, 2 l3 + 1, N]``.  ``Wt`` is ``[K_group, N]``."""
+    wgmma GEMM (``eqf_dtp_linear_fwd``): ``[E, 2 l3 + 1, N]``.  ``Wt`` is ``[K_group, N]``."""
     y, w, E, shared = _check_yw(plan, y, w)
     xs, gather = _check_gather(plan, xs, gather, E, "dtp_linear x")
     l3, _p, K = plan.out_groups[group]
@@ -618,9 +617,11 @@ def dtp_linear_fwd_raw(plan: DtpPlan, group: int, xs, y, w, Wt: torch.Tensor, ga
     return C
 
 
-# widest linear that is fused: beyond it every 128-column tile would recompute the product, so the group is written to HBM
-# once (eqf_dtp_group_forward) and read by the wide tcgen05 GEMM
-_FUSED_MAX_N = int(os.environ.get("EQF_FUSED_MAX_N", "128"))
+# widest linear that is fused: the fused kernel's column tiles are 64 wide (its consumers hold the accumulator in
+# registers), and a wider linear would recompute the product once per tile, so its group is written to HBM once
+# (eqf_dtp_group_forward) and read by the wgmma GEMM.  On the stress workload (H100) fusing the 128-column linears as
+# well measured about 1 % slower per step.
+_FUSED_MAX_N = int(os.environ.get("EQF_FUSED_MAX_N", "64"))
 
 
 def dtp_group_forward_raw(plan: DtpPlan, group: int, xs, y, w, gather=None, w_offset=None) -> torch.Tensor:
@@ -1061,31 +1062,25 @@ def segment_softmax(z: torch.Tensor, graph: Graph) -> torch.Tensor:
 
 # ----------------------------------------------------------------------------- fp32-accurate tensor-core GEMM
 
-_GEMM_WORKSPACE = {}
 _GEMM_MODE = None
 
 
 def gemm_backend() -> str:
     """Which kernel carries the fp32-accurate edge-level products:
 
-    * ``'tf32x3'`` (default) - the hand-written tcgen05 3xTF32 kernels of ``libeqf_b200.so`` (``eqf_gemm_tf32x3*``);
-    * ``'cutlass'`` - the CUTLASS fast-fp32 instantiation of ``libeqf_gemm.so`` (cross-check / fallback; the library is
-      optional and only needed when this is selected with ``EQF_GEMM=cutlass`` or ``EQF_GEMM_TF32X3=0``);
+    * ``'tf32x3'`` (default) - the hand-written wgmma 3xTF32 kernels of ``libeqf_b200.so`` (``eqf_gemm_tf32x3*``);
     * ``'torch'`` - cuBLAS SGEMM everywhere (``EQF_GEMM=torch``)."""
     global _GEMM_MODE
     if _GEMM_MODE is None:
         want = os.environ.get("EQF_GEMM", "tf32x3")
-        if want == "cutlass" or (want == "tf32x3" and not _TF32X3):
-            want = "cutlass"
-            if not _lib.GEMM_LIB_PATH.exists():
-                raise _lib.EqfError(f"{_lib.GEMM_LIB_PATH} is missing: build it with equiformer_b200._lib.build_gemm() "
-                                    "(it is optional: the default EQF_GEMM=tf32x3 does not need it)")
+        if want not in ("tf32x3", "torch"):
+            raise ValueError(f"EQF_GEMM={want!r}: expected 'tf32x3' or 'torch'")
         _GEMM_MODE = want
     return _GEMM_MODE
 
 
 def gemm_backend_forced() -> bool:
-    """EQF_GEMM_FORCE=1: every aligned product goes to the CUTLASS library kernel (tests / micro-benchmarks)."""
+    """EQF_GEMM_FORCE=1: every aligned product goes to the hand-written 3xTF32 kernels, whatever its size (tests)."""
     return os.environ.get("EQF_GEMM_FORCE", "0") == "1"
 
 
@@ -1098,22 +1093,20 @@ def _gemm_operand(t: torch.Tensor):
     return t, t.stride(0)
 
 
-# reduction length from which the weight gradient runs as the sliced tcgen05 launch; node-level products (2 324 atoms x
-# (2l+1) rows) included: 24.6 -> 22.9 ms/step against cuBLAS's single-wave SIMT kernel there (gpurun r1n)
+# reduction length from which the weight gradient runs as the sliced 3xTF32 launch (node-level products of 2 324 atoms x
+# (2l+1) rows included)
 _WGRAD_MIN_K = int(os.environ.get("EQF_WGRAD_MIN_K", "2048"))
-# rows from which forward / data-gradient products leave cuBLAS for the tcgen05 kernels; EQF_GEMM_MIN_M=1 sends the small
+# rows from which forward / data-gradient products leave the small-product kernel for the 3xTF32 kernels; EQF_GEMM_MIN_M=1 sends the small
 # reference-run fixtures (tests/golden/reference_model_*.npz) through the hand-written kernels as well
 _GEMM_MIN_M = int(os.environ.get("EQF_GEMM_MIN_M", "16384"))
-# ... or this many flops (EQF_GEMM_MIN_FLOP; off by default).  Alone, the MD17 edge-level products (6 300-14 700 rows x
-# 576-672 x 64: 0.45-0.9 GFLOP) take 15-18 us on the tcgen05 kernels against 21-36 us on the warp-MMA kernel
-# (profiles/r2_small_gemm_backends.jsonl), but inside the step a threshold of 4e8 LOSES (43.7 vs 41.1 ms per MD17 step,
-# profiles/r2_bench_md17_*_c21.json): the tcgen05 route costs a weight-split + GEMM launch pair per degree where the
-# grouped kernel takes all degrees - and, in the backward, data and weight gradients - in one launch.
+# ... or this many flops (EQF_GEMM_MIN_FLOP; off by default): the 3xTF32 route costs a weight-split + GEMM launch pair
+# per degree where the grouped small-product kernel takes all degrees - and, in the backward, data and weight gradients -
+# in one launch.
 _GEMM_MIN_FLOP = float(os.environ.get("EQF_GEMM_MIN_FLOP", "inf"))
 
 
-def _use_tcgen05(M: int, N: int, K: int) -> bool:
-    """Forward / data-gradient product [M, K] x [K, N]: the tcgen05 3xTF32 kernels (True) or the small-product kernel."""
+def _use_tensor_cores(M: int, N: int, K: int) -> bool:
+    """Forward / data-gradient product [M, K] x [K, N]: the wgmma 3xTF32 kernels (True) or the small-product kernel."""
     return M >= _GEMM_MIN_M or (M >= 1024 and 2.0 * M * N * K >= _GEMM_MIN_FLOP)
 
 
@@ -1134,45 +1127,22 @@ def gemm_raw(mode: int, A: torch.Tensor, B: torch.Tensor) -> torch.Tensor:
     fast = A.is_cuda and A.dtype == torch.float32 and aligned
     backend = gemm_backend() if fast else "torch"
     forced = fast and gemm_backend_forced()
-    # measured policy (profiles/r1_gemm_microbench.jsonl): the tensor-core kernels win on the tall edge-level products
-    # (forward / data gradient from _GEMM_MIN_M rows, weight gradient from _WGRAD_MIN_K reduction rows); below that cuBLAS.
-    # forward / data-gradient products of the edge-level linears run on the hand-written 3xTF32 tcgen05 kernels (A from
-    # shared memory for wide outputs, from TMEM for N <= 128): 1.1-1.7x the CUTLASS collective on every layer shape
-    # (profiles/r1_tf32x3_microbench.jsonl); the weight gradient (one TMEM accumulator per row slice, 32-row TMA boxes)
-    # is ahead of the sliced CUTLASS launch on every layer shape (profiles/r1_tf32x3_wgrad_microbench.jsonl)
-    if backend == "tf32x3" and not forced:
-        if mode != 2 and _use_tcgen05(M, N, K):
+    # policy: the tensor-core kernels take the tall edge-level products (forward / data gradient from _GEMM_MIN_M rows,
+    # weight gradient from _WGRAD_MIN_K reduction rows); below that the exact-fp32 small-product kernel
+    if backend == "tf32x3":
+        if mode != 2 and (forced or _use_tensor_cores(M, N, K)):
             return gemm_tf32x3_raw(A, B, b_is_kn=(mode == 0))
-        if mode == 2 and K >= _WGRAD_MIN_K:
+        if mode == 2 and (forced or K >= _WGRAD_MIN_K):
             return gemm_tf32x3_wgrad_raw(A, B)
-    use_cutlass = fast and (forced or (backend == "cutlass" and ((mode != 2 and _use_tcgen05(M, N, K))
-                                                                  or (mode == 2 and K >= _WGRAD_MIN_K))))
-    if not use_cutlass and fast and backend != "torch" and _SMALL_OWN:
+    if fast and backend != "torch" and _SMALL_OWN:
         # small products (the whole MD17 regime, node-level leftovers): the exact-fp32 CUDA-core kernel, not cuBLAS
         split = mode == 2 and K >= 1024 and not _DETERMINISTIC   # long reduction, small output: split across CTAs, atomic adds
         C = (torch.zeros if split else torch.empty)((M, N), device=A.device, dtype=torch.float32)
         grouped_gemm_raw([(mode, A, B, C, 1.0, split)])
         return C
-    if not use_cutlass:
-        if mode == 0:
-            return A @ B
-        return A @ B.t() if mode == 1 else A.t() @ B
-    A, lda = _gemm_operand(A)
-    B, ldb = _gemm_operand(B)
-    lib = _lib.load_gemm()
-    ws = _GEMM_WORKSPACE.get(A.device)
-    if ws is None:
-        ws = torch.empty(int(lib.eqf_gemm_workspace_bytes()), dtype=torch.uint8, device=A.device)
-        _GEMM_WORKSPACE[A.device] = ws
-    if mode == 2 and K >= min(4096, _WGRAD_MIN_K):
-        return _wgrad_sliced(lib, ws, A, B, lda, ldb, M, N, K)
-    C = torch.empty((M, N), device=A.device, dtype=torch.float32)
-    flops_bytes = 4 * (A.numel() + B.numel() + C.numel())
-    with torch.cuda.device(A.device), _kernel(_gemm_name("gemm_fast_f32", mode, M, N, K), flops_bytes):
-        rc = lib.eqf_gemm_f32(mode, A.data_ptr(), B.data_ptr(), C.data_ptr(), M, N, K, lda, ldb, N, 0.0,
-                              ws.data_ptr(), ws.numel(), _stream())
-    _lib.check_gemm(rc, "eqf_gemm_f32")
-    return C
+    if mode == 0:
+        return A @ B
+    return A @ B.t() if mode == 1 else A.t() @ B
 
 
 _GEMM_SHAPE_NAMES = os.environ.get("EQF_PROFILE_GEMM_SHAPES", "0") == "1"
@@ -1183,15 +1153,14 @@ def _gemm_name(base: str, mode: int, M: int, N: int, K: int) -> str:
     return f"{base}[m{mode} {M}x{N}x{K}]" if _GEMM_SHAPE_NAMES else base
 
 
-_TF32X3 = os.environ.get("EQF_GEMM_TF32X3", "1") != "0"
 # EQF_DETERMINISTIC=1: weight gradients through per-slice partials + a fixed-order column sum (bitwise reproducible)
-# instead of TMA reduce-adds whose summation order varies between runs
+# instead of atomic adds whose summation order varies between runs
 _DETERMINISTIC = os.environ.get("EQF_DETERMINISTIC", "0") == "1"
 _TF32X3_SPLIT = {}
 
 
 def gemm_tf32x3_raw(A: torch.Tensor, Bt: torch.Tensor, b_is_kn: bool = False) -> torch.Tensor:
-    """``A[M, K] @ Bt[N, K]^T`` - or ``A @ B`` with ``B[K, N]`` when ``b_is_kn`` - through the hand-written tcgen05
+    """``A[M, K] @ Bt[N, K]^T`` - or ``A @ B`` with ``B[K, N]`` when ``b_is_kn`` - through the hand-written wgmma
     3xTF32 kernels (``eqf_gemm_tf32x3``)."""
     A = _require_cuda(A, "gemm A")
     Bt = _require_cuda(Bt, "gemm B")
@@ -1217,7 +1186,7 @@ def gemm_tf32x3_raw(A: torch.Tensor, Bt: torch.Tensor, b_is_kn: bool = False) ->
 
 
 def gemm_tf32x3_wgrad_raw(A: torch.Tensor, G: torch.Tensor) -> torch.Tensor:
-    """``A[R, K1]^T @ G[R, N]`` (weight gradient) through the hand-written tcgen05 3xTF32 kernel: per-slice partial
+    """``A[R, K1]^T @ G[R, N]`` (weight gradient) through the hand-written wgmma 3xTF32 kernel: per-slice partial
     products (one CTA per row slice and output tile) + one deterministic column sum over the slices."""
     A = _require_cuda(A, "wgrad A")
     G = _require_cuda(G, "wgrad G")
@@ -1227,7 +1196,7 @@ def gemm_tf32x3_wgrad_raw(A: torch.Tensor, G: torch.Tensor) -> torch.Tensor:
     A, lda = _gemm_operand(A)
     G, ldg = _gemm_operand(G)
     lib = _lib.load()
-    if not _DETERMINISTIC:      # slices add into W through TMA reduce-adds: one launch, no partial buffer / column sum
+    if not _DETERMINISTIC:      # slices add into W through atomic adds: one launch, no partial buffer / column sum
         W = torch.empty((K1, N), device=A.device, dtype=torch.float32)
         with torch.cuda.device(A.device), _kernel(_gemm_name("gemm_tf32x3_wgrad", 2, K1, N, R), 4 * (A.numel() + G.numel() + W.numel()),
                                                   2 * R * K1 * N):
@@ -1242,40 +1211,6 @@ def gemm_tf32x3_wgrad_raw(A: torch.Tensor, G: torch.Tensor) -> torch.Tensor:
     if slices == 1:
         return part[0]
     return colsum_raw(part.view(slices, K1 * N)).view(K1, N)
-
-
-def _wgrad_sliced(lib, ws, A, B, lda, ldb, M, N, K):
-    """dW[M,N] = A[K,M]^T B[K,N] with the K rows cut into slices: one batched tcgen05 launch + a sum over slices.
-
-    The output is tiny ([224..384] x [32..352]) and the reduction long (all edges x components), so a plain GEMM
-    launches only a handful of CTAs; the batch dimension restores the parallelism (same trick as split-K, but the
-    partial products are independent batches of the same fast-fp32 kernel)."""
-    import os
-    tiles = ((M + 127) // 128) * ((N + 127) // 128 if N > 64 else 1)
-    # CTAs per SM to aim for: measured best 4 for the narrow outputs (<= 3 tiles), 2 for wider ones
-    # (profiles/r1_gemm_wgrad_slices.jsonl); EQF_WGRAD_WAVES overrides
-    waves = float(os.environ.get("EQF_WGRAD_WAVES", "4" if tiles <= 3 else "2"))
-    slices = max(1, min(int(-(-waves * 148 // tiles)), K // 256))
-    chunk = max((K // slices) & ~15, 16)             # multiple of the 16-row k-tile; the rest is the tail
-    # an exact divisor of K near the target (multiple of 4 rows keeps every slice 16-byte aligned) avoids the tail launch
-    for c in range(chunk + (-chunk % 4), min(2 * chunk, K) + 1, 4):
-        if K % c == 0:
-            chunk = c
-            break
-    slices = K // chunk
-    tail = K - slices * chunk
-    part = torch.empty((slices + (1 if tail else 0), M, N), device=A.device, dtype=torch.float32)
-    nbytes = 4 * (A.numel() + B.numel() + 2 * part.numel())
-    with torch.cuda.device(A.device), _kernel(_gemm_name("gemm_fast_f32_wgrad", 2, M, N, K), nbytes):
-        rc = lib.eqf_gemm_f32_wgrad_sliced(A.data_ptr(), B.data_ptr(), part.data_ptr(), M, N, chunk, slices, lda, ldb,
-                                           ws.data_ptr(), ws.numel(), _stream())
-        _lib.check_gemm(rc, "eqf_gemm_f32_wgrad_sliced")
-        if tail:
-            off = slices * chunk
-            rc = lib.eqf_gemm_f32(2, A.data_ptr() + 4 * off * lda, B.data_ptr() + 4 * off * ldb, part[slices].data_ptr(),
-                                  M, N, tail, lda, ldb, N, 0.0, ws.data_ptr(), ws.numel(), _stream())
-            _lib.check_gemm(rc, "eqf_gemm_f32 (tail)")
-    return colsum_raw(part.view(part.shape[0], M * N)).view(M, N)
 
 
 class Gemm(torch.autograd.Function):
@@ -1330,7 +1265,7 @@ def linear_f32(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tenso
 # data gradients and weight gradients (the two gradient sets share a launch in a first-order backward).  Round 1 sent each
 # of these 30-80 MFLOP products to cuBLAS separately (~180 SIMT SGEMM launches per QM9 step).
 _GROUPED = os.environ.get("EQF_GROUPED_GEMM", "1") != "0"
-# EQF_SMALL_GEMM=cublas hands single small products (below the tcgen05 thresholds) back to torch / cuBLAS (A/B switch)
+# EQF_SMALL_GEMM=cublas hands single small products (below the tensor-core thresholds) back to torch / cuBLAS (A/B switch)
 _SMALL_OWN = os.environ.get("EQF_SMALL_GEMM", "own") != "cublas"
 
 
@@ -1489,13 +1424,13 @@ class PlanarLinearWgrad(torch.autograd.Function):
 
 def planar_linear_grouped_ok(spec: LinearSpec, w: torch.Tensor, xs) -> bool:
     """All paths in one launch of the small-product kernel: CUDA fp32, aligned channels, every product below the row count
-    from which the tcgen05 kernels take over.  ``EQF_DETERMINISTIC=1`` keeps the per-degree route (the grouped weight
+    from which the tensor-core kernels take over.  ``EQF_DETERMINISTIC=1`` keeps the per-degree route (the grouped weight
     gradients meet in ``gw`` through fp32 atomics, whose order is not fixed)."""
     if not (_GROUPED and not _DETERMINISTIC and w.is_cuda and w.dtype == torch.float32 and w.dim() == 1 and w.is_contiguous()
             and w.data_ptr() % 16 == 0 and spec.aligned() and gemm_backend() != "torch"):
         return False
     return all(x.is_cuda and x.dtype == torch.float32 and x.dim() == 3 and x.shape[2] == p[3]
-               and not _use_tcgen05(x.shape[0] * x.shape[1], max(p[3], p[4]), min(p[3], p[4])) for p, x in zip(spec.paths, xs))
+               and not _use_tensor_cores(x.shape[0] * x.shape[1], max(p[3], p[4]), min(p[3], p[4])) for p, x in zip(spec.paths, xs))
 
 
 def planar_linear_grouped(spec: LinearSpec, w: torch.Tensor, xs):

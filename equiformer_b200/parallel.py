@@ -2,7 +2,7 @@
 
 Mirrors what the reference gets from ``DistributedDataParallel`` (``main_qm9.py:178-179``): molecules are
 independent, so the forward/backward of the edge path needs no communication; only parameter gradients are
-averaged.  The model has ~3.5 M fp32 parameters (14 MB) - latency-bound on NVLink 5 / NVSwitch - so all gradients
+averaged.  The model has ~3.5 M fp32 parameters (14 MB) - latency-bound on NVLink 4 / NVSwitch - so all gradients
 live as views of ONE contiguous buffer and a single NCCL all-reduce (in-switch NVLS reduction when available) is
 issued per step; nothing is bucketed or copied.  Works with any ``torch.distributed`` backend (gloo in the CPU tests).
 """

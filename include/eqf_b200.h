@@ -1,4 +1,4 @@
-/* eqf_b200.h - C ABI of libeqf_b200.so, the sm_100a edge kernels behind the Equiformer hot path.
+/* eqf_b200.h - C ABI of libeqf_b200.so, the sm_90a edge kernels behind the Equiformer hot path.
  *
  * The reference (atomicarchitects/equiformer) has no FFI layer of its own: the boundary is the
  * Python nn.Module surface of nets/tensor_product_rescale.py and nets/graph_attention_transformer.py
@@ -154,31 +154,28 @@ int eqf_ln_silu_fwd(const float* x, const float* bias, const float* gamma, const
 int eqf_ln_silu_bwd(const float* x, const float* bias, const float* gamma, const float* beta, const float* mean,
                     const float* rstd, const float* gy, int64_t R, int32_t C, float* gx, float* part, void* stream);
 
-/* Hand-written tcgen05 GEMM (3xTF32, fp32-level accuracy) for the tall per-degree linears: C[M, N] = A[M, K] x W, all
+/* Hand-written wgmma GEMM (3xTF32, fp32-level accuracy) for the tall per-degree linears: C[M, N] = A[M, K] x W, all
  * row-major fp32.  W is given as Bt[N, K] (b_is_kn = 0, data gradient: W = Bt^T) or as B[K, N] (b_is_kn = 1, forward);
  * `split` = device scratch of 2*N*K floats (hi / lo planes of the weights).  Replaces the e3nn 'uvw' einsum -> cuBLAS
- * SGEMM of LinearRS (nets/tensor_product_rescale.py:165-174).  Outputs wider than 128 columns: split A tile in shared
- * memory; N <= 128: A operand from TMEM. */
+ * SGEMM of LinearRS (nets/tensor_product_rescale.py:165-174). */
 int eqf_gemm_tf32x3(const float* A, const float* Bt, float* C, int64_t M, int64_t N, int64_t K, int64_t lda,
                     int64_t ldb, int64_t ldc, int32_t b_is_kn, float* split, void* stream);
 /* Weight gradient of the same linears, W[K1, N] = A[R, K1]^T G[R, N] (what autograd derives for the 'uvw' einsum of
  * LinearRS): the R rows are cut into eqf_gemm_tf32x3_wgrad_slices(R, K1, N) slices, every CTA reduces one slice into a
- * TMEM accumulator and writes partial[slice][K1][N]; the caller sums the partials over slices (eqf_colsum). */
+ * register accumulator and writes partial[slice][K1][N]; the caller sums the partials over slices (eqf_colsum). */
 int64_t eqf_gemm_tf32x3_wgrad_slices(int64_t R, int64_t K1, int64_t N);
 int eqf_gemm_tf32x3_wgrad(const float* A, const float* G, float* partial, int64_t R, int64_t K1, int64_t N, int64_t lda,
                           int64_t ldg, void* stream);
-/* same product written straight into W[K1, N]: W is zeroed, the slices add into it with TMA reduce-adds (fp32 adds in
- * L2, order not fixed - last-bit differences between runs, like the reference's atomic scatter) */
+/* same product written straight into W[K1, N]: W is zeroed, the slices add into it with fp32 atomics (order not fixed -
+ * last-bit differences between runs, like the reference's atomic scatter) */
 int eqf_gemm_tf32x3_wgrad_accumulate(const float* A, const float* G, float* W, int64_t R, int64_t K1, int64_t N,
                                      int64_t lda, int64_t ldg, void* stream);
-/* debugging aid: device buffer of 4*1024 int64 receiving CTA 0's clock64 timeline on later launches (NULL = off) */
-void eqf_gemm_tf32x3_set_timeline(long long* device_buffer);
 
 /* K1 - the depth-wise tensor product fused into the per-degree linear that consumes it (the reference's
  * nets/graph_attention_transformer.py:487-496: dtp(message, edge_attr, weight) -> sep_alpha / lin; :725-733 for the
  * edge-degree embedding): for output group `group` of the plan
  *   C[(e, k), :N] = DTP_group(x, y; w)[(e, k), :K] @ Wt[:K, :N]
- * with the [E * (2 l3 + 1), K] tensor-product block produced ON CHIP as the tensor-memory A operand of a tcgen05 3xTF32
+ * with the [E * (2 l3 + 1), K] tensor-product block produced ON CHIP as the register A operand of a wgmma 3xTF32
  * GEMM (csrc/eqf_fused.cu) - it never reaches HBM.  Operands as for eqf_dtp_forward (x gathered as x[src] + x2[dst] when
  * op->src is set; w per edge [E][W] (+ w_offset) or shared [W]).  Wt row-major [K][N], row stride ldw; C
  * [E * (2 l3 + 1)][N], row stride ldc; `split` = device scratch of 2 * N * K floats (hi / lo planes of Wt).
@@ -307,25 +304,6 @@ int eqf_gate_logits_fwd(const EqfGateLayout* lay, const float* t0, const float* 
 int eqf_gate_logits_bwd(const EqfGateLayout* lay, const float* t0, const float* bias, const float* const* gated,
                         const float* alpha_dot, const float* gz, const float* gv0, const float* const* gvout,
                         int64_t n_edges, float* gt0, float* const* ggated, float* gdot_part, void* stream);
-
-/* ---- libeqf_gemm.so: fp32-accurate tensor-core GEMM for the per-degree channel-mixing linears ------------------
- * Replaces the cuBLAS SGEMMs behind LinearRS (nets/tensor_product_rescale.py:165-174) on planar buffers.
- *   mode 0: C[M,N] = A[M,K] B[K,N]          (forward;   A, B row-major with leading dims lda, ldb)
- *   mode 1: C[M,N] = A[M,K] B[N,K]^T        (data grad; B row-major [N,K])
- *   mode 2: C[M,N] = A[K,M]^T B[K,N]        (weight grad; A row-major [K,M])
- * beta = 0 overwrites C, 1 accumulates.  All dims / leading dims must be multiples of 4 floats (16-byte TMA rows). */
-int eqf_gemm_f32(int mode, const float* A, const float* B, float* C, int64_t M, int64_t N, int64_t K,
-                 int64_t lda, int64_t ldb, int64_t ldc, float beta, void* workspace, int64_t workspace_bytes,
-                 void* stream);
-/* weight gradient with the row reduction split into `slices` chunks of `chunk` rows (batched launch):
- * part[s][M,N] = A[s*chunk:(s+1)*chunk, :M]^T B[s*chunk:(s+1)*chunk, :N]; the caller sums over s. */
-int eqf_gemm_f32_wgrad_sliced(const float* A, const float* B, float* part, int64_t M, int64_t N, int64_t chunk,
-                              int64_t slices, int64_t lda, int64_t ldb, void* workspace, int64_t workspace_bytes,
-                              void* stream);
-int64_t eqf_gemm_workspace_bytes(void);
-const char* eqf_gemm_last_error(void);
-/* compile-time tuning of the fast-fp32 mainloop: bf16 bands kept (3..5), accumulator promotion interval, K tile */
-int eqf_gemm_config(int* bands, int* promo, int* tile_k);
 
 #ifdef __cplusplus
 }

@@ -2,7 +2,7 @@
 
 What these add over ``test_gpu_model.py`` (tiny graphs, where every GEMM is below the tensor-core threshold):
 * config 2 (128 molecules, E ~ 32.5 k): forward energies and every parameter gradient of the headline model, eager and
-  through ``GraphedForwardBackward`` (the path ``bench.py`` times: tcgen05 3xTF32 GEMMs + CUDA-graph replay);
+  through ``GraphedForwardBackward`` (the path ``bench.py`` times: wgmma 3xTF32 GEMMs + CUDA-graph replay);
 * config 3 (MD17 Lmax=3, batch 5): energy, forces and the parameter gradients of the reference's energy + force loss
   (``main_md17.py:384-390``, weights of ``scripts/train/md17/equiformer/se_l3/target@aspirin.sh:22-23``);
 * config 4 (OC20 ``l1_256_nonlinear`` shapes, E ~ 58 k): one GraphAttention layer forward AND backward.
@@ -79,7 +79,7 @@ def qm9_full(cuda_device):
 
 
 def test_qm9_full_batch_energy_and_param_grads_eager(cuda_device, qm9_full):
-    """BASELINE config 2 at full size, eager: every edge-level product has M >= 16 384 rows -> tcgen05 kernels."""
+    """BASELINE config 2 at full size, eager: every edge-level product has M >= 16 384 rows -> wgmma kernels."""
     from equiformer_b200 import ops
     model, (pos, batch, z, coef), ref_e, ref_g = qm9_full
     d = lambda t: t.to(cuda_device)

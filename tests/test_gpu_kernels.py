@@ -1,4 +1,4 @@
-"""-m gpu: every sm_100a kernel against the fp64 oracle (and the table-walking emulation) on seeded inputs.
+"""-m gpu: every sm_90a kernel against the fp64 oracle (and the table-walking emulation) on seeded inputs.
 
 Tolerance: fp32 kernels vs fp64 oracle, max-abs error relative to the output's max magnitude <= 2e-5 for a single
 kernel (north_star: 1e-4 relative end to end).
@@ -176,9 +176,9 @@ def test_unsorted_edges_are_sorted_once(cuda_device):
 @pytest.mark.parametrize("M,N,K", [(36000, 352, 224), (108000, 64, 384), (180000, 32, 352), (2304, 128, 128), (36000, 960, 64),
                                    (1001 * 4, 480, 352), (12, 8, 4)])
 def test_fast_fp32_gemm_all_layouts(cuda_device, M, N, K, monkeypatch):
-    """tcgen05 fast-fp32 GEMM (libeqf_gemm.so) vs fp64 matmul: forward, data-grad and weight-grad layouts."""
+    """Fast-fp32 GEMM entry point (gemm_raw) vs fp64 matmul: forward, data-grad and weight-grad layouts."""
     from equiformer_b200 import ops
-    monkeypatch.setenv("EQF_GEMM_FORCE", "1")   # exercise the CUTLASS kernel for every layout / size, not just the policy's picks
+    monkeypatch.setenv("EQF_GEMM_FORCE", "1")   # exercise the 3xTF32 kernels for every layout / size, not just the policy's picks
     g = torch.Generator().manual_seed(M + N + K)
     A = torch.randn(M, K, generator=g)
     B = torch.randn(K, N, generator=g)
@@ -198,8 +198,8 @@ def test_fast_fp32_gemm_all_layouts(cuda_device, M, N, K, monkeypatch):
 @pytest.mark.parametrize("M,N,K", [(100, 16, 32), (1000, 48, 64), (3001, 72, 100), (36000, 224, 224), (36000, 352, 224),
                                    (36000, 960, 64), (108000, 384, 64), (33000, 128, 960), (129, 256, 16), (128, 272, 36)])
 def test_tf32x3_tcgen05_gemm(cuda_device, M, N, K):
-    """Hand-written tcgen05 3xTF32 GEMM C = A Bt^T vs fp64: ragged rows, K tails, single and multiple column tiles,
-    strided A.  Accuracy: 2-3e-6 of max|C| at K ~ 224 (TMEM accumulation), far from single-pass TF32's 1e-3."""
+    """Hand-written wgmma 3xTF32 GEMM C = A Bt^T vs fp64: ragged rows, K tails, single and multiple column tiles,
+    strided A.  Accuracy: a few 1e-6 of max|C| at K ~ 224, far from single-pass TF32's 1e-3."""
     from equiformer_b200 import ops
     g = torch.Generator().manual_seed(M + N + K)
     A = torch.randn(M, K, generator=g)
@@ -220,51 +220,30 @@ def test_tf32x3_tcgen05_gemm(cuda_device, M, N, K):
     assert rel_err(ops.gemm_tf32x3_raw(d(A), d(Bt).t().contiguous(), b_is_kn=True), ref) < tol
 
 
-@pytest.mark.parametrize("M,N,K", [(100, 64, 96), (128, 32, 32), (130, 32, 352), (1000, 64, 100), (40000, 32, 96), (97680, 64, 384)])
-def test_tf32x3_cta_pair_kernel_matches_single_cta(cuda_device, M, N, K, monkeypatch):
-    """The opt-in cta_group::2 variant of the narrow-output kernel (EQF_TF32X3_2SM=1; two CTAs share each M = 256
-    instruction) must reproduce the single-CTA kernel bit for bit - same products, same accumulation order - including
-    tiles whose second half lies past the last row."""
-    from equiformer_b200 import ops
-    g = torch.Generator().manual_seed(M + N + K)
-    A = torch.randn(M, K, generator=g).to(cuda_device)
-    Bt = torch.randn(N, K, generator=g).to(cuda_device)
-    monkeypatch.setenv("EQF_TF32X3_2SM", "0")
-    single = ops.gemm_tf32x3_raw(A, Bt)
-    monkeypatch.setenv("EQF_TF32X3_2SM", "1")
-    pair = ops.gemm_tf32x3_raw(A, Bt)
-    assert torch.equal(single, pair)
-    assert rel_err(pair, A.double().cpu() @ Bt.double().cpu().t()) < 6e-6 * max(1.0, (K / 256) ** 0.5)
-    assert torch.equal(ops.gemm_tf32x3_raw(A, Bt.t().contiguous(), b_is_kn=True), pair)
-
-
 @pytest.mark.parametrize("R,K1,N", [(100, 32, 32), (1000, 64, 48), (3001, 100, 72), (36000, 224, 224), (36000, 224, 352),
                                     (36000, 64, 960), (2324, 128, 128), (11620, 32, 32), (108000, 384, 64), (17, 260, 40)])
-@pytest.mark.parametrize("a_through_tmem", ["1", "0"])
-def test_tf32x3_tcgen05_weight_gradient(cuda_device, R, K1, N, a_through_tmem, monkeypatch):
-    """Hand-written tcgen05 3xTF32 weight gradient W = A^T G (MN-major operands, per-slice TMEM accumulators, column
-    sum over slices) vs fp64.  The TMEM accumulation truncates, so the error grows with the rows per slice (~1e-5 at
-    2 000 rows); single-pass TF32 would be 1e-3.  Outputs of <= 64 columns take the A^T operand through tensor memory
-    (the default) or, with EQF_TF32X3_WGRAD_TS=0, through shared memory like the wide ones: both are covered."""
+@pytest.mark.parametrize("deterministic", ["1", "0"])
+def test_tf32x3_tcgen05_weight_gradient(cuda_device, R, K1, N, deterministic, monkeypatch):
+    """Hand-written wgmma 3xTF32 weight gradient W = A^T G (MN-major operands, per-slice register accumulators) vs fp64.
+    The tensor-core accumulation truncates, so the error grows with the rows per slice (~1e-5 at 2 000 rows); single-pass
+    TF32 would be 1e-3.  ``deterministic`` picks the reduction route every check of the case runs on: "1" per-slice
+    partials + fixed-order column sum (bitwise reproducible), "0" atomic adds into W."""
     from equiformer_b200 import ops
-    monkeypatch.setenv("EQF_TF32X3_WGRAD_TS", a_through_tmem)
+    monkeypatch.setattr(ops, "_DETERMINISTIC", deterministic == "1")
     g = torch.Generator().manual_seed(R + K1 + N)
     A = torch.randn(R, K1, generator=g)
     G = torch.randn(R, N, generator=g)
     d = lambda t: t.to(cuda_device)
-    out = ops.gemm_tf32x3_wgrad_raw(d(A), d(G))
-    assert out.shape == (K1, N) and rel_err(out, A.double().t() @ G.double()) < 4e-5
+    out0 = ops.gemm_tf32x3_wgrad_raw(d(A), d(G))
+    assert out0.shape == (K1, N) and rel_err(out0, A.double().t() @ G.double()) < 4e-5
     wide = torch.randn(R, K1 + 8, generator=g)
     out = ops.gemm_tf32x3_wgrad_raw(d(wide)[:, 4:4 + K1], d(G))
     assert rel_err(out, wide[:, 4:4 + K1].double().t() @ G.double()) < 4e-5
     Ai = torch.randint(-4, 5, (R, K1), generator=g).float()
     Gi = torch.randint(-4, 5, (R, N), generator=g).float()
     assert torch.equal(ops.gemm_tf32x3_wgrad_raw(d(Ai), d(Gi)).cpu(), Ai.t() @ Gi)
-    # the other reduction route (TMA reduce-adds <-> per-slice partials + fixed-order column sum)
-    monkeypatch.setattr(ops, "_DETERMINISTIC", not ops._DETERMINISTIC)
-    out2 = ops.gemm_tf32x3_wgrad_raw(d(A), d(G))
-    assert rel_err(out2, A.double().t() @ G.double()) < 4e-5
-    assert torch.equal(ops.gemm_tf32x3_wgrad_raw(d(Ai), d(Gi)).cpu(), Ai.t() @ Gi)
+    if deterministic == "1":       # the fixed summation order gives the same bits on every call
+        assert torch.equal(ops.gemm_tf32x3_wgrad_raw(d(A), d(G)), out0)
 
 
 def test_gemm_autograd_closure(cuda_device):
@@ -623,9 +602,9 @@ FUSED_CASES = [("qm9_l2", False, True, 32560), ("qm9_l2", True, False, 32560), (
 
 @pytest.mark.parametrize("name,shared,gather,E", FUSED_CASES)
 def test_fused_dtp_linear_forward_vs_fp64(cuda_device, name, shared, gather, E):
-    """``eqf_dtp_linear_fwd`` (tensor product produced on chip as the TMEM A operand of the tcgen05 3xTF32 GEMM) against
+    """``eqf_dtp_linear_fwd`` (tensor product produced on chip as the register A operand of the wgmma 3xTF32 GEMM) against
     the fp64 table walk followed by an fp64 matmul, every output group; output widths as the model uses them (wide 0e
-    group in column tiles, 64 / 32 stacked) plus one odd width; gathered per-edge weights with the radial offset folded
+    group in column tiles, 64 / 32 columns) plus one odd width; gathered per-edge weights with the radial offset folded
     in, and shared weights on per-edge blocks."""
     from equiformer_b200 import ops
     plan = _dtp(name).tp.plan

@@ -1,4 +1,4 @@
-"""-m gpu: drop-in modules on the B200 (fp32) against the CPU oracle (fp64, same weights, same inputs).
+"""-m gpu: drop-in modules on the H100 (fp32) against the CPU oracle (fp64, same weights, same inputs).
 
 Tolerances follow north_star: energies / node irreps / forces within 1e-4 relative (to the max magnitude of the
 reference quantity); parameter gradients within 1e-3 of the largest gradient entry (they accumulate over all edges).

@@ -51,14 +51,10 @@ def test_library_exports_every_declared_symbol(built_lib):
     header = (Path(_lib.INCLUDE_DIR) / "eqf_b200.h").read_text()
     declared = set(re.findall(r"\b(eqf_[a-z0-9_]+)\s*\(", header))
     assert declared, "no declarations parsed"
-    bound = set(_lib.SIGNATURES) | set(_lib.GEMM_SIGNATURES)
+    bound = set(_lib.SIGNATURES)
     assert declared == bound, declared ^ bound
     for name in _lib.SIGNATURES:
         assert hasattr(built_lib, name), name
-    _lib.build_gemm()
-    gemm = _lib.load_gemm()
-    for name in _lib.GEMM_SIGNATURES:
-        assert hasattr(gemm, name), name
     assert built_lib.eqf_version() == 100
     assert built_lib.eqf_last_error() is not None
 

@@ -276,7 +276,7 @@ def test_oracle_headline_model_matches_reference_model_file():
 
 @pytest.mark.gpu
 def test_cuda_headline_model_matches_reference_model_file(cuda_device):
-    """The CUDA path of the headline configuration (generated ``qm9_l2`` kernels, tcgen05 GEMMs, planar-resident blocks)
+    """The CUDA path of the headline configuration (generated ``qm9_l2`` kernels, wgmma GEMMs, planar-resident blocks)
     against the energies the reference's own model file returned for the same parameters.  Float32 through six blocks
     against a float64 fixture whose closed-form readout weights cancel to |E| ~ 0.07 while block outputs are ~3: the
     float32 CPU oracle is 1.6e-5 away from the fixture in absolute terms, the bound here is 3e-4."""
@@ -296,7 +296,7 @@ def test_cuda_headline_model_matches_reference_model_file(cuda_device):
 @pytest.fixture
 def tensor_core_gemms_everywhere():
     """Lower the row thresholds of the GEMM policy (``ops._GEMM_MIN_M`` / ``_WGRAD_MIN_K``; env EQF_GEMM_MIN_M /
-    EQF_WGRAD_MIN_K) so that even the 16-atom reference-run fixtures go through the hand-written tcgen05 kernels instead
+    EQF_WGRAD_MIN_K) so that even the 16-atom reference-run fixtures go through the hand-written wgmma kernels instead
     of cuBLAS (VERDICT r1: at these sizes ``M = E (2l+1) << 16 384`` and every product used to be a cuBLAS call)."""
     from equiformer_b200 import ops
     old = ops._GEMM_MIN_M, ops._WGRAD_MIN_K
@@ -307,7 +307,7 @@ def tensor_core_gemms_everywhere():
 
 @pytest.mark.gpu
 def test_cuda_headline_model_matches_reference_through_tcgen05_gemms(cuda_device, tensor_core_gemms_everywhere):
-    """As ``test_cuda_headline_model_matches_reference_model_file`` with every aligned product on the tcgen05 3xTF32
+    """As ``test_cuda_headline_model_matches_reference_model_file`` with every aligned product on the wgmma 3xTF32
     kernels (forward + one backward pass; the gradients are checked against the oracle in the next test - this fixture's
     closed-form weights leave several gradients at rounding-noise level)."""
     from equiformer_b200 import ops
@@ -332,7 +332,7 @@ def test_cuda_headline_model_matches_reference_through_tcgen05_gemms(cuda_device
 @pytest.mark.gpu
 def test_cuda_small_model_gradients_through_tcgen05_gemms_match_oracle(cuda_device, tensor_core_gemms_everywhere):
     """Every parameter gradient of the headline model on a five-molecule batch, all aligned products (forward, data and
-    weight gradients, node level included) on the tcgen05 kernels, against the fp64 oracle - the same bound as the
+    weight gradients, node level included) on the wgmma kernels, against the fp64 oracle - the same bound as the
     cuBLAS-policy run of tests/test_gpu_model.py."""
     from equiformer_b200.nets import model_entrypoint
     from tests.helpers import molecules
@@ -363,7 +363,7 @@ def test_cuda_small_model_gradients_through_tcgen05_gemms_match_oracle(cuda_devi
 
 @pytest.mark.gpu
 def test_cuda_md17_model_matches_reference_through_tcgen05_gemms(cuda_device, tensor_core_gemms_everywhere):
-    """Energy and forces of the MD17 fixture (a double-backward-capable path) with the tcgen05 kernels forced on."""
+    """Energy and forces of the MD17 fixture (a double-backward-capable path) with the wgmma kernels forced on."""
     from equiformer_b200.nets.graph_attention_transformer_md17 import GraphAttentionTransformerMD17
     g = np.load(os.path.join(os.path.dirname(SMALL), "reference_model_md17_small.npz"))
     model = _mirror_model(g, GraphAttentionTransformerMD17).to(cuda_device)

@@ -1,5 +1,5 @@
 """K1 microbenchmark: the fused DTP -> per-degree linear launch (``eqf_dtp_linear_fwd``) against the round-1 pipeline
-(DTP kernel writing ``[E, K]`` to HBM + tcgen05 GEMM reading it back) on the layer shapes of the model.
+(DTP kernel writing ``[E, K]`` to HBM + wgmma GEMM reading it back) on the layer shapes of the model.
 
 usage: python tools/fused_microbench.py [config] [E] [iters] > out.jsonl     config in {qm9_l2, md17_l3, oc20_l1}
 CUDA-event timing on the launching stream after warm-up; node tables are L2-resident as in the model, the per-edge radial

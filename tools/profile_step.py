@@ -11,7 +11,7 @@ from equiformer_b200.nets import model_entrypoint  # noqa: E402
 
 
 def main():
-    out_dir = sys.argv[1] if len(sys.argv) > 1 else "gpurun_out"
+    out_dir = sys.argv[1] if len(sys.argv) > 1 else "profile_out"
     os.makedirs(out_dir, exist_ok=True)
     dev = torch.device("cuda:0")
     torch.manual_seed(0)

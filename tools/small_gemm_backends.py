@@ -1,5 +1,5 @@
 """Which kernel for a mid-size product?  The MD17 edge-level shapes (E = 2 100 edges x (2l+1) rows, DTP group channels ->
-head / value channels) and a few node-level ones on three backends: tcgen05 3xTF32 (eqf_gemm_tf32x3), the warp-MMA grouped
+head / value channels) and a few node-level ones on three backends: wgmma 3xTF32 (eqf_gemm_tf32x3), the warp-MMA grouped
 kernel (one problem), cuBLAS.  CUDA-graph timed."""
 import json
 import os
@@ -26,14 +26,14 @@ def main():
         B = torch.randn(K, N, device=dev, generator=g)
         C = torch.empty(M, N, device=dev)
         row = {"shape": name, "M": M, "K": K, "N": N, "mflop": round(2 * M * K * N / 1e6, 1)}
-        row["tcgen05_us"] = round(timeit(lambda: ops.gemm_tf32x3_raw(A, B, b_is_kn=True)), 1)
+        row["wgmma_us"] = round(timeit(lambda: ops.gemm_tf32x3_raw(A, B, b_is_kn=True)), 1)
         row["grouped_mma_us"] = round(timeit(lambda: ops.grouped_gemm_raw([(0, A, B, C, 1.0, False)])), 1)
         row["cublas_us"] = round(timeit(lambda: A @ B), 1)
         Bt = B.t().contiguous()
-        row["tcgen05_nt_us"] = round(timeit(lambda: ops.gemm_tf32x3_raw(A, Bt)), 1)
+        row["wgmma_nt_us"] = round(timeit(lambda: ops.gemm_tf32x3_raw(A, Bt)), 1)
         G = torch.randn(M, N, device=dev, generator=g)
         W = torch.zeros(K, N, device=dev)
-        row["wgrad_tcgen05_us"] = round(timeit(lambda: ops.gemm_tf32x3_wgrad_raw(A, G)), 1)
+        row["wgrad_wgmma_us"] = round(timeit(lambda: ops.gemm_tf32x3_wgrad_raw(A, G)), 1)
         row["wgrad_grouped_mma_us"] = round(timeit(lambda: ops.grouped_gemm_raw([(2, A, G, W, 1.0, True)])), 1)
         print(json.dumps(row), flush=True)
 
