@@ -6,11 +6,14 @@
 // fp32 in HBM, fp32-level accuracy through the 3xTF32 split of eqf_tc.cuh (the weights' hi / lo planes are split once per
 // call by a tiny kernel; the A operand is split in registers and fed to wgmma as its register fragment).
 //
-// Forward: one CTA per 128 x BN output tile, three warpgroups:
+// Forward: persistent CTAs (one per SM) walking the 128 x BN output tiles, three warpgroups:
 //   warpgroup 0      TMA producer (one thread): A tile [128 x 32] and the B hi / lo tiles [BN x 32] of each k-tile
-//                    (128-byte rows, SWIZZLE_128B) into a ring of shared-memory stages (full / empty mbarriers)
+//                    (128-byte rows, SWIZZLE_128B) into a ring of shared-memory stages (full / empty mbarriers); the
+//                    ring runs across tile boundaries, so the next tile's operands land while the consumers store
 //   warpgroups 1, 2  consumers, 64 rows each: A fragments from shared memory -> hi / lo in registers -> 3 wgmma per
 //                    8-deep k-step and 64-column chunk into a k-tile accumulator, added to the running sum in registers
+// Persistence matters for the tall products with a shallow reduction (K = 32, 64: the data gradients of the 1e / 2e
+// linears): they are bound by their output stores, and a CTA per tile would wait for a TMA round trip before each store.
 // Weight gradient: the same roles over the CTA's slice of the R rows.  Both operands are "MN-major" (the reduction runs
 // along the strided dimension), which tf32 wgmma cannot read from shared memory: A^T is read as register fragments
 // straight from its swizzled TMA boxes, and the consumers transpose + split each G tile into K-major hi / lo tiles first.
@@ -52,6 +55,8 @@ struct Smem {
 struct Params {
   float* C;
   long long M, ldc;
+  long long n_tiles;      // m_blocks * n_blocks, m-block major (the n-blocks of one m-block run side by side: A is
+  int n_blocks;           // read from HBM once and from L2 for the other column tiles)
   int N, K;
 };
 
@@ -67,8 +72,6 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_const
   uint64_t* empty = full + kStages;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2;
-  const long long m0 = (long long)blockIdx.x * BM;
-  const int n0 = blockIdx.y * BN;
   const int k_tiles = (p.K + BK - 1) / BK;
   if (threadIdx.x == 0) {
     for (int s = 0; s < kStages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], kConsumerWarps); }
@@ -80,38 +83,50 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_const
     reg_dealloc<40>();
     if (threadIdx.x == 0) {
       prefetch_map(&map_a); prefetch_map(&map_bhi); prefetch_map(&map_blo);
-      for (int kt = 0; kt < k_tiles; ++kt) {
-        const int s = kt % kStages;
-        mbar_wait_hint(&empty[s], ((kt / kStages) & 1) ^ 1);
-        uint8_t* st = smem + s * S::kStageBytes;
-        mbar_expect_tx(&full[s], (uint32_t)S::kStageBytes);
-        tma_load_2d(st, &map_a, kt * BK, (int)m0, &full[s]);
-        tma_load_2d(st + S::kABytes, &map_bhi, kt * BK, n0, &full[s]);
-        tma_load_2d(st + S::kABytes + S::kBBytes, &map_blo, kt * BK, n0, &full[s]);
+      int s = 0;
+      uint32_t ph = 0;
+      for (long long tile = blockIdx.x; tile < p.n_tiles; tile += gridDim.x) {
+        const int m0 = (int)(tile / p.n_blocks) * BM;
+        const int n0 = (int)(tile % p.n_blocks) * BN;
+        for (int kt = 0; kt < k_tiles; ++kt) {
+          mbar_wait_hint(&empty[s], ph ^ 1);
+          uint8_t* st = smem + s * S::kStageBytes;
+          mbar_expect_tx(&full[s], (uint32_t)S::kStageBytes);
+          tma_load_2d(st, &map_a, kt * BK, m0, &full[s]);
+          tma_load_2d(st + S::kABytes, &map_bhi, kt * BK, n0, &full[s]);
+          tma_load_2d(st + S::kABytes + S::kBBytes, &map_blo, kt * BK, n0, &full[s]);
+          if (++s == kStages) { s = 0; ph ^= 1; }
+        }
       }
     }
   } else {
     reg_alloc<232>();
     const int row_wg = (wg - 1) * 64 + (warp & 3) * 16;      // first of this warp's 16 rows inside the tile
-    float acc[BN / 2], part[BN / 2];       // running sum, this k-tile's tensor-core sum
+    int s = 0;
+    uint32_t ph = 0;
+    for (long long tile = blockIdx.x; tile < p.n_tiles; tile += gridDim.x) {
+      const long long m0 = (tile / p.n_blocks) * BM;
+      const int n0 = (int)(tile % p.n_blocks) * BN;
+      float acc[BN / 2], part[BN / 2];     // running sum, this k-tile's tensor-core sum
 #pragma unroll
-    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-    for (int kt = 0; kt < k_tiles; ++kt) {
-      const int s = kt % kStages;
-      mbar_wait_hint(&full[s], (kt / kStages) & 1);
-      const uint32_t st = smem_u32(smem + s * S::kStageBytes);
-      uint32_t hi[16], lo[16];
-      load_a_split(st, row_wg, lane, hi, lo);
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      for (int kt = 0; kt < k_tiles; ++kt) {
+        mbar_wait_hint(&full[s], ph);
+        const uint32_t st = smem_u32(smem + s * S::kStageBytes);
+        uint32_t hi[16], lo[16];
+        load_a_split(st, row_wg, lane, hi, lo);
 #pragma unroll
-      for (int i = 0; i < BN / 2; ++i) part[i] = 0.f;
-      mma_ktile_3xtf32<BN>(part, hi, lo, st + S::kABytes, st + S::kABytes + S::kBBytes);
-      wgmma_wait<0>();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&empty[s]);
+        for (int i = 0; i < BN / 2; ++i) part[i] = 0.f;
+        mma_ktile_3xtf32<BN>(part, hi, lo, st + S::kABytes, st + S::kABytes + S::kBBytes);
+        wgmma_wait<0>();
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty[s]);
 #pragma unroll
-      for (int i = 0; i < BN / 2; ++i) acc[i] += part[i];
+        for (int i = 0; i < BN / 2; ++i) acc[i] += part[i];
+        if (++s == kStages) { s = 0; ph ^= 1; }
+      }
+      store_acc<BN>(acc, p.C, p.ldc, m0 + row_wg, p.M, n0, p.N, lane, false);
     }
-    store_acc<BN>(acc, p.C, p.ldc, m0 + row_wg, p.M, n0, p.N, lane, false);
   }
 }
 
@@ -147,7 +162,12 @@ static int launch(const CUtensorMap& ma, const CUtensorMap& mh, const CUtensorMa
     attr_err = cudaFuncSetAttribute(gemm_tf32x3_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Smem<BN>::kTotal);
   });
   if (attr_err != cudaSuccess) return check_cuda(attr_err, "gemm_tf32x3 smem attribute");
-  gemm_tf32x3_kernel<BN><<<dim3((unsigned)m_blocks, (unsigned)n_blocks), kThreads, Smem<BN>::kTotal, s>>>(ma, mh, ml, p);
+  Params q = p;
+  q.n_blocks = n_blocks;
+  q.n_tiles = m_blocks * n_blocks;
+  const long long sms = device_sms();
+  const unsigned grid = (unsigned)(q.n_tiles < sms ? q.n_tiles : sms);
+  gemm_tf32x3_kernel<BN><<<grid, kThreads, Smem<BN>::kTotal, s>>>(ma, mh, ml, q);
   return check_cuda(cudaGetLastError(), "gemm_tf32x3_kernel launch");
 }
 
