@@ -6,8 +6,15 @@ Same constructor arguments, attribute / ``state_dict`` names and ``forward(data)
 cell_offsets`` when ``otf_graph=False``).  What the reference gets from ``ocpmodels`` - ``radius_graph_pbc`` and
 ``get_pbc_distances`` (``:267-302``) - is ``equiformer_b200.graph.radius_graph_pbc`` here: two sm_90a kernels around one
 prefix sum, destination-sorted, same pair / image order and the same distance masks.  The energy head is the feed-forward
-one of the shipped IS2RE configurations; the auxiliary-task and attention heads (``use_auxiliary_task``,
-``use_attention_head``), learned node attributes and atom-pair edge attributes are outside the benchmarked path and raise.
+one of the shipped IS2RE configurations (``Linear(irreps_feature -> its 0e part) -> SiLU -> Linear(-> 1x0e)``; vector
+blocks of ``irreps_feature`` such as ``512x0e+256x1e`` feed only the auxiliary head).
+
+``use_auxiliary_task=True`` adds the IS2RS head of the ``*_aux_*`` configurations (``:181-193``, ``:372-379``): one more
+``GraphAttention`` (attribute ``auxiliary_head``) over the frame's edges, reading the normed final features before
+``out_dropout`` and predicting one vector per atom (``1x1o`` if ``irreps_feature`` has a ``1o`` block, else ``1x1e``).
+``forward`` then returns ``(energy [G, 1], aux [N, 3])``; its per-edge work runs on the same kernels as the blocks.  The
+training objective that goes with it is in ``equiformer_b200.oc20_objective``.  The attention head
+(``use_attention_head``), learned node attributes and atom-pair edge attributes are not implemented and raise.
 """
 from __future__ import annotations
 
@@ -19,8 +26,8 @@ from ..o3 import Irreps
 from .drop import EquivariantDropout
 from .fast_activation import Activation
 from .gaussian_rbf import GaussianRadialBasisLayer
-from .graph_attention_transformer import (_run_blocks, clear_hoisted, hoist_radial, EdgeDegreeEmbeddingNetwork, NodeEmbeddingNetwork, ScaledScatter,
-                                          TransBlock, get_norm_layer)
+from .graph_attention_transformer import (_run_blocks, clear_hoisted, hoist_radial, EdgeDegreeEmbeddingNetwork, GraphAttention,
+                                          NodeEmbeddingNetwork, ScaledScatter, TransBlock, get_norm_layer)
 from .layer_norm import EquivariantLayerNormV2
 from .registry import register_model
 from .tensor_product_rescale import LinearRS
@@ -45,9 +52,9 @@ class GraphAttentionTransformerOC20(torch.nn.Module):
                  alpha_drop=0.2, proj_drop=0.0, out_drop=0.0, drop_path_rate=0.0, use_auxiliary_task=False,
                  auxiliary_head_dropout=True, use_attention_head=False, otf_graph=False, use_pbc=True, max_neighbors=50):
         super().__init__()
-        if use_node_attr or use_atom_edge_attr or use_auxiliary_task or use_attention_head:
-            raise NotImplementedError("learned node attributes, atom-pair edge attributes, the auxiliary task and the attention "
-                                      "head are not used by the IS2RE configurations of the hot path (out of scope)")
+        if use_node_attr or use_atom_edge_attr or use_attention_head:
+            raise NotImplementedError("learned node attributes, atom-pair edge attributes and the attention head are not "
+                                      "implemented (no shipped OC20 configuration uses them)")
         self.max_radius, self.number_of_basis = max_radius, number_of_basis
         self.alpha_drop, self.proj_drop, self.out_drop = alpha_drop, proj_drop, out_drop
         self.drop_path_rate, self.norm_layer = drop_path_rate, norm_layer
@@ -94,6 +101,12 @@ class GraphAttentionTransformerOC20(torch.nn.Module):
             LinearRS(self.irreps_feature_scalars, Irreps("1x0e")))
         self.scale_scatter = ScaledScatter(_AVG_NUM_NODES)
         self.use_auxiliary_task, self.use_attention_head = use_auxiliary_task, use_attention_head
+        if use_auxiliary_task:                                                   # IS2RS head (reference :181-193)
+            irreps_out_auxiliary = Irreps("1x1o") if o3.Irrep("1o") in self.irreps_feature else Irreps("1x1e")
+            self.auxiliary_head = GraphAttention(
+                self.irreps_feature, self.irreps_node_attr, self.irreps_edge_attr, irreps_out_auxiliary, self.fc_neurons,
+                self.irreps_head, num_heads, irreps_pre_attn, rescale_degree, nonlinear_message,
+                alpha_drop=alpha_drop if auxiliary_head_dropout else 0.0, proj_drop=0.0)
         self.apply(self._init_weights)
 
     def _init_weights(self, m):
@@ -143,7 +156,8 @@ class GraphAttentionTransformerOC20(torch.nn.Module):
     def forward_edges(self, edge_vec, batch, atomic_numbers, tags, edge_src, edge_dst, graph=None, n_graphs=None,
                       edges_sorted: bool = True):
         """Everything after the neighbour search (ref :305-380); host-synchronisation free when ``graph`` and ``n_graphs``
-        are supplied (CUDA-graph capturable).  The periodic neighbour list is sorted by destination."""
+        are supplied (CUDA-graph capturable).  The periodic neighbour list is sorted by destination.  Returns the energy
+        ``[G, 1]``, or ``(energy, aux [N, 3])`` with ``use_auxiliary_task``."""
         n_nodes = batch.shape[0]
         edge_sh = o3.spherical_harmonics(l=self.irreps_edge_attr, x=edge_vec, normalize=True, normalization="component")
         atom_embedding, _attr, _onehot = self.atom_embed(atomic_numbers)
@@ -162,12 +176,21 @@ class GraphAttentionTransformerOC20(torch.nn.Module):
             node_attr._eqf_all_ones = True
             node_features = _run_blocks(self.blocks, node_features, self.irreps_node_embedding, node_attr, edge_src, edge_dst,
                                         edge_sh, edge_length_embedding, batch, graph)
+            node_features = self.norm(node_features, batch=batch)
+            outputs_aux = None
+            if self.use_auxiliary_task:                # IS2RS head on the normed features, before out_dropout (ref :372-379)
+                # inside the hoisted region: its radial MLP's first Linear is part of the one stacked GEMM
+                outputs_aux = self.auxiliary_head(node_input=node_features, node_attr=node_attr, edge_src=edge_src,
+                                                  edge_dst=edge_dst, edge_attr=edge_sh, edge_scalars=edge_length_embedding,
+                                                  batch=batch, graph=graph)
         finally:
             clear_hoisted(served)
-        node_features = self.norm(node_features, batch=batch)
         outputs = self.out_dropout(node_features) if self.out_dropout is not None else node_features
         outputs = self.head(outputs)
-        return self.scale_scatter(outputs, batch, dim=0, dim_size=n_graphs)
+        outputs = self.scale_scatter(outputs, batch, dim=0, dim_size=n_graphs)
+        if self.use_auxiliary_task:
+            return outputs, outputs_aux
+        return outputs
 
 
 @register_model
@@ -185,3 +208,12 @@ OC20_L1_256_NONLINEAR = dict(
     irreps_pre_attn="256x0e+128x1e", rescale_degree=False, nonlinear_message=True, irreps_mlp_mid="768x0e+384x1e",
     norm_layer="layer", alpha_drop=0.2, proj_drop=0.0, out_drop=0.0, drop_path_rate=0.0, otf_graph=True, use_pbc=True,
     max_neighbors=500)
+
+# the model block of oc20/configs/is2re/all/graph_attention_transformer/l1_256_nonlinear_aux_g@2_local.yml:31-60: the IS2RS
+# auxiliary head and a final feature with a vector block.  (The 100k l1_256_nonlinear_aux_g@2 file differs only in
+# alpha_drop=0.1, out_drop=0.1 and drop_path_rate=0.0.)
+OC20_L1_256_NONLINEAR_AUX = dict(OC20_L1_256_NONLINEAR, irreps_feature="512x0e+256x1e", drop_path_rate=0.05,
+                                 use_auxiliary_task=True)
+
+# the model block of oc20/configs/is2re/all/graph_attention_transformer/l1_256_blocks@18_nonlinear_aux_g@4_local.yml:31-60
+OC20_L1_256_BLOCKS18_NONLINEAR_AUX = dict(OC20_L1_256_NONLINEAR_AUX, num_layers=18)
