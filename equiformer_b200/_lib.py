@@ -113,14 +113,14 @@ SIGNATURES = {
     "eqf_dtp_grad_y": (c_int32, [c_void_p, POINTER(EqfEdgeOperands), c_int64, c_void_p, c_void_p]),
     "eqf_dtp_grad_xw": (c_int32, [c_void_p, POINTER(EqfEdgeOperands), c_int64, POINTER(c_void_p), c_void_p, c_void_p]),
     "eqf_seg_softmax": (c_int32, [c_void_p, c_void_p, c_int64, c_int32, c_void_p, c_void_p]),
-    "eqf_seg_softmax_bwd": (c_int32, [c_void_p, c_void_p, c_void_p, c_int64, c_int32, c_void_p, c_void_p]),
+    "eqf_seg_softmax_bwd": (c_int32, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int32, c_void_p, c_void_p]),
     "eqf_attn_aggregate": (c_int32, [POINTER(EqfHeadLayout), c_void_p, POINTER(c_void_p), c_void_p, c_void_p, c_int64,
                                      POINTER(c_void_p), c_void_p]),
-    "eqf_attn_softmax_aggregate": (c_int32, [POINTER(EqfHeadLayout), c_void_p, POINTER(c_void_p), c_void_p, c_int64,
-                                             POINTER(c_void_p), c_void_p, c_void_p]),
+    "eqf_attn_softmax_aggregate": (c_int32, [POINTER(EqfHeadLayout), c_void_p, c_void_p, POINTER(c_void_p), c_void_p,
+                                             c_int64, POINTER(c_void_p), c_void_p, c_void_p]),
     "eqf_attn_edge_dot": (c_int32, [POINTER(EqfHeadLayout), POINTER(c_void_p), POINTER(c_void_p), c_void_p, c_int64,
                                     c_void_p, c_void_p]),
-    "eqf_attn_edge_scale": (c_int32, [POINTER(EqfHeadLayout), c_void_p, POINTER(c_void_p), c_void_p, c_int64,
+    "eqf_attn_edge_scale": (c_int32, [POINTER(EqfHeadLayout), c_void_p, c_void_p, POINTER(c_void_p), c_void_p, c_int64,
                                       POINTER(c_void_p), c_void_p]),
     "eqf_pointwise_rows": (c_int32, [c_int64]),
     "eqf_ln_silu_fwd": (c_int32, [c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_int64, c_int32, c_void_p, c_void_p,

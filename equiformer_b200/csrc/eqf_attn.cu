@@ -59,8 +59,10 @@ __global__ void __launch_bounds__(256) seg_softmax_kernel(const float* __restric
 }
 
 // backward of the segment softmax: gz_e = alpha_e (ga_e - sum_{f in seg(e)} alpha_f ga_f); one warp per destination node
-// (the eager version is a multiply, an index_add into [N, H], a gather back to [E, H], a multiply and a subtract)
+// (the eager version is a multiply, an index_add into [N, H], a gather back to [E, H], a multiply and a subtract).
+// `keep` (optional, [E, H]): the attention-dropout mask applied after the softmax; the cotangent is then ga * keep.
 __global__ void __launch_bounds__(256) seg_softmax_bwd_kernel(const float* __restrict__ alpha, const float* __restrict__ ga,
+                                                              const float* __restrict__ keep,
                                                               const long long* __restrict__ row_ptr, long long n_nodes, int H,
                                                               float* __restrict__ gz) {
   const long long t = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -69,11 +71,15 @@ __global__ void __launch_bounds__(256) seg_softmax_bwd_kernel(const float* __res
   const long long r0 = row_ptr[t], r1 = row_ptr[t + 1];
   for (int h = 0; h < H; ++h) {
     float s = 0.f;
-    for (long long e = r0 + lane; e < r1; e += 32) s += __ldg(alpha + e * H + h) * __ldg(ga + e * H + h);
+    for (long long e = r0 + lane; e < r1; e += 32) {
+      const float g = keep ? __ldg(ga + e * H + h) * __ldg(keep + e * H + h) : __ldg(ga + e * H + h);
+      s += __ldg(alpha + e * H + h) * g;
+    }
     s = warp_add(s);
     for (long long e = r0 + lane; e < r1; e += 32) {
       const float a = __ldg(alpha + e * H + h);
-      gz[e * H + h] = a * (__ldg(ga + e * H + h) - s);
+      const float g = keep ? __ldg(ga + e * H + h) * __ldg(keep + e * H + h) : __ldg(ga + e * H + h);
+      gz[e * H + h] = a * (g - s);
     }
   }
 }
@@ -166,8 +172,9 @@ __global__ void __launch_bounds__(256) edge_dot_kernel(HeadArgs a, const long lo
   }
 }
 
-// elementwise: out[g][e,j] = alpha[e,head(j)] * G[g][dst[e],j]; grid.y = group
+// elementwise: out[g][e,j] = alpha[e,head(j)] (* keep[e,head(j)]) * G[g][dst[e],j]; grid.y = group
 __global__ void __launch_bounds__(256) edge_scale_kernel(HeadArgs a, const float* __restrict__ alpha,
+                                                         const float* __restrict__ keep,
                                                          const long long* __restrict__ dst, long long n_edges) {
   const int g = blockIdx.y;
   const int rowlen = a.rowlen[g];
@@ -179,7 +186,10 @@ __global__ void __launch_bounds__(256) edge_scale_kernel(HeadArgs a, const float
     const int j = (int)(idx - e * rowlen);
     const long long t = dst[e];
     float v = __ldg(a.G[g] + t * rowlen + j);
-    if (alpha != nullptr) v *= __ldg(alpha + e * H + (j % C) / ch);
+    if (alpha != nullptr) {
+      const long long k = e * H + (j % C) / ch;
+      v *= keep ? __ldg(alpha + k) * __ldg(keep + k) : __ldg(alpha + k);
+    }
     a.out[g][idx] = v;
   }
 }
@@ -229,8 +239,10 @@ __global__ void __launch_bounds__(256) aggregate_vec_kernel(HeadArgs a, const fl
 // chunk) first reduces its head's logits over the destination segment (max, then sum of exponentials - the segment is a
 // few dozen edges of one L1-resident row range, every lane of a head reads the same addresses), then accumulates
 // alpha_e V_e with alpha_e = exp(z_e - max) / (sum + 1e-16) computed on the fly; alpha[E, H] is written once (by the lanes
-// that own the first channel of each head in the 0e group) because the backward needs it.
+// that own the first channel of each head in the 0e group) because the backward needs it.  `keep` (optional, [E, H]) is
+// the attention-dropout mask (0 or 1/(1-p)): the sum then runs over alpha_e keep_e V_e, while alpha stays unmasked.
 __global__ void __launch_bounds__(256) softmax_aggregate_vec_kernel(HeadArgs a, const float* __restrict__ z,
+                                                                    const float* __restrict__ keep,
                                                                     const long long* __restrict__ row_ptr, long long n_nodes,
                                                                     float* __restrict__ alpha_out) {
   const int n_chunks = a.chunk_start[a.n_groups];
@@ -256,16 +268,18 @@ __global__ void __launch_bounds__(256) softmax_aggregate_vec_kernel(HeadArgs a, 
   float4 acc0 = make_float4(0.f, 0.f, 0.f, 0.f), acc1 = acc0;
   long long e = r0;
   for (; e + 1 < r1; e += 2) {
-    const float a0 = expf(__ldg(z + e * H + h) - m) * inv, a1 = expf(__ldg(z + (e + 1) * H + h) - m) * inv;
+    float a0 = expf(__ldg(z + e * H + h) - m) * inv, a1 = expf(__ldg(z + (e + 1) * H + h) - m) * inv;
     const float4 v0 = ldv(v + e * rowlen), v1 = ldv(v + (e + 1) * rowlen);
     if (writer) { alpha_out[e * H + h] = a0; alpha_out[(e + 1) * H + h] = a1; }
+    if (keep) { a0 *= __ldg(keep + e * H + h); a1 *= __ldg(keep + (e + 1) * H + h); }
     acc0.x = fmaf(a0, v0.x, acc0.x); acc0.y = fmaf(a0, v0.y, acc0.y); acc0.z = fmaf(a0, v0.z, acc0.z); acc0.w = fmaf(a0, v0.w, acc0.w);
     acc1.x = fmaf(a1, v1.x, acc1.x); acc1.y = fmaf(a1, v1.y, acc1.y); acc1.z = fmaf(a1, v1.z, acc1.z); acc1.w = fmaf(a1, v1.w, acc1.w);
   }
   if (e < r1) {
-    const float a0 = expf(__ldg(z + e * H + h) - m) * inv;
+    float a0 = expf(__ldg(z + e * H + h) - m) * inv;
     const float4 v0 = ldv(v + e * rowlen);
     if (writer) alpha_out[e * H + h] = a0;
+    if (keep) a0 *= __ldg(keep + e * H + h);
     acc0.x = fmaf(a0, v0.x, acc0.x); acc0.y = fmaf(a0, v0.y, acc0.y); acc0.z = fmaf(a0, v0.z, acc0.z); acc0.w = fmaf(a0, v0.w, acc0.w);
   }
   *reinterpret_cast<float4*>(a.out[g] + t * rowlen + j) =
@@ -302,8 +316,9 @@ __global__ void __launch_bounds__(256) edge_dot_vec_kernel(HeadArgs a, const lon
   }
 }
 
-// one warp per edge: out[g][e, j] = alpha[e, head(j)] * G[g][dst[e], j]
+// one warp per edge: out[g][e, j] = alpha[e, head(j)] (* keep[e, head(j)]) * G[g][dst[e], j]
 __global__ void __launch_bounds__(256) edge_scale_vec_kernel(HeadArgs a, const float* __restrict__ alpha,
+                                                             const float* __restrict__ keep,
                                                              const long long* __restrict__ dst, long long n_edges) {
   const int lane = threadIdx.x & 31;
   const long long n_warps = (long long)gridDim.x * (blockDim.x >> 5);
@@ -316,7 +331,8 @@ __global__ void __launch_bounds__(256) edge_scale_vec_kernel(HeadArgs a, const f
       for (int j = lane * 4; j < rowlen; j += 128) {
         float4 v = ldv(gg + j);
         if (alpha != nullptr) {
-          const float s = __ldg(alpha + e * a.n_heads + (j % C) / ch);
+          const long long k = e * a.n_heads + (j % C) / ch;
+          const float s = keep ? __ldg(alpha + k) * __ldg(keep + k) : __ldg(alpha + k);
           v.x *= s; v.y *= s; v.z *= s; v.w *= s;
         }
         *reinterpret_cast<float4*>(o + j) = v;
@@ -365,14 +381,14 @@ extern "C" int eqf_seg_softmax(const float* z, const int64_t* row_ptr, int64_t n
   return check_cuda(cudaGetLastError(), "seg_softmax_kernel launch");
 }
 
-extern "C" int eqf_seg_softmax_bwd(const float* alpha, const float* ga, const int64_t* row_ptr, int64_t n_nodes,
-                                   int32_t n_heads, float* gz, void* stream) {
+extern "C" int eqf_seg_softmax_bwd(const float* alpha, const float* ga, const float* keep, const int64_t* row_ptr,
+                                   int64_t n_nodes, int32_t n_heads, float* gz, void* stream) {
   if (n_nodes == 0) return EQF_OK;
   if (!alpha || !ga || !row_ptr || !gz || n_heads < 1) { set_error("eqf_seg_softmax_bwd: bad arguments"); return EQF_ERR_INVALID; }
   const int wpb = 8;
   const long long blocks = (n_nodes + wpb - 1) / wpb;
   seg_softmax_bwd_kernel<<<(unsigned)blocks, wpb * 32, 0, (cudaStream_t)stream>>>(
-      alpha, ga, reinterpret_cast<const long long*>(row_ptr), n_nodes, n_heads, gz);
+      alpha, ga, keep, reinterpret_cast<const long long*>(row_ptr), n_nodes, n_heads, gz);
   return check_cuda(cudaGetLastError(), "seg_softmax_bwd_kernel launch");
 }
 
@@ -405,7 +421,7 @@ extern "C" int eqf_attn_aggregate(const EqfHeadLayout* lay, const float* alpha, 
 // out[g][t] = sum_{e -> t} softmax_t(z)[e, head] V[g][e]  and  alpha[E, H] = the softmax (PyG semantics) in ONE launch.
 // Needs the float4 layout (every group's channels % 4 == 0), a leading group with one component (0e) whose channels per
 // head are a multiple of 4 (it is the one whose lanes write alpha); EQF_ERR_UNSUPPORTED otherwise.
-extern "C" int eqf_attn_softmax_aggregate(const EqfHeadLayout* lay, const float* z, const float* const* V,
+extern "C" int eqf_attn_softmax_aggregate(const EqfHeadLayout* lay, const float* z, const float* keep, const float* const* V,
                                           const int64_t* row_ptr, int64_t n_nodes, float* const* out, float* alpha,
                                           void* stream) {
   HeadArgs a;
@@ -425,7 +441,7 @@ extern "C" int eqf_attn_softmax_aggregate(const EqfHeadLayout* lay, const float*
   const int wpb = 8;
   const long long warps = n_nodes * a.chunk_start[a.n_groups];
   softmax_aggregate_vec_kernel<<<(unsigned)((warps + wpb - 1) / wpb), wpb * 32, 0, (cudaStream_t)stream>>>(
-      a, z, reinterpret_cast<const long long*>(row_ptr), n_nodes, alpha);
+      a, z, keep, reinterpret_cast<const long long*>(row_ptr), n_nodes, alpha);
   return check_cuda(cudaGetLastError(), "softmax_aggregate_vec_kernel launch");
 }
 
@@ -457,12 +473,13 @@ extern "C" int eqf_attn_edge_dot(const EqfHeadLayout* lay, const float* const* V
   return check_cuda(cudaGetLastError(), "edge_dot_kernel launch");
 }
 
-extern "C" int eqf_attn_edge_scale(const EqfHeadLayout* lay, const float* alpha, const float* const* G,
+extern "C" int eqf_attn_edge_scale(const EqfHeadLayout* lay, const float* alpha, const float* keep, const float* const* G,
                                    const int64_t* dst, int64_t n_edges, float* const* out, void* stream) {
   HeadArgs a;
   int rc = fill_head_args(lay, a);
   if (rc != EQF_OK || n_edges == 0) return rc;
   if (G == nullptr || dst == nullptr || out == nullptr) { set_error("eqf_attn_edge_scale: null pointer"); return EQF_ERR_INVALID; }
+  if (keep != nullptr && alpha == nullptr) { set_error("eqf_attn_edge_scale: keep needs alpha"); return EQF_ERR_INVALID; }
   int max_rowlen = 0;
   for (int g = 0; g < a.n_groups; ++g) {
     if (G[g] == nullptr || out[g] == nullptr) { set_error("eqf_attn_edge_scale: null group"); return EQF_ERR_INVALID; }
@@ -473,13 +490,13 @@ extern "C" int eqf_attn_edge_scale(const EqfHeadLayout* lay, const float* alpha,
     long long vb = (n_edges + 7) / 8;
     if (vb > 132LL * 16) vb = 132LL * 16;
     edge_scale_vec_kernel<<<(unsigned)(vb < 1 ? 1 : vb), 256, 0, (cudaStream_t)stream>>>(
-        a, alpha, reinterpret_cast<const long long*>(dst), n_edges);
+        a, alpha, keep, reinterpret_cast<const long long*>(dst), n_edges);
     return check_cuda(cudaGetLastError(), "edge_scale_vec_kernel launch");
   }
   long long blocks = (n_edges * max_rowlen + 255) / 256;
   if (blocks > 132LL * 32) blocks = 132LL * 32;
   if (blocks < 1) blocks = 1;
   dim3 grid((unsigned)blocks, (unsigned)a.n_groups);
-  edge_scale_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(a, alpha, reinterpret_cast<const long long*>(dst), n_edges);
+  edge_scale_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(a, alpha, keep, reinterpret_cast<const long long*>(dst), n_edges);
   return check_cuda(cudaGetLastError(), "edge_scale_kernel launch");
 }

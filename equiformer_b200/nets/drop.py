@@ -1,7 +1,8 @@
 """Regularisers (drop-in for ``nets/drop.py``): stochastic depth per graph and irrep-wise dropout.
 
-Out of the hot path (all rates are 0 in the benchmark configurations except ``alpha_drop``, which is a plain
-``nn.Dropout``); kept so that the reference's constructors and training mode work unchanged.
+Kept so that the reference's constructors and training mode work unchanged.  ``GraphDropPath`` also hands its per-node
+factor to the planar transformer blocks (``TransBlock.forward_planar``) and, given the number of graphs, draws without
+a host synchronisation.  (``alpha_drop`` is drawn in ``GraphAttention`` and applied inside the fused attention kernel.)
 """
 from __future__ import annotations
 
@@ -38,10 +39,17 @@ class GraphDropPath(nn.Module):
         super().__init__()
         self.drop_prob = drop_prob
 
-    def forward(self, x, batch):
-        n_graphs = int(batch.max()) + 1
+    def forward(self, x, batch, n_graphs=None):
+        return x * self.node_scale(x, batch, n_graphs)
+
+    def node_scale(self, x, batch, n_graphs=None):
+        """The per-node factor (0 or 1/(1-p), 1 outside training) shaped to broadcast against ``x``.  ``n_graphs`` (the
+        number of graphs in the batch) avoids reading ``batch.max()`` on the host, so the draw can be captured in a CUDA
+        graph; it makes the same draws."""
+        if n_graphs is None:
+            n_graphs = int(batch.max()) + 1
         ones = torch.ones((n_graphs,) + (1,) * (x.ndim - 1), dtype=x.dtype, device=x.device)
-        return x * drop_path(ones, self.drop_prob, self.training)[batch]
+        return drop_path(ones, self.drop_prob, self.training)[batch]
 
     def extra_repr(self) -> str:
         return f"drop_prob={self.drop_prob}"

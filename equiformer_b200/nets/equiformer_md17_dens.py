@@ -148,7 +148,7 @@ class Equiformer_MD17_DeNS(torch.nn.Module):
         node_features = node_features + self.force_embed(force_sh)
 
         node_features = _run_blocks(self.blocks, node_features, self.irreps_node_embedding, node_attr, edge_src, edge_dst,
-                                    edge_sh, edge_length_embedding, batch, graph)
+                                    edge_sh, edge_length_embedding, batch, graph, getattr(data, "n_graphs", None))
         node_features = self.norm(node_features, batch=batch)
         if self.out_dropout is not None:
             node_features = self.out_dropout(node_features)

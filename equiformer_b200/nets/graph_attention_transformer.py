@@ -419,9 +419,16 @@ class GraphAttention(torch.nn.Module):
         # logits -> segment softmax -> weighted aggregation                               [ref :506-513]
         z = logits if logits is not None else (self.alpha_act(alpha) * self.alpha_dot).sum(dim=-1)
         no_drop = self.alpha_dropout is None or not self.training or self.alpha_dropout.p == 0.0
-        if no_drop and ops.softmax_aggregate_ok(self._head_layout, z):
+        if ops.softmax_aggregate_ok(self._head_layout, z):
             # K2: softmax over the destination segment and the weighted aggregation in one kernel
-            node = list(ops.SoftmaxAggregate.apply(self._head_layout, graph, z.contiguous(), *[v.contiguous() for v in value]))
+            vs = [v.contiguous() for v in value]
+            if no_drop:
+                node = list(ops.SoftmaxAggregate.apply(self._head_layout, graph, z.contiguous(), *vs))
+            else:
+                # [ref :509] the dropout mask, drawn as nn.Dropout draws it on the [E, H] weights (same generator use,
+                # capturable), is applied inside K2 and its backward
+                keep = torch.nn.functional.dropout(torch.ones_like(z), self.alpha_dropout.p, True)
+                node = list(ops.MaskedSoftmaxAggregate.apply(self._head_layout, graph, z.contiguous(), keep, *vs))
         else:
             attn = ops.segment_softmax(z.contiguous(), graph)
             if self.alpha_dropout is not None:
@@ -548,23 +555,30 @@ class TransBlock(torch.nn.Module):
         features = self.norm_1(node_input, batch=batch)
         features = self.attention(node_input=features, node_attr=node_attr, edge_src=edge_src, edge_dst=edge_dst,
                                   edge_attr=edge_attr, edge_scalars=edge_scalars, batch=batch, **kwargs)
+        n_graphs = kwargs.get("n_graphs")
         if self.drop_path is not None:
-            features = self.drop_path(features, batch)
+            features = self._drop_path(features, batch, n_graphs)
         node_output = node_input + features
 
         features = self.ffn(self.norm_2(node_output, batch=batch), node_attr)
         if self.ffn_shortcut is not None:
             node_output = self.ffn_shortcut(node_output, node_attr)
         if self.drop_path is not None:
-            features = self.drop_path(features, batch)
+            features = self._drop_path(features, batch, n_graphs)
         return node_output + features
+
+    def _drop_path(self, features, batch, n_graphs):
+        # n_graphs is handed over only when known, so a module with the reference's (x, batch) signature still fits
+        return self.drop_path(features, batch) if n_graphs is None else self.drop_path(features, batch, n_graphs=n_graphs)
 
     @property
     def supports_planar(self) -> bool:
-        """The whole block can run on planar node blocks: fused LayerNorms, no shortcut projection, no stochastic depth
-        or output dropout in effect."""
+        """The whole block can run on planar node blocks: fused LayerNorms, no shortcut projection, no output dropout in
+        effect, and stochastic depth (in training) only through ``GraphDropPath``, whose per-graph factor the planar route
+        applies itself."""
         return (getattr(self.norm_1, "supports_planar", False) and getattr(self.norm_2, "supports_planar", False)
-                and self.ffn_shortcut is None and (self.drop_path is None or not self.training)
+                and self.ffn_shortcut is None
+                and (self.drop_path is None or not self.training or type(self.drop_path) is GraphDropPath)
                 and self.attention.supports_planar and self.ffn.supports_planar
                 and self.irreps_node_input == self.irreps_node_output)
 
@@ -573,9 +587,17 @@ class TransBlock(torch.nn.Module):
         (saves the layout copies at every sub-layer boundary, ~24 small launches per block and step)."""
         f = self.attention.forward_planar(self.norm_1.planar(xs), node_attr, edge_src, edge_dst, edge_attr, edge_scalars,
                                           batch, **kwargs)
-        xs = [a + b for a, b in zip(xs, f)]
+        xs = self._residual(xs, f, batch, kwargs.get("n_graphs"))
         f = self.ffn.forward_planar(self.norm_2.planar(xs), node_attr)
-        return [a + b for a, b in zip(xs, f)]
+        return self._residual(xs, f, batch, kwargs.get("n_graphs"))
+
+    def _residual(self, xs, f, batch, n_graphs):
+        """``x + drop_path(f)`` on planar blocks: one per-node keep factor (drawn like the stock route draws it, attention
+        branch first) scales every block of the branch."""
+        if self.drop_path is None or not self.training:
+            return [a + b for a, b in zip(xs, f)]
+        s = self.drop_path.node_scale(f[0], batch, n_graphs)
+        return [torch.addcmul(a, b, s) for a, b in zip(xs, f)]
 
 
 class NodeEmbeddingNetwork(torch.nn.Module):
@@ -768,7 +790,7 @@ class GraphAttentionTransformer(torch.nn.Module):
             node_attr = torch.ones_like(node_features.narrow(1, 0, 1))
             node_attr._eqf_all_ones = True          # lets the node-level FCTPs skip the multiply by the constant 1
             node_features = _run_blocks(self.blocks, node_features, self.irreps_node_embedding, node_attr, edge_src, edge_dst,
-                                        edge_sh, edge_length_embedding, batch, graph)
+                                        edge_sh, edge_length_embedding, batch, graph, n_graphs)
         finally:
             clear_hoisted(served)
         node_features = self.norm(node_features, batch=batch)
@@ -804,12 +826,14 @@ def hoist_radial(model, edge_scalars):
     return hoist_first_layers(mods, edge_scalars)
 
 
-def _run_blocks(blocks, node_features, irreps, node_attr, edge_src, edge_dst, edge_sh, edge_scalars, batch, graph):
-    """The transformer blocks; consecutive blocks that support it keep the node features in planar blocks."""
+def _run_blocks(blocks, node_features, irreps, node_attr, edge_src, edge_dst, edge_sh, edge_scalars, batch, graph,
+                n_graphs=None):
+    """The transformer blocks; consecutive blocks that support it keep the node features in planar blocks.  ``n_graphs``
+    lets stochastic depth draw its per-graph factors without reading the batch vector on the host."""
     planar = None
     for blk in blocks:
         kw = dict(node_attr=node_attr, edge_src=edge_src, edge_dst=edge_dst, edge_attr=edge_sh, edge_scalars=edge_scalars,
-                  batch=batch, graph=graph)
+                  batch=batch, graph=graph, n_graphs=n_graphs)
         if getattr(blk, "supports_planar", False) and ops.fused_ok(node_features if planar is None else planar[0]):
             if planar is None:
                 planar = ops.to_planar(node_features, Irreps(irreps))

@@ -139,7 +139,7 @@ class GraphAttentionTransformerMD17(torch.nn.Module):
         node_attr = torch.ones_like(node_features.narrow(1, 0, 1))
         node_attr._eqf_all_ones = True
         node_features = _run_blocks(self.blocks, node_features, self.irreps_node_embedding, node_attr, edge_src, edge_dst,
-                                    edge_sh, edge_length_embedding, batch, graph)
+                                    edge_sh, edge_length_embedding, batch, graph, n_graphs)
         node_features = self.norm(node_features, batch=batch)
         if self.out_dropout is not None:
             node_features = self.out_dropout(node_features)

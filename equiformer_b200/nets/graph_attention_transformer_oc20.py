@@ -175,7 +175,7 @@ class GraphAttentionTransformerOC20(torch.nn.Module):
             node_attr = torch.ones_like(node_features.narrow(1, 0, 1))
             node_attr._eqf_all_ones = True
             node_features = _run_blocks(self.blocks, node_features, self.irreps_node_embedding, node_attr, edge_src, edge_dst,
-                                        edge_sh, edge_length_embedding, batch, graph)
+                                        edge_sh, edge_length_embedding, batch, graph, n_graphs)
             node_features = self.norm(node_features, batch=batch)
             outputs_aux = None
             if self.use_auxiliary_task:                # IS2RS head on the normed features, before out_dropout (ref :372-379)

@@ -830,12 +830,24 @@ def seg_softmax_raw(z: torch.Tensor, graph: Graph) -> torch.Tensor:
     return alpha
 
 
-def seg_softmax_bwd_raw(alpha: torch.Tensor, ga: torch.Tensor, graph: Graph) -> torch.Tensor:
+def _keep_ptr(keep: Optional[torch.Tensor], like: torch.Tensor):
+    """Device pointer of an optional attention-dropout mask ``[E, H]`` (None: no mask)."""
+    if keep is None:
+        return None
+    keep = _require_cuda(keep, "dropout mask")
+    if keep.shape != like.shape or keep.dtype != like.dtype:
+        raise ValueError("the dropout mask must match the attention weights [E, H]")
+    return keep.data_ptr()
+
+
+def seg_softmax_bwd_raw(alpha: torch.Tensor, ga: torch.Tensor, graph: Graph, keep=None) -> torch.Tensor:
+    """Softmax backward; with ``keep`` (the dropout mask applied after the softmax) the cotangent is ``ga * keep``."""
     ga = _require_cuda(ga, "softmax cotangent").contiguous()
     gz = torch.empty_like(alpha)
-    with torch.cuda.device(alpha.device), _kernel("seg_softmax_bwd", 12 * alpha.numel()):
-        rc = _lib.load().eqf_seg_softmax_bwd(alpha.data_ptr(), ga.data_ptr(), graph.row_ptr.data_ptr(), graph.n_nodes,
-                                             alpha.shape[1], gz.data_ptr(), _stream())
+    nbytes = (12 + (4 if keep is not None else 0)) * alpha.numel()
+    with torch.cuda.device(alpha.device), _kernel("seg_softmax_bwd", nbytes):
+        rc = _lib.load().eqf_seg_softmax_bwd(alpha.data_ptr(), ga.data_ptr(), _keep_ptr(keep, alpha), graph.row_ptr.data_ptr(),
+                                             graph.n_nodes, alpha.shape[1], gz.data_ptr(), _stream())
     _lib.check(rc, "eqf_seg_softmax_bwd")
     return gz
 
@@ -873,15 +885,18 @@ def attn_edge_dot_raw(lay: HeadLayout, Vs, Gs, graph: Graph) -> torch.Tensor:
     return out
 
 
-def attn_edge_scale_raw(lay: HeadLayout, alpha, Gs, graph: Graph) -> List[torch.Tensor]:
+def attn_edge_scale_raw(lay: HeadLayout, alpha, Gs, graph: Graph, keep=None) -> List[torch.Tensor]:
+    """``outs[g][e] = alpha[e, head] keep[e, head] G[g][dst e]`` (alpha None: gather; keep None: no mask)."""
     Gs = lay.check(Gs, graph.n_nodes, "edge_scale G")
     if alpha is not None:
         alpha = _require_cuda(alpha, "alpha")
+    elif keep is not None:
+        raise ValueError("edge_scale: a dropout mask needs alpha")
     dev = Gs[0].device
     outs = [torch.empty((graph.n_edges, d, C), device=dev, dtype=torch.float32) for d, C in zip(lay.ds, lay.Cs)]
     with torch.cuda.device(dev), _kernel("attn_edge_scale", _attn_bytes(lay, graph.n_edges, graph.n_nodes, "edge_scale")):
         rc = _lib.load().eqf_attn_edge_scale(ctypes.byref(lay.c), alpha.data_ptr() if alpha is not None else None,
-                                             _ptr_array(Gs), graph.dst.data_ptr(), graph.n_edges,
+                                             _keep_ptr(keep, alpha), _ptr_array(Gs), graph.dst.data_ptr(), graph.n_edges,
                                              _ptr_array(outs), _stream())
     _lib.check(rc, "eqf_attn_edge_scale")
     return outs
@@ -998,8 +1013,10 @@ class EdgeScale(torch.autograd.Function):
         return (None, None, ga, *gGs)
 
 
-def softmax_aggregate_raw(lay: HeadLayout, z: torch.Tensor, Vs, graph: Graph):
-    """(outs, alpha): segment softmax of ``z`` and the alpha-weighted segment sums of ``Vs`` in one kernel."""
+def softmax_aggregate_raw(lay: HeadLayout, z: torch.Tensor, Vs, graph: Graph, keep=None):
+    """(outs, alpha): segment softmax of ``z`` and the alpha-weighted segment sums of ``Vs`` in one kernel.  With ``keep``
+    (the attention-dropout mask, ``[E, H]`` of 0 or 1/(1-p)) the sums are weighted by ``alpha * keep``; ``alpha`` is
+    returned without the mask."""
     Vs = lay.check(Vs, graph.n_edges, "softmax_aggregate V")
     z = _require_cuda(z, "attention logits")
     if tuple(z.shape) != (graph.n_edges, lay.n_heads):
@@ -1007,10 +1024,11 @@ def softmax_aggregate_raw(lay: HeadLayout, z: torch.Tensor, Vs, graph: Graph):
     dev = z.device
     outs = [torch.empty((graph.n_nodes, d, C), device=dev, dtype=torch.float32) for d, C in zip(lay.ds, lay.Cs)]
     alpha = torch.empty_like(z)
-    nbytes = _attn_bytes(lay, graph.n_edges, graph.n_nodes, "aggregate") + 4 * z.numel()
+    nbytes = _attn_bytes(lay, graph.n_edges, graph.n_nodes, "aggregate") + (4 if keep is None else 8) * z.numel()
     with torch.cuda.device(dev), _kernel("softmax_aggregate", nbytes):
-        rc = _lib.load().eqf_attn_softmax_aggregate(ctypes.byref(lay.c), z.data_ptr(), _ptr_array(Vs), graph.row_ptr.data_ptr(),
-                                                    graph.n_nodes, _ptr_array(outs), alpha.data_ptr(), _stream())
+        rc = _lib.load().eqf_attn_softmax_aggregate(ctypes.byref(lay.c), z.data_ptr(), _keep_ptr(keep, z), _ptr_array(Vs),
+                                                    graph.row_ptr.data_ptr(), graph.n_nodes, _ptr_array(outs),
+                                                    alpha.data_ptr(), _stream())
     _lib.check(rc, "eqf_attn_softmax_aggregate")
     return outs, alpha
 
@@ -1020,6 +1038,40 @@ def softmax_aggregate_ok(lay: HeadLayout, z: torch.Tensor) -> bool:
     return (fused_ok(z) and lay.ds[0] == 1 and all((c // lay.n_heads) % 4 == 0 for c in lay.Cs) and z.shape[0] > 0)
 
 
+def _softmax_aggregate_forward(ctx, lay: HeadLayout, graph: Graph, z, keep, Vs):
+    # the mask operand is passed only when there is one, so the unmasked route calls exactly what it always called
+    extra = () if keep is None else (keep,)
+    outs, alpha = softmax_aggregate_raw(lay, z, Vs, graph, *extra)
+    ctx.lay, ctx.graph, ctx.has_keep = lay, graph, keep is not None
+    ctx.save_for_backward(z, alpha, *extra, *Vs)
+    return tuple(outs)
+
+
+def _softmax_aggregate_backward(ctx, Gs, need_z: bool, need_V: bool):
+    """(gz, gVs) of K2.  First order: edge_dot -> segment-softmax backward (cotangent * keep) and edge_scale (alpha * keep),
+    the same three launches with or without the mask.  Under ``create_graph`` the softmax is rebuilt differentiably and
+    ``AttnAggregate(SegSoftmax(z) * keep, V)`` - the mask is a constant - keeps the closed families in charge."""
+    lay, graph = ctx.lay, ctx.graph
+    z, alpha, *rest = ctx.saved_tensors
+    keep, Vs = (rest[0], rest[1:]) if ctx.has_keep else (None, rest)
+    extra = () if keep is None else (keep,)
+    Gs = [G.contiguous() if G is not None else torch.zeros((graph.n_nodes, d, C), device=z.device)
+          for G, d, C in zip(Gs, lay.ds, lay.Cs)]
+    if torch.is_grad_enabled():
+        def fn(zz, *vv):
+            a = SegSoftmax.apply(zz, graph)
+            return tuple(AttnAggregate.apply(lay, graph, a if keep is None else a * keep, *vv))
+        gz, *gVs = _higher_order_grads(fn, (z, *Vs), Gs)
+        return gz, gVs
+    gz = None
+    gVs = [None] * len(Vs)
+    if need_z:
+        gz = seg_softmax_bwd_raw(alpha, attn_edge_dot_raw(lay, Vs, Gs, graph), graph, *extra)
+    if need_V:
+        gVs = attn_edge_scale_raw(lay, alpha, Gs, graph, *extra)
+    return gz, gVs
+
+
 class SoftmaxAggregate(torch.autograd.Function):
     """K2 (ref :508-513): ``outs[g][t] = sum_{e->t} softmax_t(z)[e, head] V[g][e]`` - softmax and aggregation in one launch.
     apply(lay, graph, z, *Vs).  Backward: EdgeDot / EdgeScale / segment-softmax backward on the saved alpha; under
@@ -1027,29 +1079,27 @@ class SoftmaxAggregate(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, lay: HeadLayout, graph: Graph, z, *Vs):
-        outs, alpha = softmax_aggregate_raw(lay, z, Vs, graph)
-        ctx.lay, ctx.graph = lay, graph
-        ctx.save_for_backward(z, alpha, *Vs)
-        return tuple(outs)
+        return _softmax_aggregate_forward(ctx, lay, graph, z, None, Vs)
 
     @staticmethod
     def backward(ctx, *Gs):
-        lay, graph = ctx.lay, ctx.graph
-        z, alpha, *Vs = ctx.saved_tensors
-        Gs = [G.contiguous() if G is not None else torch.zeros((graph.n_nodes, d, C), device=z.device)
-              for G, d, C in zip(Gs, lay.ds, lay.Cs)]
-        need_z, need_V = ctx.needs_input_grad[2], any(ctx.needs_input_grad[3:])
-        if torch.is_grad_enabled():
-            fn = lambda zz, *vv: tuple(AttnAggregate.apply(lay, graph, SegSoftmax.apply(zz, graph), *vv))
-            grads = _higher_order_grads(fn, (z, *Vs), Gs)
-            return (None, None, *grads)
-        gz = None
-        gVs = [None] * len(Vs)
-        if need_z:
-            gz = seg_softmax_bwd_raw(alpha, attn_edge_dot_raw(lay, Vs, Gs, graph), graph)
-        if need_V:
-            gVs = attn_edge_scale_raw(lay, alpha, Gs, graph)
+        gz, gVs = _softmax_aggregate_backward(ctx, Gs, ctx.needs_input_grad[2], any(ctx.needs_input_grad[3:]))
         return (None, None, gz, *gVs)
+
+
+class MaskedSoftmaxAggregate(torch.autograd.Function):
+    """K2 with attention-weight dropout (ref :508-513 with ``alpha_dropout`` at :509): ``outs[g][t] = sum_{e->t}
+    softmax_t(z)[e, head] keep[e, head] V[g][e]``.  apply(lay, graph, z, keep, *Vs); ``keep`` ``[E, H]`` holds 0 or
+    1/(1-p) (what ``nn.Dropout`` multiplies by) and gets no gradient; ``keep=None`` is ``SoftmaxAggregate``."""
+
+    @staticmethod
+    def forward(ctx, lay: HeadLayout, graph: Graph, z, keep, *Vs):
+        return _softmax_aggregate_forward(ctx, lay, graph, z, keep, Vs)
+
+    @staticmethod
+    def backward(ctx, *Gs):
+        gz, gVs = _softmax_aggregate_backward(ctx, Gs, ctx.needs_input_grad[2], any(ctx.needs_input_grad[4:]))
+        return (None, None, gz, None, *gVs)
 
 
 def attention_aggregate(lay: HeadLayout, graph: Graph, alpha: Optional[torch.Tensor], Vs: Sequence[torch.Tensor]):

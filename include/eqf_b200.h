@@ -119,9 +119,10 @@ typedef struct {
  * at graph_attention_transformer.py:508 (PyG 2.0.3 semantics).  row_ptr is the CSR of edge_dst.   */
 int eqf_seg_softmax(const float* z, const int64_t* row_ptr, int64_t n_nodes, int32_t n_heads,
                     float* alpha, void* stream);
-/* its backward: gz[e,h] = alpha[e,h] (ga[e,h] - sum_{f -> dst(e)} alpha[f,h] ga[f,h]) */
-int eqf_seg_softmax_bwd(const float* alpha, const float* ga, const int64_t* row_ptr, int64_t n_nodes, int32_t n_heads,
-                        float* gz, void* stream);
+/* its backward: gz[e,h] = alpha[e,h] (ga'[e,h] - sum_{f -> dst(e)} alpha[f,h] ga'[f,h]) with ga' = ga * keep, where
+ * keep [E][H] (may be NULL: ga' = ga) is the attention-dropout mask that followed the softmax (:509).           */
+int eqf_seg_softmax_bwd(const float* alpha, const float* ga, const float* keep, const int64_t* row_ptr, int64_t n_nodes,
+                        int32_t n_heads, float* gz, void* stream);
 
 /* out[g][t,j] = sum_{e in seg(t)} alpha[e,head(j)] * V[g][e,j]   (alpha NULL: plain segment sum)
  * == value*alpha followed by torch_scatter.scatter(..., edge_dst) (:512-513).
@@ -133,15 +134,18 @@ int eqf_attn_aggregate(const EqfHeadLayout* lay, const float* alpha, const float
  * in ONE kernel over the destination-sorted edge list: out[g][t] = sum_{e->t} softmax_t(z)[e, head] V[g][e], one warp per
  * (node, 128 columns), no atomics; alpha [E][H] (the softmax itself) is written once for the backward.  Needs the float4
  * layout and a leading 0e group (EQF_ERR_UNSUPPORTED otherwise - callers fall back to eqf_seg_softmax + eqf_attn_aggregate). */
-int eqf_attn_softmax_aggregate(const EqfHeadLayout* lay, const float* z, const float* const* V,
+/* keep [E][H] (may be NULL) is the attention-dropout mask (:509), entries 0 or 1/(1-p): the sum then runs over
+ * softmax * keep * V, while alpha is still written without the mask (the softmax backward needs it).                */
+int eqf_attn_softmax_aggregate(const EqfHeadLayout* lay, const float* z, const float* keep, const float* const* V,
                                const int64_t* row_ptr, int64_t n_nodes, float* const* out, float* alpha, void* stream);
 
 /* galpha[e,h] = sum_{j in head h} V[g][e,j] * G[g][dst[e],j]       (transpose of aggregate w.r.t. alpha) */
 int eqf_attn_edge_dot(const EqfHeadLayout* lay, const float* const* V, const float* const* G,
                       const int64_t* dst, int64_t n_edges, float* galpha, void* stream);
 
-/* out[g][e,j] = alpha[e,head(j)] * G[g][dst[e],j]                  (transpose w.r.t. V; alpha NULL: gather) */
-int eqf_attn_edge_scale(const EqfHeadLayout* lay, const float* alpha, const float* const* G,
+/* out[g][e,j] = alpha[e,head(j)] * keep[e,head(j)] * G[g][dst[e],j]  (transpose w.r.t. V; alpha NULL: gather;
+ * keep NULL: no mask; keep needs alpha)                                                                              */
+int eqf_attn_edge_scale(const EqfHeadLayout* lay, const float* alpha, const float* keep, const float* const* G,
                         const int64_t* dst, int64_t n_edges, float* const* out, void* stream);
 
 /* ---- fused pointwise kernels around the GEMMs -------------------------------------------------------------------

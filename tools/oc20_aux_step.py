@@ -3,6 +3,7 @@
 
     python tools/oc20_aux_step.py --workload aux6  [--steps K --warmup W]   # OC20_L1_256_NONLINEAR_AUX, 16 frames
     python tools/oc20_aux_step.py --workload aux18 [--eager]                # OC20_L1_256_BLOCKS18_NONLINEAR_AUX, 8 frames
+    python tools/oc20_aux_step.py --workload aux6 --drop-path-rate 0 --alpha-drop 0    # regularisers off
 
 Inputs are ``synthetic.oc20_like_frames`` (as ``bench.py --workload oc20_l1``) plus seeded relaxed positions.  One step:
 
@@ -13,10 +14,10 @@ Inputs are ``synthetic.oc20_like_frames`` (as ``bench.py --workload oc20_l1``) p
 4. AdamW (``parallel.FlatAdamW``, lr 5e-4, weight decay 1e-3 as in the configurations).
 
 The interpolation generator is re-seeded every step, so every step sees the same positions and edge count and the one
-capture is replayed (a new edge count would need a new capture).  Both configurations set ``drop_path_rate=0.05``, and
-``GraphDropPath`` reads ``batch.max()`` on the host, which a CUDA graph cannot capture: by default the step is captured with
-the rate at 0; ``--eager`` times it without capture at the configured rate.  The JSON line says which one was timed.
-Attention-weight dropout is 0 unless ``--alpha-drop`` says otherwise (as in ``bench.py``).
+capture is replayed (a new edge count would need a new capture).  The regularisers run as configured (``drop_path_rate=0.05``,
+``alpha_drop=0.2``) unless ``--drop-path-rate`` / ``--alpha-drop`` override them: stochastic depth draws its per-graph
+factors from ``n_graphs`` and attention dropout draws its mask with torch's generator, so both are captured and every
+replay draws afresh.  ``--eager`` times the same step without capture.  The JSON line says what was timed.
 """
 from __future__ import annotations
 
@@ -44,8 +45,9 @@ def main():
     ap.add_argument("--workload", choices=sorted(WORKLOADS), default="aux6")
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
-    ap.add_argument("--eager", action="store_true", help="no CUDA graph; stochastic depth at the configured rate")
-    ap.add_argument("--alpha-drop", type=float, default=0.0)
+    ap.add_argument("--eager", action="store_true", help="no CUDA graph")
+    ap.add_argument("--drop-path-rate", type=float, default=None, help="stochastic depth rate (default: as configured)")
+    ap.add_argument("--alpha-drop", type=float, default=None, help="attention-weight dropout (default: as configured)")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise RuntimeError("oc20_aux_step.py needs a CUDA device")
@@ -63,9 +65,11 @@ def main():
     torch.cuda.set_device(dev)
     torch.backends.cuda.matmul.allow_tf32 = False
     cfg_name, n_frames, pos_std = WORKLOADS[args.workload]
-    cfg = dict(getattr(M, cfg_name), alpha_drop=args.alpha_drop)
-    if not args.eager:
-        cfg["drop_path_rate"] = 0.0
+    cfg = dict(getattr(M, cfg_name))
+    if args.drop_path_rate is not None:
+        cfg["drop_path_rate"] = args.drop_path_rate
+    if args.alpha_drop is not None:
+        cfg["alpha_drop"] = args.alpha_drop
     torch.manual_seed(0)
     model = M.GraphAttentionTransformerOC20(None, None, 1, **cfg).to(dev).train()
     bucket = FlatGradAllReduce(model.parameters())
@@ -133,10 +137,11 @@ def main():
         "metric": f"edges/sec fwd+bwd, OC20 IS2RE {cfg_name} + IS2RS auxiliary loss", "workload": args.workload,
         "value": e / (ms * 1e-3), "unit": "edges/s", "ms_per_step": ms, "steps": args.steps, "edges_per_step": e,
         "atoms_per_step": n, "frames": n_frames, "num_layers": cfg["num_layers"],
-        "launch": ("eager (no CUDA graph), drop_path_rate %g as configured" % cfg["drop_path_rate"] if args.eager else
-                   "CUDA-graph replay of forward+loss+backward with drop_path_rate 0 (configured 0.05); interpolation, "
-                   "neighbour list and AdamW eager"),
-        "alpha_drop": args.alpha_drop, "captures": getattr(graphed, "captures", None), "loss": loss.item(),
+        "launch": ("eager (no CUDA graph)" if args.eager else
+                   "CUDA-graph replay of forward+loss+backward; interpolation, neighbour list and AdamW eager"),
+        "drop_path_rate": cfg["drop_path_rate"], "alpha_drop": cfg["alpha_drop"],
+        "configured": {"drop_path_rate": getattr(M, cfg_name)["drop_path_rate"], "alpha_drop": getattr(M, cfg_name)["alpha_drop"]},
+        "captures": getattr(graphed, "captures", None), "loss": loss.item(),
         "max_memory_gb": torch.cuda.max_memory_allocated(dev) / 1e9,
         "device": torch.cuda.get_device_name(dev), "power_limit_w": bench.power_limit(0),
     }), flush=True)
