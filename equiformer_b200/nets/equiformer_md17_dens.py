@@ -123,10 +123,42 @@ class Equiformer_MD17_DeNS(torch.nn.Module):
 
     @torch.enable_grad()
     def forward(self, data):
+        """``(energy, dy)`` of a batch (ref :238-354).  The attributes present on ``data`` select the branches as in the
+        reference: ``force`` the force encoding (with ``noise_mask``), ``noise_mask`` the denoising head, and, only when
+        ``use_force_encoding=False``, ``denoising_mask`` / ``denoising_pos_mask`` the masking of energies / outputs."""
         node_atom, pos, batch = data.z, data.pos, data.batch
         pos = pos.requires_grad_(True)
         edge_src, edge_dst = radius_graph(pos, r=self.max_radius, batch=batch, max_num_neighbors=1000)
-        graph = ops.Graph(edge_src, edge_dst, pos.shape[0], check_sorted=False)
+        force = noise_mask = denoising_mask = denoising_pos_mask = None
+        if hasattr(data, "force") and self.use_force_encoding:
+            force, noise_mask = data.force, data.noise_mask
+        if hasattr(data, "noise_mask"):
+            noise_mask = data.noise_mask
+            if not self.use_force_encoding:
+                denoising_pos_mask = data.denoising_pos_mask
+        if hasattr(data, "denoising_mask") and not self.use_force_encoding:
+            denoising_mask = data.denoising_mask
+        return self.forward_edges(node_atom, pos, batch, edge_src, edge_dst, force=force, noise_mask=noise_mask,
+                                  n_graphs=getattr(data, "n_graphs", None), denoising_mask=denoising_mask,
+                                  denoising_pos_mask=denoising_pos_mask)
+
+    @torch.enable_grad()
+    def forward_edges(self, node_atom, pos, batch, edge_src, edge_dst, force=None, noise_mask=None, graph=None,
+                      n_graphs=None, denoising_mask=None, denoising_pos_mask=None):
+        """Everything after the neighbour search: ``(energy, dy)`` with ``dy = -dE/dpos`` (``create_graph=True``) for
+        the clean atoms and the predicted noise for the atoms in ``noise_mask``.
+
+        * ``force`` ``[N, 3]`` (with ``noise_mask``) is encoded for the atoms in ``noise_mask`` when
+          ``use_force_encoding``; without it the encoding input is zero.
+        * ``noise_mask`` ``[N]`` bool runs the denoising head; without it ``dy`` is the forces of every atom.
+        * ``denoising_mask`` / ``denoising_pos_mask`` (only read when ``use_force_encoding=False``) zero the energies /
+          outputs of the denoised atoms, as the reference does.
+
+        ``pos`` must require grad.  With ``graph`` (CSR of the destination-sorted edge list) and ``n_graphs`` supplied
+        nothing here synchronises with the host, so the whole energy + force + denoising step can be captured in a CUDA
+        graph."""
+        if graph is None:
+            graph = ops.Graph(edge_src, edge_dst, pos.shape[0], check_sorted=False)
         _vec, edge_length, edge_sh = edge_features(self.irreps_edge_attr, pos, graph)
         atom_embedding, _attr, _onehot = self.atom_embed(node_atom)
         edge_length_embedding = self.rbf(edge_length)
@@ -137,38 +169,42 @@ class Equiformer_MD17_DeNS(torch.nn.Module):
         node_attr._eqf_all_ones = True
 
         # forces of the corrupted atoms as an equivariant input (ref :273-292)
-        if hasattr(data, "force") and self.use_force_encoding:
-            force_sh = o3.spherical_harmonics(l=self.irreps_node_equivariant_inputs, x=data.force, normalize=True,
+        if force is not None and self.use_force_encoding:
+            if noise_mask is None:
+                raise ValueError("the force encoding needs noise_mask (the atoms whose forces are encoded)")
+            force_sh = o3.spherical_harmonics(l=self.irreps_node_equivariant_inputs, x=force, normalize=True,
                                               normalization="component")
-            force_sh = force_sh * data.noise_mask.to(force_sh.dtype).unsqueeze(-1)
-            force_sh = force_sh * (data.force.norm(dim=1, keepdim=True) / math.sqrt(3.0))
+            force_sh = force_sh * noise_mask.to(force_sh.dtype).unsqueeze(-1)
+            force_sh = force_sh * (force.norm(dim=1, keepdim=True) / math.sqrt(3.0))
         else:
             force_sh = torch.zeros((node_features.shape[0], self.irreps_node_equivariant_inputs.dim),
                                    device=node_features.device, dtype=node_features.dtype)
         node_features = node_features + self.force_embed(force_sh)
 
         node_features = _run_blocks(self.blocks, node_features, self.irreps_node_embedding, node_attr, edge_src, edge_dst,
-                                    edge_sh, edge_length_embedding, batch, graph, getattr(data, "n_graphs", None))
+                                    edge_sh, edge_length_embedding, batch, graph, n_graphs)
         node_features = self.norm(node_features, batch=batch)
         if self.out_dropout is not None:
             node_features = self.out_dropout(node_features)
 
         energy = self.energy_head(node_features)
-        if hasattr(data, "denoising_mask") and not self.use_force_encoding:
-            energy = energy * (~data.denoising_mask).to(energy.dtype).view(-1, 1)
-        energy = self.scale_scatter(energy, batch, dim=0)
+        if denoising_mask is not None and not self.use_force_encoding:
+            energy = energy * (~denoising_mask).to(energy.dtype).view(-1, 1)
+        energy = self.scale_scatter(energy, batch, dim=0, dim_size=n_graphs)
         if self.scale is not None:
             energy = self.scale * energy
         forces = -1 * torch.autograd.grad(energy, pos, grad_outputs=torch.ones_like(energy), create_graph=True)[0]
 
-        if hasattr(data, "noise_mask"):
+        if noise_mask is not None:
             noise = self.denoising_pos_head(node_input=node_features, node_attr=node_attr, edge_src=edge_src,
                                             edge_dst=edge_dst, edge_attr=edge_sh, edge_scalars=edge_length_embedding,
-                                            batch=batch, graph=graph)
-            mask = data.noise_mask.view(-1, 1)
+                                            batch=batch, graph=graph, n_graphs=n_graphs)
+            mask = noise_mask.view(-1, 1)
             outputs_dy = torch.where(mask, noise, forces)          # forces of clean atoms, predicted noise of corrupted ones
             if not self.use_force_encoding:
-                outputs_dy = outputs_dy * (~data.denoising_pos_mask).to(outputs_dy.dtype).view(-1, 1)
+                if denoising_pos_mask is None:
+                    raise ValueError("use_force_encoding=False with a noise_mask needs denoising_pos_mask")
+                outputs_dy = outputs_dy * (~denoising_pos_mask).to(outputs_dy.dtype).view(-1, 1)
             return energy, outputs_dy
         return energy, forces
 
@@ -176,3 +212,24 @@ class Equiformer_MD17_DeNS(torch.nn.Module):
 @register_model
 def equiformer_md17_dens(**kwargs):
     return Equiformer_MD17_DeNS(**kwargs)
+
+
+# the model block of md17/configs/equiformer_dens/equiformer_dens_N@6_L@2_C@128-64-32.yml (scripts/train/md17/
+# equiformer_dens/se_l2/: batch 8, lr 5e-4)
+MD17_DENS_L2 = dict(
+    irreps_in="64x0e", irreps_equivariant_inputs="1x0e+1x1e+1x2e", irreps_node_embedding="128x0e+64x1e+32x2e",
+    num_layers=6, irreps_node_attr="1x0e", irreps_sh="1x0e+1x1e+1x2e", max_radius=5.0, number_of_basis=32,
+    basis_type="exp", fc_neurons=[64, 64], irreps_feature="512x0e+256x1e+128x2e", irreps_head="32x0e+16x1e+8x2e",
+    num_heads=4, irreps_pre_attn="128x0e+64x1e+32x2e", rescale_degree=False, nonlinear_message=True,
+    irreps_mlp_mid="384x0e+192x1e+96x2e", norm_layer="layer", alpha_drop=0.0, proj_drop=0.0, out_drop=0.0,
+    drop_path_rate=0.0, use_force_encoding=True)
+
+# the model block of md17/configs/equiformer_dens/equiformer_dens_N@6_L@3_C@128-64-64-32.yml (se_l3/: batch 5, lr 2e-4);
+# the file leaves use_force_encoding at its default, True
+MD17_DENS_L3 = dict(
+    irreps_in="64x0e", irreps_equivariant_inputs="1x0e+1x1e+1x2e+1x3e", irreps_node_embedding="128x0e+64x1e+64x2e+32x3e",
+    num_layers=6, irreps_node_attr="1x0e", irreps_sh="1x0e+1x1e+1x2e+1x3e", max_radius=5.0, number_of_basis=32,
+    basis_type="exp", fc_neurons=[64, 64], irreps_feature="512x0e+256x1e+256x2e+128x3e",
+    irreps_head="32x0e+16x1e+16x2e+8x3e", num_heads=4, irreps_pre_attn="128x0e+64x1e+64x2e+32x3e", rescale_degree=False,
+    nonlinear_message=True, irreps_mlp_mid="384x0e+192x1e+192x2e+96x3e", norm_layer="layer", alpha_drop=0.0,
+    proj_drop=0.0, out_drop=0.0, drop_path_rate=0.0, use_force_encoding=True)
