@@ -14,10 +14,11 @@ import torch
 from equiformer_b200 import ops
 
 
-def _cg(plan, p, dtype):
+def _cg(plan, p, like):
+    """Coupling block of path ``p`` in the dtype and on the device of ``like`` (the references also run on a GPU in fp64)."""
     d1, d2, d3 = 2 * p.l1 + 1, 2 * p.l2 + 1, 2 * p.l3 + 1
     c = torch.from_numpy(plan.cg64[p.cg_off:p.cg_off + d1 * d2 * d3].copy()).reshape(d1, d2, d3)
-    return c.to(dtype)
+    return c.to(device=like.device, dtype=like.dtype)
 
 
 def _w(plan, p, w):
@@ -42,7 +43,7 @@ def dtp_forward_raw(plan, xs, y, w, gather=None, w_offset=None):
     E = y.shape[0]
     outs = [y.new_zeros((E, 2 * l + 1, mul)) for l, _p, mul in plan.out_groups]
     for p in plan.paths:
-        M = torch.einsum("ijk,ej->eik", _cg(plan, p, y.dtype), y[:, p.in2_off:p.in2_off + 2 * p.l2 + 1])
+        M = torch.einsum("ijk,ej->eik", _cg(plan, p, y), y[:, p.in2_off:p.in2_off + 2 * p.l2 + 1])
         val = torch.einsum("eiu,eik->eku", xs[p.in1_block], M) * _w(plan, p, w)[:, None, :]
         outs[p.out_group][:, :, p.out_chan_off:p.out_chan_off + p.mul] = val
     return outs
@@ -61,7 +62,7 @@ def dtp_grad_x_raw(plan, gs, y, w):
     E = y.shape[0]
     gxs = [y.new_zeros((E, 2 * l + 1, mul)) for l, mul in plan.in1_blocks]
     for p in plan.paths:
-        M = torch.einsum("ijk,ej->eik", _cg(plan, p, y.dtype), y[:, p.in2_off:p.in2_off + 2 * p.l2 + 1])
+        M = torch.einsum("ijk,ej->eik", _cg(plan, p, y), y[:, p.in2_off:p.in2_off + 2 * p.l2 + 1])
         g = gs[p.out_group][:, :, p.out_chan_off:p.out_chan_off + p.mul]
         gxs[p.in1_block] = gxs[p.in1_block] + torch.einsum("eku,eik->eiu", g, M) * _w(plan, p, w)[:, None, :]
     return gxs
@@ -71,7 +72,7 @@ def dtp_grad_w_raw(plan, xs, y, gs, shared):
     E = y.shape[0]
     gw = y.new_zeros((E, plan.weight_numel))
     for p in plan.paths:
-        M = torch.einsum("ijk,ej->eik", _cg(plan, p, y.dtype), y[:, p.in2_off:p.in2_off + 2 * p.l2 + 1])
+        M = torch.einsum("ijk,ej->eik", _cg(plan, p, y), y[:, p.in2_off:p.in2_off + 2 * p.l2 + 1])
         g = gs[p.out_group][:, :, p.out_chan_off:p.out_chan_off + p.mul]
         gw[:, p.w_off:p.w_off + p.mul] = torch.einsum("eiu,eik,eku->eu", xs[p.in1_block], M, g)
     return gw.sum(0) if shared else gw
@@ -85,7 +86,7 @@ def dtp_grad_y_raw(plan, xs, w, gs, y_like):
         N = torch.einsum("eiu,eku,eu->eik", xs[p.in1_block], g, _w(plan, p, w).expand(E, -1))
         d2 = 2 * p.l2 + 1
         gy[:, p.in2_off:p.in2_off + d2] = gy[:, p.in2_off:p.in2_off + d2] + torch.einsum(
-            "ijk,eik->ej", _cg(plan, p, y_like.dtype), N)
+            "ijk,eik->ej", _cg(plan, p, y_like), N)
     return gy
 
 

@@ -326,8 +326,7 @@ def test_dtp_weight_offset_fused(cuda_device, cfg):
     forward and grad_xw vs the fp64 statement on w + offset; the autograd wrapper returns colsum(gw) for the offset."""
     from equiformer_b200 import ops
     plan = _dtp(cfg).tp.plan
-    if not plan.generated:
-        pytest.skip("no plan-specialised kernels for this configuration")
+    assert plan.generated, f"the shipped {cfg} plan no longer matches its plan-specialised kernels"
     n_nodes, E = 41, 523
     graph, src, dst = _graph(n_nodes, E, 5, cuda_device)
     g = torch.Generator().manual_seed(9)
@@ -475,10 +474,14 @@ def test_equivariant_layer_norm_planar(cuda_device, entries, N):
         assert rel_err(a, r) < 5e-5
 
 
-@pytest.mark.parametrize("cfg", [dict(A0=128, S=128, H=4, ds=(3, 5), Cs=(64, 32)), dict(A0=256, S=256, H=8, ds=(3,), Cs=(128,)),
-                                 dict(A0=128, S=128, H=4, ds=(3, 5, 7), Cs=(64, 64, 32)),
-                                 dict(A0=16, S=16, H=4, ds=(3, 5), Cs=(8, 4)),       # tiny heads: one lane per head
-                                 dict(A0=64, S=20, H=4, ds=(3,), Cs=(6,))])          # falls back to the scalar kernels
+GATE_LOGITS_CFGS = [dict(A0=128, S=128, H=4, ds=(3, 5), Cs=(64, 32)), dict(A0=256, S=256, H=8, ds=(3,), Cs=(128,)),
+                    dict(A0=128, S=128, H=4, ds=(3, 5, 7), Cs=(64, 64, 32)),
+                    dict(A0=16, S=16, H=4, ds=(3, 5), Cs=(8, 4)),       # tiny heads: one lane per head
+                    dict(A0=64, S=20, H=4, ds=(3,), Cs=(6,))]          # falls back to the scalar kernels
+GATE_ONLY_CFGS = [dict(S=384, ds=(3, 5), Cs=(192, 96)), dict(S=20, ds=(3,), Cs=(6,))]   # vec / scalar kernels
+
+
+@pytest.mark.parametrize("cfg", GATE_LOGITS_CFGS)
 def test_gate_logits_fused(cuda_device, cfg):
     """bias + Gate + attention logits in one kernel (ref :492-495, :506-507) vs the fp64 torch statement, fwd and bwd."""
     from equiformer_b200 import ops
@@ -506,7 +509,7 @@ def test_gate_logits_fused(cuda_device, cfg):
         assert rel_err(a, b) < 5e-5
 
 
-@pytest.mark.parametrize("cfg", [dict(S=384, ds=(3, 5), Cs=(192, 96)), dict(S=20, ds=(3,), Cs=(6,))])   # vec / scalar kernels
+@pytest.mark.parametrize("cfg", GATE_ONLY_CFGS)
 def test_gate_only_fused(cuda_device, cfg):
     """Gate-only use of the fused kernel (FFN: bias + SiLU on scalars + sigmoid gates on the rest, ref :128-154)."""
     from equiformer_b200 import ops

@@ -36,6 +36,35 @@ def test_plan_tables_reproduce_oracle_tensor_product(irreps, sh):
     assert plan.weight_numel == dtp.tp.weight_numel
 
 
+def _generated_signatures():
+    """tag -> the signature literal a committed ``csrc/gen/dtp_gen_<tag>.cu`` registers its kernels under."""
+    from equiformer_b200 import codegen
+    out = {}
+    for tag, _irreps, _sh in codegen.KNOWN_CONFIGS:
+        text = (codegen.GEN_DIR / f"dtp_gen_{tag}.cu").read_text()
+        found = re.findall(r'GeneratedKernels kernels = \{0x([0-9a-f]{16})ULL, "([a-z0-9_]+)"', text)
+        assert [t for _s, t in found] == [tag], (tag, found)
+        out[tag] = int(found[0][0], 16)
+    return out
+
+
+def test_generated_kernel_signatures_match_the_shipped_plans():
+    """The plan-specialised kernels run only when a plan's hash equals the literal in its generated file: every committed
+    file matches its configuration, and the depth-wise products of the QM9 and MD17-L3 models (radial degree embedding,
+    attention value) land on one of them - a drift would move the shipped models onto the generic kernels silently."""
+    from equiformer_b200 import codegen
+    from equiformer_b200.nets import model_entrypoint
+    sigs = _generated_signatures()
+    for tag, irreps, sh in codegen.KNOWN_CONFIGS:
+        assert sigs[tag] == codegen.plan_signature(codegen.plan_for(irreps, sh)), tag
+    for name, irreps_in, tag in (("graph_attention_transformer_nonlinear_l2", "5x0e", "qm9_l2"),
+                                 ("graph_attention_transformer_nonlinear_exp_l3_md17", "64x0e", "md17_l3")):
+        model = model_entrypoint(name)(irreps_in=irreps_in, radius=5.0, num_basis=128)
+        plans = [model.edge_deg_embed.dw.tp.plan] + [blk.ga.sep_value.dtp.tp.plan for blk in model.blocks]
+        for plan in plans:
+            assert codegen.plan_signature(plan) == sigs[tag], (name, tag)
+
+
 def test_plan_info_and_bytes(built_lib):
     from equiformer_b200.nets.graph_attention_transformer import DepthwiseTensorProduct
     irreps = "128x0e+64x1e+32x2e"
