@@ -150,6 +150,8 @@ SIGNATURES = {
     "eqf_edge_geom_bwd": (c_int32, [c_void_p, c_void_p, c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_void_p, c_void_p]),
     "eqf_expnorm_fwd": (c_int32, [c_void_p, c_void_p, c_void_p, c_float, c_float, c_int64, c_int32, c_void_p, c_void_p]),
     "eqf_expnorm_bwd": (c_int32, [c_void_p, c_void_p, c_void_p, c_float, c_float, c_int64, c_int32, c_void_p, c_void_p, c_void_p]),
+    "eqf_bessel_fwd": (c_int32, [c_void_p, c_void_p, c_float, c_int64, c_int32, c_void_p, c_void_p]),
+    "eqf_bessel_bwd": (c_int32, [c_void_p, c_void_p, c_float, c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_void_p]),
     "eqf_rbf_fwd": (c_int32, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_int64, c_void_p, c_void_p]),
     "eqf_rbf_bwd": (c_int32, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_int64, c_void_p, c_void_p,
                               c_void_p]),

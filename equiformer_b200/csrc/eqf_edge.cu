@@ -7,7 +7,10 @@
 //                                                      normalize=True, normalization='component'); edge_vec.norm(dim=1)
 //   nets/graph_attention_transformer_oc20.py:283-296   the same with the periodic image offsets added
 //   nets/expnorm_rbf.py:11-33, 73-78                   CosineCutoff * exp(-beta (exp(-alpha d) - mean)^2)
-// One thread per edge for the geometry (a few hundred flops, ~100 bytes), one warp per edge row for the basis.  The
+//   nets/graph_attention_transformer.py:786-787,       RadialBasis(num_basis, cutoff, rbf={'name': 'spherical_bessel'})
+//   ..._md17.py:179-180, equiformer_md17_dens.py:123   of ocpmodels 0.0.3 (gemnet/layers/radial_basis.py): polynomial
+//                                                      envelope (p = 5) * sqrt(2 / c^3) sin(f_k d / c) / (d / c)
+// One thread per edge for the geometry (a few hundred flops, ~100 bytes), one warp per edge row for the bases.  The
 // harmonics follow e3nn's coupling recurrence  Y_{l+1,k} = sum_ji A_l[k,j,i] x_j Y_{l,i}  ('norm' normalisation, y polar,
 // Y_1 = (x, y, z)); the host passes the coupling tensors A_1, A_2 (equiformer_b200/o3/sh.py computes them from the real
 // Wigner 3j), so kernel and torch statement share one table.  Second derivatives (MD17 force training) go through the
@@ -189,6 +192,88 @@ __global__ void __launch_bounds__(256) expnorm_bwd_kernel(const float* __restric
   if (lane == 0) g_dist[e] = acc;
 }
 
+// spherical Bessel radial basis (B <= 128 functions, lane owns k = lane + 32 j): with x = d / c,
+//   env(x) = 1 - 21 x^5 + 35 x^6 - 15 x^7 for x < 1, else 0;   out[e, k] = env(x) sqrt(2 / c^3) sin(f_k x) / x.
+// d = 0 gives 0 / 0 = NaN, as in the reference; neighbour lists never contain a zero-length edge.  The argument f_k x reaches
+// 128 pi for the MD17 configurations: the accurate sincosf, never the __sinf intrinsic.
+constexpr int kBesselMaxB = 128;
+constexpr int kBesselPerLane = kBesselMaxB / 32;
+
+__device__ __forceinline__ void bessel_envelope(float x, float& env, float& denv) {
+  const bool in = x < 1.f;
+  const float x2 = x * x, x4 = x2 * x2;
+  env = in ? 1.f + x4 * x * fmaf(x, fmaf(x, -15.f, 35.f), -21.f) : 0.f;
+  denv = in ? x4 * fmaf(x, fmaf(x, -105.f, 210.f), -105.f) : 0.f;      // 5a x^4 + 6b x^5 + 7c x^6
+}
+
+__global__ void __launch_bounds__(256) bessel_fwd_kernel(const float* __restrict__ dist, const float* __restrict__ freq,
+                                                         float inv_cut, float norm, long long E, int B,
+                                                         float* __restrict__ out) {
+  const int lane = threadIdx.x & 31;
+  const long long warp = (long long)blockIdx.x * 8 + (threadIdx.x >> 5), n_warps = (long long)gridDim.x * 8;
+  float f[kBesselPerLane];
+#pragma unroll
+  for (int j = 0; j < kBesselPerLane; ++j) f[j] = lane + 32 * j < B ? __ldg(freq + lane + 32 * j) : 0.f;
+  for (long long e = warp; e < E; e += n_warps) {
+    const float x = __ldg(dist + e) * inv_cut;
+    float env, denv;
+    bessel_envelope(x, env, denv);
+    const float scale = env * norm / x;
+#pragma unroll
+    for (int j = 0; j < kBesselPerLane; ++j) {
+      const int k = lane + 32 * j;
+      if (k < B) out[e * B + k] = scale * sinf(f[j] * x);
+    }
+  }
+}
+
+// g_dist[e] = sum_k g[e, k] d out[e, k] / d d_e (skipped when g_dist is NULL) and per-CTA partial rows
+// part[grid][B] of d <g, out> / d f_k = sum_e g[e, k] env norm cos(f_k x_e)
+__global__ void __launch_bounds__(256) bessel_bwd_kernel(const float* __restrict__ dist, const float* __restrict__ freq,
+                                                         float inv_cut, float norm, const float* __restrict__ g, long long E,
+                                                         int B, float* __restrict__ g_dist, float* __restrict__ part) {
+  __shared__ float sacc[kBesselMaxB];
+  for (int i = threadIdx.x; i < B; i += blockDim.x) sacc[i] = 0.f;
+  __syncthreads();
+  const int lane = threadIdx.x & 31;
+  const long long warp = (long long)blockIdx.x * 8 + (threadIdx.x >> 5), n_warps = (long long)gridDim.x * 8;
+  float f[kBesselPerLane], af[kBesselPerLane];
+#pragma unroll
+  for (int j = 0; j < kBesselPerLane; ++j) {
+    f[j] = lane + 32 * j < B ? __ldg(freq + lane + 32 * j) : 0.f;
+    af[j] = 0.f;
+  }
+  for (long long e = warp; e < E; e += n_warps) {
+    const float x = __ldg(dist + e) * inv_cut;
+    float env, denv;
+    bessel_envelope(x, env, denv);
+    const float inv_x = 1.f / x;
+    float gx = 0.f;
+#pragma unroll
+    for (int j = 0; j < kBesselPerLane; ++j) {
+      const int k = lane + 32 * j;
+      if (k < B) {
+        const float gk = __ldg(g + e * B + k);
+        float s, c;
+        sincosf(f[j] * x, &s, &c);
+        af[j] = fmaf(gk, env * c, af[j]);
+        // d/dx [env sin(f x) / x] = denv sin / x + env (f cos - sin / x) / x
+        gx = fmaf(gk, fmaf(denv, s, env * fmaf(f[j], c, -s * inv_x)) * inv_x, gx);
+      }
+    }
+    if (g_dist != nullptr) {
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) gx += __shfl_xor_sync(0xffffffffu, gx, o);
+      if (lane == 0) g_dist[e] = gx * norm * inv_cut;
+    }
+  }
+#pragma unroll
+  for (int j = 0; j < kBesselPerLane; ++j)
+    if (lane + 32 * j < B) atomicAdd(&sacc[lane + 32 * j], af[j] * norm);
+  __syncthreads();
+  for (int i = threadIdx.x; i < B; i += blockDim.x) part[(long long)blockIdx.x * B + i] = sacc[i];
+}
+
 }  // namespace eqf
 
 using namespace eqf;
@@ -242,4 +327,32 @@ extern "C" int eqf_expnorm_bwd(const float* dist, const float* means, const floa
   if (!dist || !means || !betas || !g || !g_dist) { set_error("eqf_expnorm_bwd: null pointer"); return EQF_ERR_INVALID; }
   expnorm_bwd_kernel<<<(unsigned)((E + 7) / 8), 256, 0, (cudaStream_t)stream>>>(dist, means, betas, alpha, cutoff_upper, E, B, g, g_dist);
   return check_cuda(cudaGetLastError(), "expnorm_bwd_kernel launch");
+}
+
+static int check_bessel(int32_t B, float cutoff, const char* who) {
+  // B % 4 == 0 keeps the [E, B] output a legal TMA operand of the first-layer GEMM
+  if (B < 1 || B > kBesselMaxB || B % 4 != 0) { set_error(std::string(who) + ": B must be a multiple of 4 in 4..128"); return EQF_ERR_UNSUPPORTED; }
+  if (!(cutoff > 0.f)) { set_error(std::string(who) + ": cutoff must be positive"); return EQF_ERR_INVALID; }
+  return EQF_OK;
+}
+
+extern "C" int eqf_bessel_fwd(const float* dist, const float* freq, float cutoff, int64_t E, int32_t B, float* out,
+                              void* stream) {
+  int rc = check_bessel(B, cutoff, "eqf_bessel_fwd");
+  if (rc != EQF_OK || E <= 0) return rc;
+  if (!dist || !freq || !out) { set_error("eqf_bessel_fwd: null pointer"); return EQF_ERR_INVALID; }
+  bessel_fwd_kernel<<<eqf_pointwise_rows(E), 256, 0, (cudaStream_t)stream>>>(dist, freq, 1.f / cutoff,
+                                                                            sqrtf(2.f / (cutoff * cutoff * cutoff)), E, B, out);
+  return check_cuda(cudaGetLastError(), "bessel_fwd_kernel launch");
+}
+
+extern "C" int eqf_bessel_bwd(const float* dist, const float* freq, float cutoff, const float* g, int64_t E, int32_t B,
+                              float* g_dist, float* part, void* stream) {
+  int rc = check_bessel(B, cutoff, "eqf_bessel_bwd");
+  if (rc != EQF_OK || E <= 0) return rc;
+  if (!dist || !freq || !g || !part) { set_error("eqf_bessel_bwd: null pointer"); return EQF_ERR_INVALID; }
+  bessel_bwd_kernel<<<eqf_pointwise_rows(E), 256, 0, (cudaStream_t)stream>>>(dist, freq, 1.f / cutoff,
+                                                                            sqrtf(2.f / (cutoff * cutoff * cutoff)), g, E, B,
+                                                                            g_dist, part);
+  return check_cuda(cudaGetLastError(), "bessel_bwd_kernel launch");
 }

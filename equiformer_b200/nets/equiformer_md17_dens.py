@@ -16,12 +16,12 @@ import torch
 from .. import o3, ops
 from ..graph import radius_graph
 from ..o3 import Irreps
+from .bessel_rbf import RadialBasis
 from .drop import EquivariantDropout
-from .expnorm_rbf import ExpNormalSmearing
 from .fast_activation import Activation
 from .gaussian_rbf import GaussianRadialBasisLayer
 from .graph_attention_transformer import (_run_blocks, edge_features, EdgeDegreeEmbeddingNetwork, GraphAttention,
-                                          NodeEmbeddingNetwork, ScaledScatter, TransBlock, get_norm_layer)
+                                          NodeEmbeddingNetwork, ScaledScatter, TransBlock, get_norm_layer, radial_basis)
 from .layer_norm import EquivariantLayerNormV2
 from .registry import register_model
 from .tensor_product_rescale import LinearRS
@@ -64,15 +64,7 @@ class Equiformer_MD17_DeNS(torch.nn.Module):
 
         self.atom_embed = NodeEmbeddingNetwork(self.irreps_node_embedding, _MAX_ATOM_TYPE)
         self.basis_type = basis_type
-        if basis_type == "gaussian":
-            self.rbf = GaussianRadialBasisLayer(self.number_of_basis, cutoff=self.max_radius)
-        elif basis_type == "exp":
-            self.rbf = ExpNormalSmearing(cutoff_lower=0.0, cutoff_upper=self.max_radius, num_rbf=self.number_of_basis,
-                                         trainable=False)
-        elif basis_type == "bessel":
-            raise NotImplementedError("Bessel basis comes from ocpmodels (absent dependency; out of scope)")
-        else:
-            raise ValueError(basis_type)
+        self.rbf = radial_basis(basis_type, self.number_of_basis, self.max_radius, ("gaussian", "bessel", "exp"))
         self.edge_deg_embed = EdgeDegreeEmbeddingNetwork(self.irreps_node_embedding, self.irreps_edge_attr,
                                                          self.fc_neurons, _AVG_DEGREE)
         self.force_embed = LinearRS(self.irreps_node_equivariant_inputs, self.irreps_node_embedding, rescale=_RESCALE)
@@ -114,7 +106,8 @@ class Equiformer_MD17_DeNS(torch.nn.Module):
     def no_weight_decay(self):
         skip = set()
         for mod_name, mod in self.named_modules():
-            if isinstance(mod, (torch.nn.Linear, torch.nn.LayerNorm, EquivariantLayerNormV2, GaussianRadialBasisLayer)):
+            if isinstance(mod, (torch.nn.Linear, torch.nn.LayerNorm, EquivariantLayerNormV2, GaussianRadialBasisLayer,
+                                RadialBasis)):
                 for p_name, _ in mod.named_parameters():
                     if isinstance(mod, torch.nn.Linear) and "weight" in p_name:
                         continue

@@ -24,7 +24,9 @@ import torch
 from .. import o3, ops
 from ..graph import radius_graph, scatter_sum
 from ..o3 import Irreps
+from .bessel_rbf import RadialBasis
 from .drop import EquivariantDropout, GraphDropPath
+from .expnorm_rbf import ExpNormalSmearing
 from .fast_activation import Activation, Gate
 from .gaussian_rbf import GaussianRadialBasisLayer
 from .layer_norm import EquivariantLayerNormV2
@@ -703,12 +705,7 @@ class GraphAttentionTransformer(torch.nn.Module):
 
         self.atom_embed = NodeEmbeddingNetwork(self.irreps_node_embedding, _MAX_ATOM_TYPE)
         self.basis_type = basis_type
-        if basis_type == "gaussian":
-            self.rbf = GaussianRadialBasisLayer(self.number_of_basis, cutoff=self.max_radius)
-        elif basis_type == "bessel":
-            raise NotImplementedError("Bessel basis comes from ocpmodels (absent dependency; out of scope, SURVEY.md 2#5)")
-        else:
-            raise ValueError(basis_type)
+        self.rbf = radial_basis(basis_type, self.number_of_basis, self.max_radius, ("gaussian", "bessel"))
         self.edge_deg_embed = EdgeDegreeEmbeddingNetwork(self.irreps_node_embedding, self.irreps_edge_attr,
                                                          self.fc_neurons, _AVG_DEGREE)
         self.blocks = torch.nn.ModuleList()
@@ -749,7 +746,8 @@ class GraphAttentionTransformer(torch.nn.Module):
         skip = set()
         names = {n for n, _ in self.named_parameters()}
         for mod_name, mod in self.named_modules():
-            if isinstance(mod, (torch.nn.Linear, torch.nn.LayerNorm, EquivariantLayerNormV2, GaussianRadialBasisLayer)):
+            if isinstance(mod, (torch.nn.Linear, torch.nn.LayerNorm, EquivariantLayerNormV2, GaussianRadialBasisLayer,
+                                RadialBasis)):
                 for p_name, _ in mod.named_parameters():
                     if isinstance(mod, torch.nn.Linear) and "weight" in p_name:
                         continue
@@ -801,6 +799,20 @@ class GraphAttentionTransformer(torch.nn.Module):
         if self.scale is not None:
             outputs = self.scale * outputs
         return outputs
+
+
+def radial_basis(basis_type: str, number_of_basis: int, max_radius: float, supported):
+    """The edge-length embedding ``basis_type`` names (ref :782-789, ..._md17.py:175-185, equiformer_md17_dens.py:119-129);
+    ``supported`` lists the types the calling model accepts (the QM9 model has no exp-normal basis)."""
+    if basis_type not in supported:
+        raise ValueError(basis_type)
+    if basis_type == "gaussian":
+        return GaussianRadialBasisLayer(number_of_basis, cutoff=max_radius)
+    if basis_type == "bessel":
+        return RadialBasis(number_of_basis, cutoff=max_radius, rbf={"name": "spherical_bessel"})
+    if basis_type == "exp":
+        return ExpNormalSmearing(cutoff_lower=0.0, cutoff_upper=max_radius, num_rbf=number_of_basis, trainable=False)
+    raise ValueError(basis_type)
 
 
 def edge_features(irreps_edge_attr, pos, graph, edge_vec=None):

@@ -1983,6 +1983,68 @@ def expnorm_rbf(dist, means, betas, alpha: float, cutoff_upper: float):
     return expnorm_torch(dist, means, betas, alpha, cutoff_upper)
 
 
+def bessel_rbf_torch(dist, freq, cutoff: float):
+    """Torch statement of ocpmodels 0.0.3 ``RadialBasis(B, cutoff, rbf={'name': 'spherical_bessel'})`` with its default
+    polynomial envelope (p = 5), as the reference builds it (nets/graph_attention_transformer.py:785-787).  ``d = 0`` gives
+    ``0 / 0 = NaN``, as in the reference."""
+    x = (dist / cutoff).unsqueeze(-1)
+    env = (1.0 - 21.0 * x ** 5 + 35.0 * x ** 6 - 15.0 * x ** 7) * (x < 1.0).to(x.dtype)
+    return env * ((2.0 / cutoff ** 3) ** 0.5 * torch.sin(freq * x) / x)
+
+
+def bessel_fwd_raw(dist, freq, cutoff: float):
+    dist = _require_cuda(dist, "bessel dist")
+    E, B = dist.shape[0], freq.numel()
+    out = torch.empty((E, B), device=dist.device, dtype=torch.float32)
+    with torch.cuda.device(dist.device), _kernel("bessel_fwd", 4 * (E + E * B)):
+        rc = _lib.load().eqf_bessel_fwd(dist.data_ptr(), freq.data_ptr(), float(cutoff), E, B, out.data_ptr(), _stream())
+    _lib.check(rc, "eqf_bessel_fwd")
+    return out
+
+
+def bessel_bwd_raw(dist, freq, cutoff: float, g, need_dist: bool):
+    """(g_dist or None, g_freq): one kernel + one column sum of its per-CTA partial rows."""
+    g = _require_cuda(g, "bessel g").contiguous()
+    E, B = g.shape
+    lib = _lib.load()
+    g_dist = torch.empty(E, device=g.device, dtype=torch.float32) if need_dist else None
+    part = torch.empty((lib.eqf_pointwise_rows(E), B), device=g.device, dtype=torch.float32)
+    with torch.cuda.device(g.device), _kernel("bessel_bwd", 4 * (E * B + 2 * E)):
+        rc = lib.eqf_bessel_bwd(dist.data_ptr(), freq.data_ptr(), float(cutoff), g.data_ptr(), E, B,
+                                g_dist.data_ptr() if need_dist else None, part.data_ptr(), _stream())
+    _lib.check(rc, "eqf_bessel_bwd")
+    return g_dist, colsum_raw(part)
+
+
+class BesselRbf(torch.autograd.Function):
+    """Spherical Bessel radial basis on ``[E]`` distances -> ``[E, B]`` with trainable frequencies ``[B]``: forward one
+    kernel, backward one kernel + one column sum; second order through the torch statement."""
+
+    @staticmethod
+    def forward(ctx, dist, freq, cutoff: float):
+        ctx.cutoff = cutoff
+        ctx.save_for_backward(dist, freq)
+        return bessel_fwd_raw(dist, freq, cutoff)
+
+    @staticmethod
+    def backward(ctx, g):
+        dist, freq = ctx.saved_tensors
+        if torch.is_grad_enabled():
+            fn = lambda d, f: bessel_rbf_torch(d, f, ctx.cutoff)
+            gd, gf = _higher_order_grads(fn, (dist, freq), (g,))
+            return gd, gf, None
+        gd, gf = bessel_bwd_raw(dist, freq, ctx.cutoff, g, ctx.needs_input_grad[0])
+        return gd, gf.view_as(freq), None
+
+
+def bessel_rbf(dist, freq, cutoff: float):
+    """``[E, B]`` spherical Bessel basis: the fused kernels for CUDA float32 (``B`` a multiple of 4 up to 128, anything
+    else raises); the torch statement on the CPU and in float64."""
+    if fused_ok(dist) and dist.dim() == 1 and dist.shape[0] > 0:
+        return BesselRbf.apply(dist.contiguous(), freq.contiguous(), float(cutoff))
+    return bessel_rbf_torch(dist, freq, cutoff)
+
+
 class GateLayout:
     """Static description of the fused gate + logits op (see ``eqf_gate_logits_fwd`` in include/eqf_b200.h)."""
 

@@ -209,6 +209,16 @@ int eqf_expnorm_fwd(const float* dist, const float* means, const float* betas, f
                     int32_t B, float* out, void* stream);
 int eqf_expnorm_bwd(const float* dist, const float* means, const float* betas, float alpha, float cutoff_upper, int64_t E,
                     int32_t B, const float* g, float* g_dist, void* stream);
+/* Spherical Bessel radial basis of the Bessel configurations: ocpmodels 0.0.3 RadialBasis(B, cutoff,
+ * rbf={'name': 'spherical_bessel'}) with its default polynomial envelope (p = 5), built at
+ * nets/graph_attention_transformer.py:785-787, nets/graph_attention_transformer_md17.py:178-180 and
+ * nets/equiformer_md17_dens.py:122-124.  With x = d_e / cutoff:
+ * out[e][k] = env(x) sqrt(2 / cutoff^3) sin(freq[k] x) / x,  env(x) = 1 - 21 x^5 + 35 x^6 - 15 x^7 (x < 1, else 0).
+ * B is a multiple of 4 in 4..128.  _bwd writes g_dist[E] = d <g, out> / d d_e (skipped when g_dist is NULL) and
+ * per-CTA partial sums part[eqf_pointwise_rows(E)][B] of d <g, out> / d freq[k] (reduce with eqf_colsum). */
+int eqf_bessel_fwd(const float* dist, const float* freq, float cutoff, int64_t E, int32_t B, float* out, void* stream);
+int eqf_bessel_bwd(const float* dist, const float* freq, float cutoff, const float* g, int64_t E, int32_t B, float* g_dist,
+                   float* part, void* stream);
 
 /* Neighbour list of the batched molecules: edge (j -> i) iff same graph, j != i (unless loop), |pos_j - pos_i| < r, at
  * most max_neighbors per centre (the first ones in index order); sorted by centre, neighbours ascending - what
