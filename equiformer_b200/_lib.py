@@ -118,6 +118,11 @@ SIGNATURES = {
                                      POINTER(c_void_p), c_void_p]),
     "eqf_attn_softmax_aggregate": (c_int32, [POINTER(EqfHeadLayout), c_void_p, c_void_p, POINTER(c_void_p), c_void_p,
                                              c_int64, POINTER(c_void_p), c_void_p, c_void_p]),
+    "eqf_attn_dot_softmax_aggregate": (c_int32, [POINTER(EqfHeadLayout), POINTER(c_void_p), POINTER(c_void_p), c_void_p,
+                                                 c_void_p, c_int64, POINTER(c_void_p), c_void_p, c_void_p]),
+    "eqf_attn_dot_softmax_aggregate_bwd": (c_int32, [POINTER(EqfHeadLayout), POINTER(c_void_p), POINTER(c_void_p),
+                                                     POINTER(c_void_p), c_void_p, c_void_p, c_void_p, c_int64,
+                                                     POINTER(c_void_p), POINTER(c_void_p), c_void_p, c_void_p]),
     "eqf_attn_edge_dot": (c_int32, [POINTER(EqfHeadLayout), POINTER(c_void_p), POINTER(c_void_p), c_void_p, c_int64,
                                     c_void_p, c_void_p]),
     "eqf_attn_edge_scale": (c_int32, [POINTER(EqfHeadLayout), c_void_p, c_void_p, POINTER(c_void_p), c_void_p, c_int64,

@@ -13,6 +13,8 @@
 // the channel-innermost planar layout.
 #include <math_constants.h>
 
+#include <type_traits>
+
 #include "eqf_common.cuh"
 
 namespace eqf {
@@ -341,6 +343,237 @@ __global__ void __launch_bounds__(256) edge_scale_vec_kernel(HeadArgs a, const f
   }
 }
 
+// ------------------------------------------------------------------------------------------------ dot-product attention
+// The DP layer's q[dst] . k -> segment softmax -> (dropout) -> sum alpha v (ref nets/dp_attention_transformer.py:145-151)
+// in one launch, reading keys and values straight from the key / value blocks kv[g] = [E, d_g, 2 C_g] (keys in channels
+// [0, C_g), values in [C_g, 2 C_g)).  One warp per destination node, grid-stride over the nodes; a lane owns up to S float4
+// slots of the node row (all groups concatenated, slot = lane + 32 s), every slot inside one head.  Two passes over the
+// segment: the first reads the keys, forms z per head (a warp reduction per head), keeps an online max and sum of
+// exponentials and parks z in alpha[e, h]; the second turns z into alpha = exp(z - max) / (sum + 1e-16) over it and
+// accumulates alpha keep v from the values.  Lane h writes and re-reads its own alpha[e, h], so no cross-lane ordering is
+// needed; a segment of any length costs no shared memory.  The key / value row is read once in all, the q row once per
+// node; no atomics, and the order of every sum is fixed.
+struct DotArgs {
+  int n_groups, n_slots;
+  int C[EQF_MAX_BLOCKS];                 // channels of group g in q / out (kv rows hold 2 C)
+  int d[EQF_MAX_BLOCKS];
+  int slot_start[EQF_MAX_BLOCKS + 1];    // prefix sum of d C / 4
+  const float* q[EQF_MAX_BLOCKS];        // [N, d, C]
+  const float* kv[EQF_MAX_BLOCKS];       // [E, d, 2C]
+  const float* G[EQF_MAX_BLOCKS];        // [N, d, C]  (backward: d L / d out)
+  float* out[EQF_MAX_BLOCKS];            // [N, d, C]  forward: out; backward: gq
+  float* gkv[EQF_MAX_BLOCKS];            // [E, d, 2C] (backward)
+};
+
+constexpr int DOT_MAX_SLOTS = 8;         // float4 slots per lane: node rows of up to 1024 floats
+
+__device__ __forceinline__ float dot4(float4 x, float4 y) { return x.x * y.x + x.y * y.y + x.z * y.z + x.w * y.w; }
+__device__ __forceinline__ void fma4(float4& acc, float s, float4 v) {
+  acc.x = fmaf(s, v.x, acc.x); acc.y = fmaf(s, v.y, acc.y); acc.z = fmaf(s, v.z, acc.z); acc.w = fmaf(s, v.w, acc.w);
+}
+__device__ __forceinline__ void st4(float* p, float4 v) { *reinterpret_cast<float4*>(p) = v; }
+
+// slot c of a group-concatenated node row: its group, offset in the node row, offset in the kv row, head
+__device__ __forceinline__ void dot_slot(const DotArgs& a, int H, int c, int& g, int& node_off, int& kv_off, int& head) {
+  g = 0;
+  while (g + 1 < a.n_groups && c >= a.slot_start[g + 1]) ++g;
+  const int C = a.C[g], local = (c - a.slot_start[g]) * 4;
+  const int i = local / C, j = local - i * C;
+  node_off = local; kv_off = i * 2 * C + j; head = j / (C / H);
+}
+
+// the lane's slots, fixed for the whole kernel: head (-1: no slot), kv row stride, value offset C and the key columns of
+// kv / gkv at edge 0 (the value columns are C further)
+template <int H, int S>
+struct DotSlots {
+  int head[S], stride[S], C[S];
+  const float* k[S];
+  float* gk[S];
+  __device__ __forceinline__ DotSlots(const DotArgs& a, int lane) {
+#pragma unroll
+    for (int s = 0; s < S; ++s) {
+      const int c = lane + 32 * s;
+      int g, node_off, kv_off, h;
+      dot_slot(a, H, c < a.n_slots ? c : 0, g, node_off, kv_off, h);
+      head[s] = c < a.n_slots ? h : -1;
+      stride[s] = 2 * a.C[g] * a.d[g];
+      C[s] = a.C[g];
+      k[s] = a.kv[g] + kv_off;
+      gk[s] = a.gkv[g] == nullptr ? nullptr : a.gkv[g] + kv_off;
+    }
+  }
+};
+
+// element offset of slot c in node row t, and its group
+__device__ __forceinline__ long long node_index(const DotArgs& a, int H, int c, long long t, int& g) {
+  int node_off, kv_off, h;
+  dot_slot(a, H, c, g, node_off, kv_off, h);
+  return t * (long long)(a.d[g] * a.C[g]) + node_off;
+}
+
+template <int H, int S>
+__device__ __forceinline__ void load_node_row(const DotArgs& a, const float* const* base, const DotSlots<H, S>& sl, int lane,
+                                              long long t, float4 (&x)[S]) {
+#pragma unroll
+  for (int s = 0; s < S; ++s) {
+    x[s] = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (sl.head[s] >= 0) {
+      int g;
+      const long long i = node_index(a, H, lane + 32 * s, t, g);
+      x[s] = ldv(base[g] + i);
+    }
+  }
+}
+
+template <int H, int S>
+__device__ __forceinline__ void store_node_row(const DotArgs& a, const DotSlots<H, S>& sl, int lane, long long t,
+                                               const float4 (&x)[S]) {
+#pragma unroll
+  for (int s = 0; s < S; ++s) {
+    if (sl.head[s] >= 0) {
+      int g;
+      const long long i = node_index(a, H, lane + 32 * s, t, g);
+      st4(a.out[g] + i, x[s]);
+    }
+  }
+}
+
+// per-head sums of the lanes' slot products: every lane gets all H
+template <int H, int S>
+__device__ __forceinline__ void head_sums(const float (&p)[S], const int (&head)[S], float (&z)[H]) {
+#pragma unroll
+  for (int h = 0; h < H; ++h) {
+    float acc = 0.f;
+#pragma unroll
+    for (int s = 0; s < S; ++s) acc += (head[s] == h) ? p[s] : 0.f;
+    z[h] = warp_add(acc);
+  }
+}
+
+template <int H>
+__device__ __forceinline__ float lane_pick(const float (&x)[H], int lane) {
+  float r = 0.f;
+#pragma unroll
+  for (int h = 0; h < H; ++h) r = (lane == h) ? x[h] : r;
+  return r;
+}
+
+template <int H, int S>
+__global__ void __launch_bounds__(256) dot_softmax_aggregate_kernel(DotArgs a, const float* __restrict__ keep,
+                                                                    const long long* __restrict__ row_ptr, long long n_nodes,
+                                                                    float* __restrict__ alpha) {
+  const int lane = threadIdx.x & 31;
+  const long long n_warps = (long long)gridDim.x * (blockDim.x >> 5);
+  const DotSlots<H, S> sl(a, lane);
+  for (long long t = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); t < n_nodes; t += n_warps) {
+    const long long r0 = row_ptr[t], r1 = row_ptr[t + 1];
+    float4 q[S];
+    load_node_row<H, S>(a, a.q, sl, lane, t, q);
+    // pass 1 (keys): z per head, online max and sum of exponentials; z parked in alpha
+    float m[H], sum[H];
+#pragma unroll
+    for (int h = 0; h < H; ++h) { m[h] = -CUDART_INF_F; sum[h] = 0.f; }
+    for (long long e = r0; e < r1; ++e) {
+      float p[S];
+#pragma unroll
+      for (int s = 0; s < S; ++s) p[s] = sl.head[s] >= 0 ? dot4(q[s], ldv(sl.k[s] + e * sl.stride[s])) : 0.f;
+      float z[H];
+      head_sums<H, S>(p, sl.head, z);
+#pragma unroll
+      for (int h = 0; h < H; ++h) {
+        if (z[h] > m[h]) { sum[h] = sum[h] * expf(m[h] - z[h]) + 1.f; m[h] = z[h]; }
+        else sum[h] += expf(z[h] - m[h]);
+      }
+      if (lane < H) alpha[e * H + lane] = lane_pick<H>(z, lane);
+    }
+    // pass 2 (values): alpha over z, out = sum alpha keep v
+    float my_m = 0.f, my_inv = 0.f;
+#pragma unroll
+    for (int h = 0; h < H; ++h) {
+      if (lane == h) { my_m = m[h]; my_inv = 1.f / (sum[h] + 1e-16f); }
+    }
+    float4 acc[S];
+#pragma unroll
+    for (int s = 0; s < S; ++s) acc[s] = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (long long e = r0; e < r1; ++e) {
+      float w = 0.f;
+      if (lane < H) {
+        const float al = expf(alpha[e * H + lane] - my_m) * my_inv;
+        alpha[e * H + lane] = al;
+        w = keep ? al * __ldg(keep + e * H + lane) : al;
+      }
+#pragma unroll
+      for (int s = 0; s < S; ++s) {
+        const float ws = __shfl_sync(0xffffffffu, w, sl.head[s] & 31);
+        if (sl.head[s] >= 0) fma4(acc[s], ws, ldv(sl.k[s] + e * sl.stride[s] + sl.C[s]));
+      }
+    }
+    store_node_row<H, S>(a, sl, lane, t, acc);
+  }
+}
+
+// Backward of the kernel above, same warp-per-node layout; G = d L / d out.  Pass 1 (values): ga_e = v_e . G[t] per head
+// (parked in work[e, h] by lane h), s_t = sum alpha keep ga and gv_e = alpha_e keep_e G[t].  Pass 2 (keys):
+// gz_e = alpha_e (keep_e ga_e - s_t), gk_e = gz_e q[t] and gq[t] = sum gz_e k_e.  Every output row has one owner; the key /
+// value row is read once and its gradient row written once.
+template <int H, int S>
+__global__ void __launch_bounds__(256) dot_softmax_aggregate_bwd_kernel(DotArgs a, const float* __restrict__ alpha,
+                                                                        const float* __restrict__ keep,
+                                                                        const long long* __restrict__ row_ptr,
+                                                                        long long n_nodes, float* __restrict__ work) {
+  const int lane = threadIdx.x & 31;
+  const long long n_warps = (long long)gridDim.x * (blockDim.x >> 5);
+  const DotSlots<H, S> sl(a, lane);
+  for (long long t = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); t < n_nodes; t += n_warps) {
+    const long long r0 = row_ptr[t], r1 = row_ptr[t + 1];
+    float4 x[S];
+    load_node_row<H, S>(a, a.G, sl, lane, t, x);
+    float s_t = 0.f;                   // lane h: sum over the segment of alpha keep ga for head h
+    for (long long e = r0; e < r1; ++e) {
+      float p[S];
+#pragma unroll
+      for (int s = 0; s < S; ++s)
+        p[s] = sl.head[s] >= 0 ? dot4(x[s], ldv(sl.k[s] + e * sl.stride[s] + sl.C[s])) : 0.f;
+      float ga[H];
+      head_sums<H, S>(p, sl.head, ga);
+      float w = 0.f;
+      if (lane < H) {
+        const float g = lane_pick<H>(ga, lane);
+        w = __ldg(alpha + e * H + lane);
+        if (keep) w *= __ldg(keep + e * H + lane);
+        s_t = fmaf(w, g, s_t);
+        work[e * H + lane] = g;
+      }
+#pragma unroll
+      for (int s = 0; s < S; ++s) {
+        const float ws = __shfl_sync(0xffffffffu, w, sl.head[s] & 31);
+        if (sl.head[s] >= 0)
+          st4(sl.gk[s] + e * sl.stride[s] + sl.C[s], make_float4(ws * x[s].x, ws * x[s].y, ws * x[s].z, ws * x[s].w));
+      }
+    }
+    load_node_row<H, S>(a, a.q, sl, lane, t, x);
+    float4 gq[S];
+#pragma unroll
+    for (int s = 0; s < S; ++s) gq[s] = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (long long e = r0; e < r1; ++e) {
+      float gz = 0.f;
+      if (lane < H) {
+        const float kp = keep ? __ldg(keep + e * H + lane) : 1.f;
+        gz = __ldg(alpha + e * H + lane) * (kp * work[e * H + lane] - s_t);
+      }
+#pragma unroll
+      for (int s = 0; s < S; ++s) {
+        const float gs = __shfl_sync(0xffffffffu, gz, sl.head[s] & 31);
+        if (sl.head[s] >= 0) {
+          fma4(gq[s], gs, ldv(sl.k[s] + e * sl.stride[s]));
+          st4(sl.gk[s] + e * sl.stride[s], make_float4(gs * x[s].x, gs * x[s].y, gs * x[s].z, gs * x[s].w));
+        }
+      }
+    }
+    store_node_row<H, S>(a, sl, lane, t, gq);
+  }
+}
+
 static bool vec_ok(const HeadArgs& a) {
   for (int g = 0; g < a.n_groups; ++g)
     if (a.rowlen[g] % 4 != 0 || (a.C[g] / a.n_heads) % 4 != 0) return false;
@@ -499,4 +732,118 @@ extern "C" int eqf_attn_edge_scale(const EqfHeadLayout* lay, const float* alpha,
   dim3 grid((unsigned)blocks, (unsigned)a.n_groups);
   edge_scale_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(a, alpha, keep, reinterpret_cast<const long long*>(dst), n_edges);
   return check_cuda(cudaGetLastError(), "edge_scale_kernel launch");
+}
+
+// ------------------------------------------------------------------------------------------------ dot-product attention
+namespace {
+
+// DotArgs from the q / out head layout; EQF_ERR_UNSUPPORTED outside the float4 layout (channels per head % 4), above
+// DOT_MAX_SLOTS float4 slots per lane or for a head count without a kernel instance
+int fill_dot_args(const EqfHeadLayout* lay, DotArgs& a, int& slots_per_lane, const char* what) {
+  HeadArgs h;
+  int rc = fill_head_args(lay, h);
+  if (rc != EQF_OK) return rc;
+  a.n_groups = h.n_groups;
+  a.slot_start[0] = 0;
+  for (int g = 0; g < EQF_MAX_BLOCKS; ++g) {
+    a.q[g] = a.kv[g] = a.G[g] = nullptr; a.out[g] = a.gkv[g] = nullptr;
+    a.C[g] = a.d[g] = 0;
+  }
+  const int H = h.n_heads;
+  bool ok = H == 1 || H == 2 || H == 4 || H == 8 || H == 16;
+  for (int g = 0; g < h.n_groups; ++g) {
+    a.C[g] = h.C[g]; a.d[g] = h.d[g];
+    ok = ok && (h.C[g] / H) % 4 == 0;
+    a.slot_start[g + 1] = a.slot_start[g] + h.d[g] * h.C[g] / 4;
+  }
+  a.n_slots = a.slot_start[a.n_groups];
+  slots_per_lane = (a.n_slots + 31) / 32;
+  if (!ok || slots_per_lane > DOT_MAX_SLOTS) {
+    set_error(std::string(what) + ": layout not supported (channels per head must be a multiple of 4, at most 1024 "
+              "channels per node row, 1 / 2 / 4 / 8 / 16 heads)");
+    return EQF_ERR_UNSUPPORTED;
+  }
+  return EQF_OK;
+}
+
+// one warp per node, grid-stride: min(ceil(N / 8), 132 * 16) CTAs of 8 warps
+unsigned dot_grid(long long n_nodes) {
+  long long b = (n_nodes + 7) / 8;
+  if (b > 132LL * 16) b = 132LL * 16;
+  return (unsigned)(b < 1 ? 1 : b);
+}
+
+template <int S, typename Launch>
+int dispatch_heads(int H, Launch&& launch) {
+  switch (H) {
+    case 1: launch(std::integral_constant<int, 1>{}, std::integral_constant<int, S>{}); break;
+    case 2: launch(std::integral_constant<int, 2>{}, std::integral_constant<int, S>{}); break;
+    case 4: launch(std::integral_constant<int, 4>{}, std::integral_constant<int, S>{}); break;
+    case 8: launch(std::integral_constant<int, 8>{}, std::integral_constant<int, S>{}); break;
+    default: launch(std::integral_constant<int, 16>{}, std::integral_constant<int, S>{}); break;
+  }
+  return EQF_OK;
+}
+
+// float4 slots per lane: 4 (node rows up to 512 floats: the QM9 L2 heads), 5 (640: OC20 L1) or 8 (1024: MD17 L3); the
+// register count grows with S, so the shipped layouts get the smallest instance that holds their row
+template <typename Launch>
+void dispatch_dot(int H, int slots_per_lane, Launch&& launch) {
+  if (slots_per_lane <= 4) dispatch_heads<4>(H, launch);
+  else if (slots_per_lane == 5) dispatch_heads<5>(H, launch);
+  else dispatch_heads<DOT_MAX_SLOTS>(H, launch);
+}
+
+}  // namespace
+
+extern "C" int eqf_attn_dot_softmax_aggregate(const EqfHeadLayout* lay, const float* const* q, const float* const* kv,
+                                              const float* keep, const int64_t* row_ptr, int64_t n_nodes, float* const* out,
+                                              float* alpha, void* stream) {
+  DotArgs a;
+  int S = 0;
+  int rc = fill_dot_args(lay, a, S, "eqf_attn_dot_softmax_aggregate");
+  if (rc != EQF_OK || n_nodes == 0) return rc;
+  if (q == nullptr || kv == nullptr || out == nullptr || row_ptr == nullptr || alpha == nullptr) {
+    set_error("eqf_attn_dot_softmax_aggregate: null pointer"); return EQF_ERR_INVALID;
+  }
+  for (int g = 0; g < a.n_groups; ++g) {
+    if (q[g] == nullptr || kv[g] == nullptr || out[g] == nullptr) {
+      set_error("eqf_attn_dot_softmax_aggregate: null group"); return EQF_ERR_INVALID;
+    }
+    a.q[g] = q[g]; a.kv[g] = kv[g]; a.out[g] = out[g];
+  }
+  const long long* rp = reinterpret_cast<const long long*>(row_ptr);
+  cudaStream_t st = (cudaStream_t)stream;
+  dispatch_dot(lay->n_heads, S, [&](auto Hc, auto Sc) {
+    dot_softmax_aggregate_kernel<decltype(Hc)::value, decltype(Sc)::value><<<dot_grid(n_nodes), 256, 0, st>>>(
+        a, keep, rp, n_nodes, alpha);
+  });
+  return check_cuda(cudaGetLastError(), "dot_softmax_aggregate_kernel launch");
+}
+
+extern "C" int eqf_attn_dot_softmax_aggregate_bwd(const EqfHeadLayout* lay, const float* const* G, const float* const* q,
+                                                  const float* const* kv, const float* alpha, const float* keep,
+                                                  const int64_t* row_ptr, int64_t n_nodes, float* const* gq,
+                                                  float* const* gkv, float* work, void* stream) {
+  DotArgs a;
+  int S = 0;
+  int rc = fill_dot_args(lay, a, S, "eqf_attn_dot_softmax_aggregate_bwd");
+  if (rc != EQF_OK || n_nodes == 0) return rc;
+  if (G == nullptr || q == nullptr || kv == nullptr || alpha == nullptr || row_ptr == nullptr || gq == nullptr ||
+      gkv == nullptr || work == nullptr) {
+    set_error("eqf_attn_dot_softmax_aggregate_bwd: null pointer"); return EQF_ERR_INVALID;
+  }
+  for (int g = 0; g < a.n_groups; ++g) {
+    if (G[g] == nullptr || q[g] == nullptr || kv[g] == nullptr || gq[g] == nullptr || gkv[g] == nullptr) {
+      set_error("eqf_attn_dot_softmax_aggregate_bwd: null group"); return EQF_ERR_INVALID;
+    }
+    a.G[g] = G[g]; a.q[g] = q[g]; a.kv[g] = kv[g]; a.out[g] = gq[g]; a.gkv[g] = gkv[g];
+  }
+  const long long* rp = reinterpret_cast<const long long*>(row_ptr);
+  cudaStream_t st = (cudaStream_t)stream;
+  dispatch_dot(lay->n_heads, S, [&](auto Hc, auto Sc) {
+    dot_softmax_aggregate_bwd_kernel<decltype(Hc)::value, decltype(Sc)::value><<<dot_grid(n_nodes), 256, 0, st>>>(
+        a, alpha, keep, rp, n_nodes, work);
+  });
+  return check_cuda(cudaGetLastError(), "dot_softmax_aggregate_bwd_kernel launch");
 }

@@ -2,9 +2,12 @@
 
 Same machinery as the graph-attention path - node-level per-degree GEMMs, the fused gather + depth-wise tensor product,
 the per-degree edge linears, segment softmax and the segment sum - with the MLP attention logits replaced by scaled
-``q . k``.  On the kernels that is ``ops.EdgeDot`` (``eqf_attn_edge_dot``: per edge and head, the dot product of an edge
-row with a node row - the kernel that already serves the backward of the aggregation), so the layer needs no new CUDA
-code and keeps the closed autograd family (forces and their training gradients work as for ``GraphAttention``).
+``q . k``.  On CUDA the logits, the segment softmax, the attention dropout and the weighted sum run as one kernel pair
+(``ops.DotSoftmaxAggregate``: ``eqf_attn_dot_softmax_aggregate`` and its backward), which reads the keys and values in
+place from the key / value blocks; under ``create_graph`` (forces) its backward is rebuilt from the closed family.  The
+chain it replaces - ``ops.EdgeDot`` (per edge and head, the dot product of an edge row with a node row), segment softmax,
+``nn.Dropout``, ``ops.attention_aggregate`` on contiguous key and value halves - remains the route for CPU tensors and
+layouts the kernel does not take.
 
 Key / value layout: ``key_value`` emits ``irreps_head x 2H`` sorted and simplified, i.e. per degree a block of
 ``2 H m_l`` channels in which head ``g`` owns channels ``[g m_l, (g + 1) m_l)`` (``Vec2AttnHeads`` :252-285); the first
@@ -112,14 +115,24 @@ class DotProductAttention(torch.nn.Module):
         kv = self.key_value                                                                      # [ref :137-138]
         weight = kv.dtp_rad(edge_scalars, add_offset=False)
         out = kv.lin.planar(kv.dtp.tp.planar_depthwise_gathered(graph, m_src, m_dst, edge_attr, weight, kv.dtp_rad.offset))
-        k = [t.narrow(2, 0, t.shape[2] // 2).contiguous() for t in out]                          # [ref :139-142]
-        v = [t.narrow(2, t.shape[2] // 2, t.shape[2] // 2).contiguous() for t in out]
-
-        z = ops.EdgeDot.apply(self._head_layout, graph, *k, *[t.contiguous() for t in q])        # [ref :145]  q[dst] . k
-        attn = ops.segment_softmax(z.contiguous(), graph)                                        # [ref :146]
-        if self.alpha_dropout is not None:
-            attn = self.alpha_dropout(attn)
-        node = ops.attention_aggregate(self._head_layout, graph, attn.contiguous(), v)           # [ref :149-152]
+        lay = self._head_layout
+        if ops.dot_softmax_aggregate_ok(lay, q[0], graph):
+            # [ref :139-152] q[dst] . k, segment softmax, dropout and the weighted sum in one kernel that reads the keys
+            # and values in place; the mask is drawn as nn.Dropout draws it on the [E, H] weights (same generator use)
+            keep = None
+            if self.alpha_dropout is not None and self.training and self.alpha_dropout.p != 0.0:
+                ones = torch.ones((graph.n_edges, lay.n_heads), device=q[0].device, dtype=q[0].dtype)
+                keep = torch.nn.functional.dropout(ones, self.alpha_dropout.p, True)
+            node = list(ops.DotSoftmaxAggregate.apply(lay, graph, keep, *[t.contiguous() for t in q],
+                                                      *[t.contiguous() for t in out]))
+        else:
+            k = [t.narrow(2, 0, t.shape[2] // 2).contiguous() for t in out]                      # [ref :139-142]
+            v = [t.narrow(2, t.shape[2] // 2, t.shape[2] // 2).contiguous() for t in out]
+            z = ops.EdgeDot.apply(lay, graph, *k, *[t.contiguous() for t in q])                  # [ref :145]  q[dst] . k
+            attn = ops.segment_softmax(z.contiguous(), graph)                                    # [ref :146]
+            if self.alpha_dropout is not None:
+                attn = self.alpha_dropout(attn)
+            node = ops.attention_aggregate(lay, graph, attn.contiguous(), v)                     # [ref :149-152]
         if self.rescale_degree:                                                                  # [ref :154-158]
             degree = (graph.row_ptr[1:] - graph.row_ptr[:-1]).to(node[0].dtype).view(-1, 1, 1)
             node = [t * (degree / _AVG_DEGREE) for t in node]                                    # [ref :152] DP variant only

@@ -1102,6 +1102,109 @@ class MaskedSoftmaxAggregate(torch.autograd.Function):
         return (None, None, gz, None, *gVs)
 
 
+def _kv_check(lay: HeadLayout, kvs, rows: int, what: str):
+    """Key / value blocks ``[rows, d, 2C]`` of the head layout ``lay`` (keys in channels ``[0, C)``, values in ``[C, 2C)``)."""
+    return HeadLayout(lay.ds, [2 * c for c in lay.Cs], lay.n_heads).check(kvs, rows, what)
+
+
+def dot_softmax_aggregate_raw(lay: HeadLayout, qs, kvs, graph: Graph, keep=None):
+    """(outs, alpha) of the dot-product attention kernel: ``z = q[dst] . k`` per head, ``alpha`` = segment softmax of ``z``,
+    ``outs[g][t] = sum_{e->t} alpha keep v`` with keys and values read from the key / value blocks ``kvs``.  ``alpha`` is
+    returned without the mask."""
+    qs = lay.check(qs, graph.n_nodes, "dot_softmax_aggregate q")
+    kvs = _kv_check(lay, kvs, graph.n_edges, "dot_softmax_aggregate kv")
+    dev = qs[0].device
+    outs = [torch.empty((graph.n_nodes, d, C), device=dev, dtype=torch.float32) for d, C in zip(lay.ds, lay.Cs)]
+    alpha = torch.empty((graph.n_edges, lay.n_heads), device=dev, dtype=torch.float32)
+    nbytes = _dot_attn_bytes(lay, graph.n_edges, graph.n_nodes, keep is not None, "forward")
+    with torch.cuda.device(dev), _kernel("dot_softmax_aggregate", nbytes):
+        rc = _lib.load().eqf_attn_dot_softmax_aggregate(ctypes.byref(lay.c), _ptr_array(qs), _ptr_array(kvs),
+                                                        _keep_ptr(keep, alpha), graph.row_ptr.data_ptr(), graph.n_nodes,
+                                                        _ptr_array(outs), alpha.data_ptr(), _stream())
+    _lib.check(rc, "eqf_attn_dot_softmax_aggregate")
+    return outs, alpha
+
+
+def dot_softmax_aggregate_bwd_raw(lay: HeadLayout, Gs, qs, kvs, alpha, graph: Graph, keep=None):
+    """(gqs, gkvs): first-order backward of ``dot_softmax_aggregate_raw`` for the cotangents ``Gs`` of its outputs; the
+    key / value gradient comes in blocks laid out like ``kvs``."""
+    Gs = lay.check(Gs, graph.n_nodes, "dot_softmax_aggregate_bwd G")
+    qs = lay.check(qs, graph.n_nodes, "dot_softmax_aggregate_bwd q")
+    kvs = _kv_check(lay, kvs, graph.n_edges, "dot_softmax_aggregate_bwd kv")
+    alpha = _require_cuda(alpha, "alpha")
+    dev = qs[0].device
+    gqs = [torch.empty_like(q) for q in qs]
+    gkvs = [torch.empty_like(kv) for kv in kvs]
+    work = torch.empty_like(alpha)
+    nbytes = _dot_attn_bytes(lay, graph.n_edges, graph.n_nodes, keep is not None, "backward")
+    with torch.cuda.device(dev), _kernel("dot_softmax_aggregate_bwd", nbytes):
+        rc = _lib.load().eqf_attn_dot_softmax_aggregate_bwd(ctypes.byref(lay.c), _ptr_array(Gs), _ptr_array(qs),
+                                                            _ptr_array(kvs), alpha.data_ptr(), _keep_ptr(keep, alpha),
+                                                            graph.row_ptr.data_ptr(), graph.n_nodes, _ptr_array(gqs),
+                                                            _ptr_array(gkvs), work.data_ptr(), _stream())
+    _lib.check(rc, "eqf_attn_dot_softmax_aggregate_bwd")
+    return gqs, gkvs
+
+
+def _dot_attn_bytes(lay: HeadLayout, E: int, N: int, masked: bool, kind: str) -> int:
+    """Bytes the dot-product attention kernels must move, from shapes: the key / value rows once (and, backward, their
+    gradient once), the node rows once, the [E, H] weights (z parked and re-read in the forward, ga in the backward)."""
+    dv = sum(d * c for d, c in zip(lay.ds, lay.Cs))
+    eh = E * lay.n_heads
+    if kind == "forward":      # kv; q, out; alpha written twice, read once; keep
+        return 4 * (E * 2 * dv + 2 * N * dv + 3 * eh + (eh if masked else 0))
+    # kv, gkv; G, q, gq; alpha read twice, work written and read; keep read twice
+    return 4 * (2 * E * 2 * dv + 3 * N * dv + 4 * eh + (2 * eh if masked else 0))
+
+
+def dot_softmax_aggregate_ok(lay: HeadLayout, q: torch.Tensor, graph: Graph) -> bool:
+    """The dot-product attention kernels run on real CUDA float32 tensors (never on the emulated stand-ins) with float4
+    lanes: channels per head a multiple of 4, node rows of at most 1024 floats, a head count with a kernel instance."""
+    return (q.is_cuda and q.dtype == torch.float32 and graph.n_edges > 0 and lay.n_heads in (1, 2, 4, 8, 16)
+            and all((c // lay.n_heads) % 4 == 0 for c in lay.Cs) and sum(d * c for d, c in zip(lay.ds, lay.Cs)) <= 1024)
+
+
+class DotSoftmaxAggregate(torch.autograd.Function):
+    """Dot-product attention (ref dp_attention_transformer.py:145-151): ``outs[g][t] = sum_{e->t} softmax_t(q[t] . k_e)
+    keep_e v_e``, keys and values read from the key / value blocks ``[E, d, 2C]``.  apply(lay, graph, keep, *qs, *kvs);
+    ``keep`` is None or the ``[E, H]`` attention-dropout mask (0 or 1/(1-p), no gradient).  First-order backward: one
+    kernel.  Under ``create_graph`` the op is rebuilt from the closed family - ``EdgeDot`` on the key half,
+    ``SegSoftmax``, ``* keep``, ``AttnAggregate`` on the value half - so higher derivatives are those of that chain."""
+
+    @staticmethod
+    def forward(ctx, lay: HeadLayout, graph: Graph, keep, *qkv):
+        n = len(lay.ds)
+        qs, kvs = qkv[:n], qkv[n:]
+        extra = () if keep is None else (keep,)
+        outs, alpha = dot_softmax_aggregate_raw(lay, qs, kvs, graph, *extra)
+        ctx.lay, ctx.graph, ctx.has_keep = lay, graph, keep is not None
+        ctx.save_for_backward(alpha, *extra, *qs, *kvs)
+        return tuple(outs)
+
+    @staticmethod
+    def backward(ctx, *Gs):
+        lay, graph = ctx.lay, ctx.graph
+        n = len(lay.ds)
+        alpha, *rest = ctx.saved_tensors
+        keep, qkv = (rest[0], rest[1:]) if ctx.has_keep else (None, rest)
+        qs, kvs = qkv[:n], qkv[n:]
+        Gs = [G.contiguous() if G is not None else torch.zeros((graph.n_nodes, d, C), device=alpha.device)
+              for G, d, C in zip(Gs, lay.ds, lay.Cs)]
+        if torch.is_grad_enabled():
+            def fn(*ins):
+                qq, kk = ins[:n], ins[n:]
+                k = [t.narrow(2, 0, C).contiguous() for t, C in zip(kk, lay.Cs)]
+                v = [t.narrow(2, C, C).contiguous() for t, C in zip(kk, lay.Cs)]
+                a = SegSoftmax.apply(EdgeDot.apply(lay, graph, *k, *qq), graph)
+                return tuple(AttnAggregate.apply(lay, graph, a if keep is None else a * keep, *v))
+            grads = _higher_order_grads(fn, (*qs, *kvs), Gs)
+        else:
+            gqs, gkvs = dot_softmax_aggregate_bwd_raw(lay, Gs, qs, kvs, alpha, graph, *(() if keep is None else (keep,)))
+            grads = [*gqs, *gkvs]
+        grads = [g if need else None for g, need in zip(grads, ctx.needs_input_grad[3:])]
+        return (None, None, None, *grads)
+
+
 def attention_aggregate(lay: HeadLayout, graph: Graph, alpha: Optional[torch.Tensor], Vs: Sequence[torch.Tensor]):
     return list(AttnAggregate.apply(lay, graph, alpha, *Vs))
 

@@ -139,6 +139,25 @@ int eqf_attn_aggregate(const EqfHeadLayout* lay, const float* alpha, const float
 int eqf_attn_softmax_aggregate(const EqfHeadLayout* lay, const float* z, const float* keep, const float* const* V,
                                const int64_t* row_ptr, int64_t n_nodes, float* const* out, float* alpha, void* stream);
 
+/* Dot-product attention (nets/dp_attention_transformer.py:145-151) in ONE kernel over the destination-sorted edge list:
+ * z[e,h] = sum_{j in head h} q[g][dst e, j] k[g][e, j] over all groups, alpha = the PyG segment softmax of z (+1e-16),
+ * out[g][t] = sum_{e->t} alpha[e, head] keep[e, head] v[g][e].  `lay` is the q / out layout [N][d_g][C_g]; the keys and
+ * values are read from the key / value blocks kv[g] [E][d_g][2 C_g] (keys in channels [0, C_g), values in [C_g, 2 C_g)).
+ * keep [E][H] (may be NULL) is the attention-dropout mask (entries 0 or 1/(1-p)); alpha [E][H] is written unmasked for
+ * the backward.  One warp per node, no atomics, deterministic; zero-in-degree nodes get zeros.  Needs channels per head
+ * % 4 == 0, at most 1024 channels per node row and 1 / 2 / 4 / 8 / 16 heads (EQF_ERR_UNSUPPORTED otherwise).      */
+int eqf_attn_dot_softmax_aggregate(const EqfHeadLayout* lay, const float* const* q, const float* const* kv,
+                                   const float* keep, const int64_t* row_ptr, int64_t n_nodes, float* const* out,
+                                   float* alpha, void* stream);
+/* its first-order backward, G[g] = d L / d out [N][d_g][C_g]: with ga = v . G[t] per head and s_t = sum alpha keep ga,
+ * gz = alpha (keep ga - s_t); gkv[g] [E][d_g][2 C_g] gets gk = gz q[t] in the key channels and gv = alpha keep G[t] in
+ * the value channels, gq[g] [N][d_g][C_g] = sum_e gz k.  work [E][H] is scratch (it ends up holding ga).  Same layout
+ * rules; no atomics.                                                                                                */
+int eqf_attn_dot_softmax_aggregate_bwd(const EqfHeadLayout* lay, const float* const* G, const float* const* q,
+                                       const float* const* kv, const float* alpha, const float* keep,
+                                       const int64_t* row_ptr, int64_t n_nodes, float* const* gq, float* const* gkv,
+                                       float* work, void* stream);
+
 /* galpha[e,h] = sum_{j in head h} V[g][e,j] * G[g][dst[e],j]       (transpose of aggregate w.r.t. alpha) */
 int eqf_attn_edge_dot(const EqfHeadLayout* lay, const float* const* V, const float* const* G,
                       const int64_t* dst, int64_t n_edges, float* galpha, void* stream);
