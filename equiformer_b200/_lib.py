@@ -123,6 +123,13 @@ SIGNATURES = {
     "eqf_attn_dot_softmax_aggregate_bwd": (c_int32, [POINTER(EqfHeadLayout), POINTER(c_void_p), POINTER(c_void_p),
                                                      POINTER(c_void_p), c_void_p, c_void_p, c_void_p, c_int64,
                                                      POINTER(c_void_p), POINTER(c_void_p), c_void_p, c_void_p]),
+    "eqf_attn_mlp_rows": (c_int32, [c_int64]),
+    "eqf_attn_mlp_softmax_aggregate": (c_int32, [POINTER(EqfHeadLayout), c_int32, c_float, c_float, c_void_p,
+                                                 POINTER(c_void_p), c_void_p, c_void_p, c_void_p, c_int64,
+                                                 POINTER(c_void_p), c_void_p, c_void_p]),
+    "eqf_attn_mlp_softmax_aggregate_bwd": (c_int32, [POINTER(EqfHeadLayout), c_int32, c_float, c_float, POINTER(c_void_p),
+                                                     c_void_p, POINTER(c_void_p), c_void_p, c_void_p, c_void_p, c_void_p,
+                                                     c_int64, c_void_p, POINTER(c_void_p), c_void_p, c_void_p, c_void_p]),
     "eqf_attn_edge_dot": (c_int32, [POINTER(EqfHeadLayout), POINTER(c_void_p), POINTER(c_void_p), c_void_p, c_int64,
                                     c_void_p, c_void_p]),
     "eqf_attn_edge_scale": (c_int32, [POINTER(EqfHeadLayout), c_void_p, c_void_p, POINTER(c_void_p), c_void_p, c_int64,

@@ -574,6 +574,225 @@ __global__ void __launch_bounds__(256) dot_softmax_aggregate_bwd_kernel(DotArgs 
   }
 }
 
+// ------------------------------------------------------------------------------------------------ linear-message attention
+// The linear-message GraphAttention (ref nets/graph_attention_transformer.py:497-513 with nonlinear_message=False) from the
+// output of sep.lin on: z = sum_k c SLR(t0[alpha k]) alpha_dot[k] per head, the segment softmax, (dropout) and the weighted
+// sum of the value scalars and the l >= 1 value blocks, in one launch.  The 0e row t0 [E, H (A + R)] is read in place: head
+// h owns the alpha pre-activations [h (A + R), h (A + R) + A) and the value scalars [h (A + R) + A, (h + 1)(A + R)) (the
+// Vec2AttnHeads split).  Same warp-per-node scheme as the dot-product kernel: a lane owns up to SA float4 slots of the
+// alpha row and up to SV float4 slots of the value row (value groups concatenated: g = 0 the value scalars inside t0,
+// g >= 1 the blocks V[g] = [E, d_g, H C_g]), every slot inside one head.  Pass 1 reads the alpha channels, forms z per
+// head and keeps an online max and sum of exponentials, parking z in alpha[e, h]; pass 2 turns it into alpha and
+// accumulates alpha keep v.  Lane h alone writes and re-reads alpha[e, h]; no atomics, fixed summation order.
+struct MlpArgs {
+  int H, A, R, T;                        // heads; alpha / value-scalar channels per head; t0 row length H (A + R)
+  int n_groups, n_aslots, n_vslots;      // value groups (g = 0: the value scalars); float4 slots of alpha / value rows
+  int d[EQF_MAX_BLOCKS];                 // components of value group g (d[0] = 1)
+  int C[EQF_MAX_BLOCKS];                 // channels per head of value group g (C[0] = R)
+  int vslot_start[EQF_MAX_BLOCKS + 1];   // prefix sum of d H C / 4
+  float c_slr, k1, k2;                   // alpha_act: c ((1+a)/2 x + (1-a)/2 x (2 sigmoid(x) - 1))
+  const float* t0;                       // [E, T]
+  const float* V[EQF_MAX_BLOCKS];        // g >= 1: [E, d, H C]
+  const float* alpha_dot;                // [H, A]
+  const float* G[EQF_MAX_BLOCKS];        // backward: d L / d out, [N, d, H C]
+  float* out[EQF_MAX_BLOCKS];            // forward: [N, d, H C]
+  float* gt0;                            // backward: [E, T], every channel written
+  float* gV[EQF_MAX_BLOCKS];             // backward, g >= 1: [E, d, H C]
+  float* gdot_part;                      // backward: per-CTA partial sums of d L / d alpha_dot, [grid, H A]
+};
+
+__device__ __forceinline__ float slr_sig(float x) { return 1.f / (1.f + expf(-x)); }
+__device__ __forceinline__ float mlp_act(const MlpArgs& a, float x) {
+  return a.c_slr * (a.k1 * x + a.k2 * x * (2.f * slr_sig(x) - 1.f));
+}
+__device__ __forceinline__ float mlp_dact(const MlpArgs& a, float x) {
+  const float s = slr_sig(x);
+  return a.c_slr * (a.k1 + a.k2 * ((2.f * s - 1.f) + 2.f * x * s * (1.f - s)));
+}
+
+// the lane's slots, fixed for the whole kernel.  Alpha slot c (float4 c of alpha_dot): head c / (A / 4), t0 column
+// head (A + R) + 4 (c % (A / 4)).  Value slot c: group g, offset `local` in the group's node row; its edge row is t0
+// (g = 0, column head (A + R) + A + local % R) or V[g] (column local).  `node` is the node-row buffer (out in the
+// forward, G in the backward), `grad` the edge-row gradient (backward only).
+template <int SA, int SV>
+struct MlpSlots {
+  int ahead[SA], aoff[SA];
+  float4 ad[SA];
+  int vhead[SV], vstride[SV], nrow[SV];
+  const float* v[SV];
+  float* gv[SV];
+  float* node[SV];
+  __device__ __forceinline__ MlpSlots(const MlpArgs& a, int lane, float* const* node_rows, bool backward) {
+    const int H4 = a.A / 4;
+#pragma unroll
+    for (int s = 0; s < SA; ++s) {
+      const int c = lane + 32 * s;
+      const bool on = c < a.n_aslots;
+      const int h = (on ? c : 0) / H4;
+      ahead[s] = on ? h : -1;
+      aoff[s] = h * (a.A + a.R) + 4 * ((on ? c : 0) % H4);
+      ad[s] = on ? ldv(a.alpha_dot + 4 * c) : make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+#pragma unroll
+    for (int s = 0; s < SV; ++s) {
+      const int c0 = lane + 32 * s;
+      const bool on = c0 < a.n_vslots;
+      const int c = on ? c0 : 0;
+      int g = 0;
+      while (g + 1 < a.n_groups && c >= a.vslot_start[g + 1]) ++g;
+      const int HC = a.C[g] * a.H;
+      const int local = (c - a.vslot_start[g]) * 4;
+      const int j = local % HC, h = j / a.C[g];
+      vhead[s] = on ? h : -1;
+      nrow[s] = a.d[g] * HC;
+      node[s] = node_rows[g] + local;
+      if (g == 0) {
+        const int col = h * (a.A + a.R) + a.A + (j - h * a.C[0]);
+        vstride[s] = a.T;
+        v[s] = a.t0 + col;
+        gv[s] = backward ? a.gt0 + col : nullptr;
+      } else {
+        vstride[s] = nrow[s];
+        v[s] = a.V[g] + local;
+        gv[s] = backward ? a.gV[g] + local : nullptr;
+      }
+    }
+  }
+};
+
+template <int H, int SA, int SV>
+__global__ void __launch_bounds__(256) mlp_softmax_aggregate_kernel(MlpArgs a, const float* __restrict__ keep,
+                                                                    const long long* __restrict__ row_ptr, long long n_nodes,
+                                                                    float* __restrict__ alpha) {
+  const int lane = threadIdx.x & 31;
+  const long long n_warps = (long long)gridDim.x * (blockDim.x >> 5);
+  const MlpSlots<SA, SV> sl(a, lane, a.out, false);
+  for (long long t = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); t < n_nodes; t += n_warps) {
+    const long long r0 = row_ptr[t], r1 = row_ptr[t + 1];
+    // pass 1 (alpha channels): z per head; lane h keeps head h's online max and sum of exponentials, z parked in alpha
+    float m = -CUDART_INF_F, sum = 0.f;
+    for (long long e = r0; e < r1; ++e) {
+      const float* row = a.t0 + e * a.T;
+      float p[SA];
+#pragma unroll
+      for (int s = 0; s < SA; ++s) {
+        p[s] = 0.f;
+        if (sl.ahead[s] >= 0) {
+          const float4 x = ldv(row + sl.aoff[s]);
+          p[s] = mlp_act(a, x.x) * sl.ad[s].x + mlp_act(a, x.y) * sl.ad[s].y + mlp_act(a, x.z) * sl.ad[s].z +
+                 mlp_act(a, x.w) * sl.ad[s].w;
+        }
+      }
+      float z[H];
+      head_sums<H, SA>(p, sl.ahead, z);
+      if (lane < H) {
+        const float zl = lane_pick<H>(z, lane);
+        if (zl > m) { sum = sum * expf(m - zl) + 1.f; m = zl; }
+        else sum += expf(zl - m);
+        alpha[e * H + lane] = zl;
+      }
+    }
+    // pass 2 (values): alpha over z, out = sum alpha keep v
+    const float inv = 1.f / (sum + 1e-16f);
+    float4 acc[SV];
+#pragma unroll
+    for (int s = 0; s < SV; ++s) acc[s] = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (long long e = r0; e < r1; ++e) {
+      float w = 0.f;
+      if (lane < H) {
+        const float al = expf(alpha[e * H + lane] - m) * inv;
+        alpha[e * H + lane] = al;
+        w = keep ? al * __ldg(keep + e * H + lane) : al;
+      }
+#pragma unroll
+      for (int s = 0; s < SV; ++s) {
+        const float ws = __shfl_sync(0xffffffffu, w, sl.vhead[s] & 31);
+        if (sl.vhead[s] >= 0) fma4(acc[s], ws, ldv(sl.v[s] + e * sl.vstride[s]));
+      }
+    }
+#pragma unroll
+    for (int s = 0; s < SV; ++s)
+      if (sl.vhead[s] >= 0) st4(sl.node[s] + t * sl.nrow[s], acc[s]);
+  }
+}
+
+// Backward of the kernel above, same layout; G = d L / d out.  Pass 1 (values): ga_e = v_e . G[t] per head (parked in
+// work[e, h] by lane h), s_t = sum alpha keep ga and gv_e = alpha_e keep_e G[t] (the value channels of gt0 and gV).
+// Pass 2 (alpha channels): gz_e = alpha_e (keep_e ga_e - s_t), gt0 = gz alpha_dot act'(t0) and the lane's share of
+// d L / d alpha_dot = sum_e gz act(t0) in registers.  At the end the CTA adds its warps' shares in warp order (shared
+// memory, no atomics) into gdot_part[blockIdx.x]; eqf_colsum reduces the rows.  Every output element has one owner.
+template <int H, int SA, int SV>
+__global__ void __launch_bounds__(256) mlp_softmax_aggregate_bwd_kernel(MlpArgs a, const float* __restrict__ alpha,
+                                                                        const float* __restrict__ keep,
+                                                                        const long long* __restrict__ row_ptr,
+                                                                        long long n_nodes, float* __restrict__ work) {
+  __shared__ float4 red[8][SA * 32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const long long n_warps = (long long)gridDim.x * (blockDim.x >> 5);
+  const MlpSlots<SA, SV> sl(a, lane, const_cast<float* const*>(a.G), true);
+  float4 gdot[SA];
+#pragma unroll
+  for (int s = 0; s < SA; ++s) gdot[s] = make_float4(0.f, 0.f, 0.f, 0.f);
+  for (long long t = (long long)blockIdx.x * (blockDim.x >> 5) + warp; t < n_nodes; t += n_warps) {
+    const long long r0 = row_ptr[t], r1 = row_ptr[t + 1];
+    float4 x[SV];
+#pragma unroll
+    for (int s = 0; s < SV; ++s) x[s] = sl.vhead[s] >= 0 ? ldv(sl.node[s] + t * sl.nrow[s]) : make_float4(0.f, 0.f, 0.f, 0.f);
+    float s_t = 0.f;                   // lane h: sum over the segment of alpha keep ga for head h
+    for (long long e = r0; e < r1; ++e) {
+      float p[SV];
+#pragma unroll
+      for (int s = 0; s < SV; ++s) p[s] = sl.vhead[s] >= 0 ? dot4(x[s], ldv(sl.v[s] + e * sl.vstride[s])) : 0.f;
+      float ga[H];
+      head_sums<H, SV>(p, sl.vhead, ga);
+      float w = 0.f;
+      if (lane < H) {
+        const float g = lane_pick<H>(ga, lane);
+        w = __ldg(alpha + e * H + lane);
+        if (keep) w *= __ldg(keep + e * H + lane);
+        s_t = fmaf(w, g, s_t);
+        work[e * H + lane] = g;
+      }
+#pragma unroll
+      for (int s = 0; s < SV; ++s) {
+        const float ws = __shfl_sync(0xffffffffu, w, sl.vhead[s] & 31);
+        if (sl.vhead[s] >= 0)
+          st4(sl.gv[s] + e * sl.vstride[s], make_float4(ws * x[s].x, ws * x[s].y, ws * x[s].z, ws * x[s].w));
+      }
+    }
+    for (long long e = r0; e < r1; ++e) {
+      float gz = 0.f;
+      if (lane < H) {
+        const float kp = keep ? __ldg(keep + e * H + lane) : 1.f;
+        gz = __ldg(alpha + e * H + lane) * (kp * work[e * H + lane] - s_t);
+      }
+#pragma unroll
+      for (int s = 0; s < SA; ++s) {
+        const float gs = __shfl_sync(0xffffffffu, gz, sl.ahead[s] & 31);
+        if (sl.ahead[s] >= 0) {
+          const float4 xa = ldv(a.t0 + e * a.T + sl.aoff[s]);
+          const float4 ad = sl.ad[s];
+          st4(a.gt0 + e * a.T + sl.aoff[s], make_float4(gs * ad.x * mlp_dact(a, xa.x), gs * ad.y * mlp_dact(a, xa.y),
+                                                         gs * ad.z * mlp_dact(a, xa.z), gs * ad.w * mlp_dact(a, xa.w)));
+          fma4(gdot[s], gs, make_float4(mlp_act(a, xa.x), mlp_act(a, xa.y), mlp_act(a, xa.z), mlp_act(a, xa.w)));
+        }
+      }
+    }
+  }
+#pragma unroll
+  for (int s = 0; s < SA; ++s) red[warp][s * 32 + lane] = gdot[s];
+  __syncthreads();
+  for (int c = threadIdx.x; c < a.n_aslots; c += blockDim.x) {
+    float4 r = red[0][c];
+#pragma unroll
+    for (int w = 1; w < 8; ++w) {
+      const float4 q = red[w][c];
+      r.x += q.x; r.y += q.y; r.z += q.z; r.w += q.w;
+    }
+    st4(a.gdot_part + (long long)blockIdx.x * 4 * a.n_aslots + 4 * c, r);
+  }
+}
+
 static bool vec_ok(const HeadArgs& a) {
   for (int g = 0; g < a.n_groups; ++g)
     if (a.rowlen[g] % 4 != 0 || (a.C[g] / a.n_heads) % 4 != 0) return false;
@@ -846,4 +1065,124 @@ extern "C" int eqf_attn_dot_softmax_aggregate_bwd(const EqfHeadLayout* lay, cons
         a, alpha, keep, rp, n_nodes, work);
   });
   return check_cuda(cudaGetLastError(), "dot_softmax_aggregate_bwd_kernel launch");
+}
+
+// ------------------------------------------------------------------------------------------------ linear-message attention
+namespace {
+
+// float4 slots per lane of the kernel instance for H heads: <SA 2, SV 5> for 8 heads (alpha rows of up to 256 floats,
+// value rows of up to 640: OC20 L1), <SA 1, SV 4> for 2 and 4 (128 / 512: the QM9 / MD17 L2 heads)
+int mlp_alpha_slots(int H) { return H == 8 ? 2 : 1; }
+int mlp_value_slots(int H) { return H == 8 ? 5 : 4; }
+
+// MlpArgs from the output layout `lay` (group 0: the value scalars [N, 1, H R]; groups >= 1: the l >= 1 blocks) and the
+// alpha channels per head; EQF_ERR_UNSUPPORTED outside the float4 layout (A, R and every C_g per head % 4), above the
+// slot counts of the instances or for a head count without one
+int fill_mlp_args(const EqfHeadLayout* lay, int n_alpha, float c_slr, float slope, MlpArgs& a, const char* what) {
+  HeadArgs h;
+  int rc = fill_head_args(lay, h);
+  if (rc != EQF_OK) return rc;
+  const int H = h.n_heads;
+  a.H = H; a.A = n_alpha; a.R = h.C[0] / H; a.T = H * (n_alpha + a.R);
+  a.n_groups = h.n_groups;
+  a.n_aslots = H * n_alpha / 4;
+  a.vslot_start[0] = 0;
+  a.c_slr = c_slr; a.k1 = 0.5f * (1.f + slope); a.k2 = 0.5f * (1.f - slope);
+  a.t0 = a.alpha_dot = nullptr; a.gt0 = a.gdot_part = nullptr;
+  bool ok = (H == 2 || H == 4 || H == 8) && n_alpha > 0 && n_alpha % 4 == 0 && h.d[0] == 1;
+  for (int g = 0; g < EQF_MAX_BLOCKS; ++g) {
+    a.V[g] = a.G[g] = nullptr; a.out[g] = a.gV[g] = nullptr;
+    a.d[g] = a.C[g] = 0;
+  }
+  for (int g = 0; g < h.n_groups; ++g) {
+    a.d[g] = h.d[g]; a.C[g] = h.C[g] / H;
+    ok = ok && a.C[g] % 4 == 0;
+    a.vslot_start[g + 1] = a.vslot_start[g] + h.d[g] * h.C[g] / 4;
+  }
+  a.n_vslots = a.vslot_start[a.n_groups];
+  if (!ok || a.n_aslots > 32 * mlp_alpha_slots(H) || a.n_vslots > 32 * mlp_value_slots(H)) {
+    set_error(std::string(what) + ": layout not supported (2 / 4 / 8 heads, a leading 0e value group, alpha and value "
+              "channels per head multiples of 4, at most 128 alpha and 512 value channels per edge (256 and 640 with 8 "
+              "heads))");
+    return EQF_ERR_UNSUPPORTED;
+  }
+  return EQF_OK;
+}
+
+template <typename Launch>
+void dispatch_mlp(int H, Launch&& launch) {
+  switch (H) {
+    case 2: launch(std::integral_constant<int, 2>{}, std::integral_constant<int, 1>{}, std::integral_constant<int, 4>{}); break;
+    case 4: launch(std::integral_constant<int, 4>{}, std::integral_constant<int, 1>{}, std::integral_constant<int, 4>{}); break;
+    default: launch(std::integral_constant<int, 8>{}, std::integral_constant<int, 2>{}, std::integral_constant<int, 5>{}); break;
+  }
+}
+
+bool aligned16(const void* p) { return ((uintptr_t)p & 15) == 0; }
+
+}  // namespace
+
+extern "C" int eqf_attn_mlp_rows(int64_t n_nodes) { return (int)dot_grid(n_nodes); }
+
+extern "C" int eqf_attn_mlp_softmax_aggregate(const EqfHeadLayout* lay, int32_t n_alpha, float c_slr, float slope,
+                                              const float* t0, const float* const* V, const float* alpha_dot,
+                                              const float* keep, const int64_t* row_ptr, int64_t n_nodes,
+                                              float* const* out, float* alpha, void* stream) {
+  MlpArgs a;
+  int rc = fill_mlp_args(lay, n_alpha, c_slr, slope, a, "eqf_attn_mlp_softmax_aggregate");
+  if (rc != EQF_OK || n_nodes == 0) return rc;
+  if (t0 == nullptr || alpha_dot == nullptr || row_ptr == nullptr || out == nullptr || alpha == nullptr ||
+      (a.n_groups > 1 && V == nullptr)) {
+    set_error("eqf_attn_mlp_softmax_aggregate: null pointer"); return EQF_ERR_INVALID;
+  }
+  a.t0 = t0; a.alpha_dot = alpha_dot;
+  bool al = aligned16(t0) && aligned16(alpha_dot);
+  for (int g = 0; g < a.n_groups; ++g) {
+    if (out[g] == nullptr || (g > 0 && V[g - 1] == nullptr)) {
+      set_error("eqf_attn_mlp_softmax_aggregate: null group"); return EQF_ERR_INVALID;
+    }
+    a.out[g] = out[g];
+    if (g > 0) a.V[g] = V[g - 1];
+    al = al && aligned16(a.out[g]) && (g == 0 || aligned16(a.V[g]));
+  }
+  if (!al) { set_error("eqf_attn_mlp_softmax_aggregate: operands must be 16-byte aligned"); return EQF_ERR_INVALID; }
+  const long long* rp = reinterpret_cast<const long long*>(row_ptr);
+  cudaStream_t st = (cudaStream_t)stream;
+  dispatch_mlp(a.H, [&](auto Hc, auto SAc, auto SVc) {
+    mlp_softmax_aggregate_kernel<decltype(Hc)::value, decltype(SAc)::value, decltype(SVc)::value>
+        <<<dot_grid(n_nodes), 256, 0, st>>>(a, keep, rp, n_nodes, alpha);
+  });
+  return check_cuda(cudaGetLastError(), "mlp_softmax_aggregate_kernel launch");
+}
+
+extern "C" int eqf_attn_mlp_softmax_aggregate_bwd(const EqfHeadLayout* lay, int32_t n_alpha, float c_slr, float slope,
+                                                  const float* const* G, const float* t0, const float* const* V,
+                                                  const float* alpha_dot, const float* alpha, const float* keep,
+                                                  const int64_t* row_ptr, int64_t n_nodes, float* gt0, float* const* gV,
+                                                  float* work, float* gdot_part, void* stream) {
+  MlpArgs a;
+  int rc = fill_mlp_args(lay, n_alpha, c_slr, slope, a, "eqf_attn_mlp_softmax_aggregate_bwd");
+  if (rc != EQF_OK || n_nodes == 0) return rc;
+  if (G == nullptr || t0 == nullptr || alpha_dot == nullptr || alpha == nullptr || row_ptr == nullptr || gt0 == nullptr ||
+      work == nullptr || gdot_part == nullptr || (a.n_groups > 1 && (V == nullptr || gV == nullptr))) {
+    set_error("eqf_attn_mlp_softmax_aggregate_bwd: null pointer"); return EQF_ERR_INVALID;
+  }
+  a.t0 = t0; a.alpha_dot = alpha_dot; a.gt0 = gt0; a.gdot_part = gdot_part;
+  bool al = aligned16(t0) && aligned16(alpha_dot) && aligned16(gt0) && aligned16(gdot_part);
+  for (int g = 0; g < a.n_groups; ++g) {
+    if (G[g] == nullptr || (g > 0 && (V[g - 1] == nullptr || gV[g - 1] == nullptr))) {
+      set_error("eqf_attn_mlp_softmax_aggregate_bwd: null group"); return EQF_ERR_INVALID;
+    }
+    a.G[g] = G[g];
+    if (g > 0) { a.V[g] = V[g - 1]; a.gV[g] = gV[g - 1]; }
+    al = al && aligned16(a.G[g]) && (g == 0 || (aligned16(a.V[g]) && aligned16(a.gV[g])));
+  }
+  if (!al) { set_error("eqf_attn_mlp_softmax_aggregate_bwd: operands must be 16-byte aligned"); return EQF_ERR_INVALID; }
+  const long long* rp = reinterpret_cast<const long long*>(row_ptr);
+  cudaStream_t st = (cudaStream_t)stream;
+  dispatch_mlp(a.H, [&](auto Hc, auto SAc, auto SVc) {
+    mlp_softmax_aggregate_bwd_kernel<decltype(Hc)::value, decltype(SAc)::value, decltype(SVc)::value>
+        <<<dot_grid(n_nodes), 256, 0, st>>>(a, alpha, keep, rp, n_nodes, work);
+  });
+  return check_cuda(cudaGetLastError(), "mlp_softmax_aggregate_bwd_kernel launch");
 }

@@ -327,6 +327,15 @@ class GraphAttention(torch.nn.Module):
             raise NotImplementedError("irreps_head must be sorted (l ascending, even first) with one entry per irrep")
         self._head_layout = ops.HeadLayout([ir.dim for _, ir in irreps_attn_heads],
                                            [mul for mul, _ in irreps_attn_heads], num_heads)
+        # linear message: the fused logits + softmax + aggregation kernel (ops.MlpSoftmaxAggregate) reads the 0e row of
+        # sep.lin, [alpha | value scalars] per head, when that row leads the output and the value scalars lead the heads
+        self._mlp_layout = None
+        if not self.nonlinear_message:
+            lin_out = self.sep.lin.irreps_out
+            width = num_heads * mul_alpha_head + self._head_layout.Cs[0]
+            if (lin_out[0].ir.is_scalar() and lin_out[0].mul == width and irreps_attn_heads[0].ir.is_scalar()
+                    and mul_alpha_head > 0):
+                self._mlp_layout = ops.MlpAttnLayout(self._head_layout, mul_alpha_head, self.alpha_act.acts[0].cst, 0.2)
         # K1 (ops.DtpLinear): both depth-wise products feed their per-degree linears on chip when the linears are canonical
         self._fuse_act = (self._gate_layout is not None and _fused_linear_possible(self.sep_act.lin, self.sep_act.dtp))
         self._fuse_value = (self.nonlinear_message and _fused_linear_possible(self.sep_value.lin, self.sep_value.dtp))
@@ -418,24 +427,39 @@ class GraphAttention(torch.nn.Module):
             rest = per_head.shape[2] - A
             value = ([per_head.narrow(2, A, rest).reshape(E, 1, H * rest)] if rest > 0 else []) + list(out[1:])
 
-        # logits -> segment softmax -> weighted aggregation                               [ref :506-513]
-        z = logits if logits is not None else (self.alpha_act(alpha) * self.alpha_dot).sum(dim=-1)
         no_drop = self.alpha_dropout is None or not self.training or self.alpha_dropout.p == 0.0
-        if ops.softmax_aggregate_ok(self._head_layout, z):
-            # K2: softmax over the destination segment and the weighted aggregation in one kernel
-            vs = [v.contiguous() for v in value]
-            if no_drop:
-                node = list(ops.SoftmaxAggregate.apply(self._head_layout, graph, z.contiguous(), *vs))
+        node = None
+        if not self.nonlinear_message and self._mlp_layout is not None:
+            t0 = first.reshape(E, -1)
+            if ops.mlp_softmax_aggregate_ok(self._mlp_layout, t0, graph):
+                # [ref :500-513] logits, segment softmax, dropout and the weighted sum in one kernel that reads the alpha
+                # channels and the value scalars of the sep.lin row in place; the mask is drawn as below (same
+                # generator use, capturable)
+                keep = None
+                if not no_drop:
+                    ones = torch.ones((E, H), device=t0.device, dtype=t0.dtype)
+                    keep = torch.nn.functional.dropout(ones, self.alpha_dropout.p, True)
+                node = list(ops.MlpSoftmaxAggregate.apply(self._mlp_layout, graph, keep, self.alpha_dot.view(H, A),
+                                                          t0.contiguous(), *[t.contiguous() for t in out[1:]]))
+        if node is None:
+            # logits -> segment softmax -> weighted aggregation                           [ref :506-513]
+            z = logits if logits is not None else (self.alpha_act(alpha) * self.alpha_dot).sum(dim=-1)
+            if ops.softmax_aggregate_ok(self._head_layout, z):
+                # K2: softmax over the destination segment and the weighted aggregation in one kernel
+                vs = [v.contiguous() for v in value]
+                if no_drop:
+                    node = list(ops.SoftmaxAggregate.apply(self._head_layout, graph, z.contiguous(), *vs))
+                else:
+                    # [ref :509] the dropout mask, drawn as nn.Dropout draws it on the [E, H] weights (same generator
+                    # use, capturable), is applied inside K2 and its backward
+                    keep = torch.nn.functional.dropout(torch.ones_like(z), self.alpha_dropout.p, True)
+                    node = list(ops.MaskedSoftmaxAggregate.apply(self._head_layout, graph, z.contiguous(), keep, *vs))
             else:
-                # [ref :509] the dropout mask, drawn as nn.Dropout draws it on the [E, H] weights (same generator use,
-                # capturable), is applied inside K2 and its backward
-                keep = torch.nn.functional.dropout(torch.ones_like(z), self.alpha_dropout.p, True)
-                node = list(ops.MaskedSoftmaxAggregate.apply(self._head_layout, graph, z.contiguous(), keep, *vs))
-        else:
-            attn = ops.segment_softmax(z.contiguous(), graph)
-            if self.alpha_dropout is not None:
-                attn = self.alpha_dropout(attn)
-            node = ops.attention_aggregate(self._head_layout, graph, attn.contiguous(), [v.contiguous() for v in value])
+                attn = ops.segment_softmax(z.contiguous(), graph)
+                if self.alpha_dropout is not None:
+                    attn = self.alpha_dropout(attn)
+                node = ops.attention_aggregate(self._head_layout, graph, attn.contiguous(),
+                                               [v.contiguous() for v in value])
 
         if self.rescale_degree:                                                           # [ref :516-520]
             degree = (graph.row_ptr[1:] - graph.row_ptr[:-1]).to(node[0].dtype).view(-1, 1, 1)

@@ -217,3 +217,8 @@ OC20_L1_256_NONLINEAR_AUX = dict(OC20_L1_256_NONLINEAR, irreps_feature="512x0e+2
 
 # the model block of oc20/configs/is2re/all/graph_attention_transformer/l1_256_blocks@18_nonlinear_aux_g@4_local.yml:31-60
 OC20_L1_256_BLOCKS18_NONLINEAR_AUX = dict(OC20_L1_256_NONLINEAR_AUX, num_layers=18)
+
+# the model block of oc20/configs/is2re/all/graph_attention_transformer/l1_256_g@2_local.yml:5-31, the linear-message
+# configuration (its attention runs on ops.MlpSoftmaxAggregate).  The model blocks of all/.../l1_256_g@4_local.yml and
+# 100k/.../l1_256_g@2_local.yml are identical.
+OC20_L1_256 = dict(OC20_L1_256_NONLINEAR, num_layers=8, nonlinear_message=False)

@@ -1205,6 +1205,162 @@ class DotSoftmaxAggregate(torch.autograd.Function):
         return (None, None, None, *grads)
 
 
+class MlpAttnLayout:
+    """Static description of the linear-message attention op (see ``eqf_attn_mlp_softmax_aggregate`` in
+    include/eqf_b200.h): ``head`` is the output layout (group 0 the value scalars ``[N, 1, H R]``, then the l >= 1
+    blocks), ``n_alpha`` the alpha channels per head, ``c_slr`` and ``slope`` the constant and slope of ``alpha_act``.
+    The op's 0e input row ``t0`` is ``[E, H (A + R)]``, head h owning ``[h (A + R), (h + 1)(A + R))``: A alpha
+    pre-activations, then R value scalars."""
+
+    def __init__(self, head: HeadLayout, n_alpha: int, c_slr: float, slope: float):
+        self.head, self.n_alpha, self.c_slr, self.slope = head, int(n_alpha), float(c_slr), float(slope)
+        self.n_scalars = head.Cs[0] // head.n_heads
+        self.width = head.n_heads * (self.n_alpha + self.n_scalars)
+
+
+def mlp_logits_torch(lay: MlpAttnLayout, t0, alpha_dot):
+    """``z [E, H]``: ``alpha_act`` on the alpha channels of ``t0``, times ``alpha_dot``, summed per head (ref :506-507);
+    the differentiable statement the ``create_graph`` route and the CPU tests use."""
+    E, H, A = t0.shape[0], lay.head.n_heads, lay.n_alpha
+    a = t0.reshape(E, H, A + lay.n_scalars)[:, :, :A]
+    slr = 0.5 * (1 + lay.slope) * a + 0.5 * (1 - lay.slope) * a * (2 * torch.sigmoid(a) - 1)
+    return (lay.c_slr * slr * alpha_dot.reshape(1, H, A)).sum(-1)
+
+
+def mlp_value_scalars(lay: MlpAttnLayout, t0):
+    """The value scalars of ``t0`` as the ``[E, 1, H R]`` group 0 of the output layout (a strided view)."""
+    E, H, A, R = t0.shape[0], lay.head.n_heads, lay.n_alpha, lay.n_scalars
+    return t0.reshape(E, H, A + R).narrow(2, A, R).reshape(E, 1, H * R)
+
+
+def _mlp_check(lay: MlpAttnLayout, t0, Vs, graph: Graph, what: str):
+    t0 = _require_cuda(t0, f"{what} t0")
+    if tuple(t0.shape) != (graph.n_edges, lay.width):
+        raise ValueError(f"{what}: t0 must be [{graph.n_edges}, {lay.width}], got {tuple(t0.shape)}")
+    hl = lay.head
+    if len(Vs) != len(hl.ds) - 1:
+        raise ValueError(f"{what}: expected {len(hl.ds) - 1} value blocks")
+    out = []
+    for v, d, C in zip(Vs, hl.ds[1:], hl.Cs[1:]):
+        v = _require_cuda(v, f"{what} V")
+        if tuple(v.shape) != (graph.n_edges, d, C):
+            raise ValueError(f"{what}: value block shape {tuple(v.shape)} != {(graph.n_edges, d, C)}")
+        out.append(v)
+    return t0, out
+
+
+def mlp_softmax_aggregate_raw(lay: MlpAttnLayout, t0, Vs, alpha_dot, graph: Graph, keep=None):
+    """(outs, alpha) of the linear-message attention kernel: ``z`` from the alpha channels of ``t0``, ``alpha`` = segment
+    softmax of ``z``, ``outs[g][t] = sum_{e->t} alpha keep v`` over the value scalars of ``t0`` and the blocks ``Vs``.
+    ``alpha`` is returned without the mask."""
+    t0, Vs = _mlp_check(lay, t0, Vs, graph, "mlp_softmax_aggregate")
+    alpha_dot = _require_cuda(alpha_dot, "alpha_dot")
+    hl, dev = lay.head, t0.device
+    outs = [torch.empty((graph.n_nodes, d, C), device=dev, dtype=torch.float32) for d, C in zip(hl.ds, hl.Cs)]
+    alpha = torch.empty((graph.n_edges, hl.n_heads), device=dev, dtype=torch.float32)
+    nbytes = _mlp_attn_bytes(lay, graph.n_edges, graph.n_nodes, keep is not None, "forward")
+    with torch.cuda.device(dev), _kernel("mlp_softmax_aggregate", nbytes):
+        rc = _lib.load().eqf_attn_mlp_softmax_aggregate(ctypes.byref(hl.c), lay.n_alpha, lay.c_slr, lay.slope,
+                                                        t0.data_ptr(), _ptr_array(Vs), alpha_dot.data_ptr(),
+                                                        _keep_ptr(keep, alpha), graph.row_ptr.data_ptr(), graph.n_nodes,
+                                                        _ptr_array(outs), alpha.data_ptr(), _stream())
+    _lib.check(rc, "eqf_attn_mlp_softmax_aggregate")
+    return outs, alpha
+
+
+def mlp_softmax_aggregate_bwd_raw(lay: MlpAttnLayout, Gs, t0, Vs, alpha_dot, alpha, graph: Graph, keep=None):
+    """(gt0, gVs, galpha_dot): first-order backward of ``mlp_softmax_aggregate_raw`` for the cotangents ``Gs`` of its
+    outputs; ``gt0`` covers the whole row (alpha and value channels), ``galpha_dot`` is ``[H A]``."""
+    hl = lay.head
+    Gs = hl.check(Gs, graph.n_nodes, "mlp_softmax_aggregate_bwd G")
+    t0, Vs = _mlp_check(lay, t0, Vs, graph, "mlp_softmax_aggregate_bwd")
+    alpha_dot = _require_cuda(alpha_dot, "alpha_dot")
+    alpha = _require_cuda(alpha, "alpha")
+    lib = _lib.load()
+    gt0 = torch.empty_like(t0)
+    gVs = [torch.empty_like(v) for v in Vs]
+    work = torch.empty_like(alpha)
+    part = torch.empty((lib.eqf_attn_mlp_rows(graph.n_nodes), hl.n_heads * lay.n_alpha), device=t0.device,
+                       dtype=torch.float32)
+    nbytes = _mlp_attn_bytes(lay, graph.n_edges, graph.n_nodes, keep is not None, "backward")
+    with torch.cuda.device(t0.device), _kernel("mlp_softmax_aggregate_bwd", nbytes):
+        rc = lib.eqf_attn_mlp_softmax_aggregate_bwd(ctypes.byref(hl.c), lay.n_alpha, lay.c_slr, lay.slope, _ptr_array(Gs),
+                                                    t0.data_ptr(), _ptr_array(Vs), alpha_dot.data_ptr(), alpha.data_ptr(),
+                                                    _keep_ptr(keep, alpha), graph.row_ptr.data_ptr(), graph.n_nodes,
+                                                    gt0.data_ptr(), _ptr_array(gVs), work.data_ptr(), part.data_ptr(),
+                                                    _stream())
+    _lib.check(rc, "eqf_attn_mlp_softmax_aggregate_bwd")
+    return gt0, gVs, colsum_raw(part)
+
+
+def _mlp_attn_bytes(lay: MlpAttnLayout, E: int, N: int, masked: bool, kind: str) -> int:
+    """Bytes the linear-message attention kernels must move, from shapes: the t0 row and the value blocks once (and,
+    backward, their gradient once), the node rows once, the [E, H] weights (z parked and re-read in the forward, ga in
+    the backward).  The backward's per-CTA ``alpha_dot`` partials (a few hundred rows of H A floats) are left out."""
+    hl = lay.head
+    dv = sum(d * c for d, c in zip(hl.ds, hl.Cs))          # value channels per row, value scalars included
+    ea = E * hl.n_heads * lay.n_alpha                        # alpha channels of t0
+    eh = E * hl.n_heads
+    if kind == "forward":      # t0 alpha + values; out; alpha written twice, read once; keep
+        return 4 * (ea + E * dv + N * dv + 3 * eh + (eh if masked else 0))
+    # t0 alpha + values, gt0; G; alpha read twice, work written and read; keep read twice
+    return 4 * (2 * (ea + E * dv) + N * dv + 4 * eh + (2 * eh if masked else 0))
+
+
+def mlp_softmax_aggregate_ok(lay: MlpAttnLayout, t0: torch.Tensor, graph: Graph) -> bool:
+    """The linear-message attention kernels run on real CUDA float32 tensors (never on the emulated stand-ins) with
+    float4 lanes: 2 / 4 / 8 heads, a leading 0e value group, alpha and value channels per head multiples of 4, at most
+    128 alpha and 512 value channels per edge (256 and 640 with 8 heads)."""
+    hl = lay.head
+    H = hl.n_heads
+    wide = H == 8
+    return (t0.is_cuda and t0.dtype == torch.float32 and graph.n_edges > 0 and H in (2, 4, 8) and hl.ds[0] == 1
+            and lay.n_alpha % 4 == 0 and all((c // H) % 4 == 0 for c in hl.Cs)
+            and H * lay.n_alpha <= (256 if wide else 128)
+            and sum(d * c for d, c in zip(hl.ds, hl.Cs)) <= (640 if wide else 512))
+
+
+class MlpSoftmaxAggregate(torch.autograd.Function):
+    """Linear-message graph attention (ref graph_attention_transformer.py:497-513, ``nonlinear_message=False``):
+    ``outs[g][t] = sum_{e->t} softmax_t(z)[e, head] keep_e v_e`` with ``z = sum_k c SLR(t0[alpha k]) alpha_dot[k]`` per
+    head and the values = the value scalars of ``t0``, then the l >= 1 blocks.  apply(lay, graph, keep, alpha_dot [H, A],
+    t0 [E, H (A + R)], *Vs); ``keep`` is None or the ``[E, H]`` attention-dropout mask (0 or 1/(1-p), no gradient).
+    First-order backward: one kernel plus the column sum of its ``alpha_dot`` partials.  Under ``create_graph`` the op is
+    rebuilt from the activation statement (``mlp_logits_torch``), ``SegSoftmax``, ``* keep`` and ``AttnAggregate``, so
+    higher derivatives are those of that chain."""
+
+    @staticmethod
+    def forward(ctx, lay: MlpAttnLayout, graph: Graph, keep, alpha_dot, t0, *Vs):
+        extra = () if keep is None else (keep,)
+        alpha_dot = alpha_dot.contiguous()
+        outs, alpha = mlp_softmax_aggregate_raw(lay, t0, Vs, alpha_dot, graph, *extra)
+        ctx.lay, ctx.graph, ctx.has_keep = lay, graph, keep is not None
+        ctx.save_for_backward(alpha, *extra, alpha_dot, t0, *Vs)
+        return tuple(outs)
+
+    @staticmethod
+    def backward(ctx, *Gs):
+        lay, graph = ctx.lay, ctx.graph
+        hl = lay.head
+        alpha, *rest = ctx.saved_tensors
+        keep, rest = (rest[0], rest[1:]) if ctx.has_keep else (None, rest)
+        alpha_dot, t0, *Vs = rest
+        Gs = [G.contiguous() if G is not None else torch.zeros((graph.n_nodes, d, C), device=alpha.device, dtype=alpha.dtype)
+              for G, d, C in zip(Gs, hl.ds, hl.Cs)]
+        if torch.is_grad_enabled():
+            def fn(ad, tt, *vv):
+                a = SegSoftmax.apply(mlp_logits_torch(lay, tt, ad).contiguous(), graph)
+                vals = [mlp_value_scalars(lay, tt).contiguous(), *vv]
+                return tuple(AttnAggregate.apply(hl, graph, a if keep is None else a * keep, *vals))
+            grads = _higher_order_grads(fn, (alpha_dot, t0, *Vs), Gs)
+        else:
+            gt0, gVs, gdot = mlp_softmax_aggregate_bwd_raw(lay, Gs, t0, Vs, alpha_dot, alpha, graph,
+                                                           *(() if keep is None else (keep,)))
+            grads = [gdot.view_as(alpha_dot), gt0, *gVs]
+        grads = [g if need else None for g, need in zip(grads, ctx.needs_input_grad[3:])]
+        return (None, None, None, *grads)
+
+
 def attention_aggregate(lay: HeadLayout, graph: Graph, alpha: Optional[torch.Tensor], Vs: Sequence[torch.Tensor]):
     return list(AttnAggregate.apply(lay, graph, alpha, *Vs))
 

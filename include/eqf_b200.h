@@ -158,6 +158,33 @@ int eqf_attn_dot_softmax_aggregate_bwd(const EqfHeadLayout* lay, const float* co
                                        const int64_t* row_ptr, int64_t n_nodes, float* const* gq, float* const* gkv,
                                        float* work, void* stream);
 
+/* Linear-message graph attention (nets/graph_attention_transformer.py:497-513, nonlinear_message=False) in ONE kernel
+ * over the destination-sorted edge list, from the 0e output of sep.lin (bias included) read in place: t0 [E][H (A+R)],
+ * head h owning the alpha pre-activations [h(A+R), h(A+R)+A) and the value scalars [h(A+R)+A, (h+1)(A+R)) (Vec2AttnHeads).
+ *   z[e,h] = sum_k c_slr SLR(t0[e, h(A+R)+k]) alpha_dot[h,k],  SLR(x) = (1+s)/2 x + (1-s)/2 x (2 sigmoid(x) - 1), s = slope;
+ *   alpha  = the PyG segment softmax of z (+1e-16);
+ *   out[g][t] = sum_{e->t} alpha[e, head] keep[e, head] v[g][e], v[0] = the value scalars, v[g >= 1] = V[g-1].
+ * `lay` is the output layout: group 0 [N][1][H R], groups g >= 1 [N][d_g][H C_g]; V holds the n_groups - 1 blocks
+ * [E][d_g][H C_g] of the l >= 1 values.  alpha_dot [H][A]; keep [E][H] (may be NULL) is the attention-dropout mask
+ * (entries 0 or 1/(1-p)); alpha [E][H] is written unmasked for the backward.  One warp per node in a grid of
+ * eqf_attn_mlp_rows(n_nodes) CTAs, no atomics, deterministic; zero-in-degree nodes get zeros.  Needs 2 / 4 / 8 heads, A,
+ * R and every C_g multiples of 4, at most 128 alpha and 512 value channels per edge with 2 or 4 heads (256 and 640 with
+ * 8), 16-byte aligned operands (EQF_ERR_UNSUPPORTED / EQF_ERR_INVALID otherwise).                                     */
+int eqf_attn_mlp_rows(int64_t n_nodes);
+int eqf_attn_mlp_softmax_aggregate(const EqfHeadLayout* lay, int32_t n_alpha, float c_slr, float slope, const float* t0,
+                                   const float* const* V, const float* alpha_dot, const float* keep,
+                                   const int64_t* row_ptr, int64_t n_nodes, float* const* out, float* alpha, void* stream);
+/* its first-order backward, G[g] = d L / d out [N][d_g][H C_g]: with ga = v . G[t] per head, s_t = sum alpha keep ga
+ * and gz = alpha (keep ga - s_t), gt0 [E][H (A+R)] gets gz alpha_dot c_slr SLR'(t0) in the alpha channels and
+ * alpha keep G[0][t] in the value channels (every channel written), gV[g-1] = alpha keep G[g][t], and
+ * gdot_part [eqf_attn_mlp_rows(n_nodes)][H A] the per-CTA partial sums of d L / d alpha_dot = sum_e gz c_slr SLR(t0)
+ * (reduce the rows with eqf_colsum).  work [E][H] is scratch.  Same layout rules; no atomics: bitwise repeatable.      */
+int eqf_attn_mlp_softmax_aggregate_bwd(const EqfHeadLayout* lay, int32_t n_alpha, float c_slr, float slope,
+                                       const float* const* G, const float* t0, const float* const* V,
+                                       const float* alpha_dot, const float* alpha, const float* keep,
+                                       const int64_t* row_ptr, int64_t n_nodes, float* gt0, float* const* gV,
+                                       float* work, float* gdot_part, void* stream);
+
 /* galpha[e,h] = sum_{j in head h} V[g][e,j] * G[g][dst[e],j]       (transpose of aggregate w.r.t. alpha) */
 int eqf_attn_edge_dot(const EqfHeadLayout* lay, const float* const* V, const float* const* G,
                       const int64_t* dst, int64_t n_edges, float* galpha, void* stream);
