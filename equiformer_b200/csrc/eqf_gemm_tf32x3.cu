@@ -11,12 +11,18 @@
 //                    (128-byte rows, SWIZZLE_128B) into a ring of shared-memory stages (full / empty mbarriers); the
 //                    ring runs across tile boundaries, so the next tile's operands land while the consumers store
 //   warpgroups 1, 2  consumers, 64 rows each: A fragments from shared memory -> hi / lo in registers -> 3 wgmma per
-//                    8-deep k-step and 64-column chunk into a k-tile accumulator, added to the running sum in registers
+//                    8-deep k-step and 64-column chunk into a k-tile accumulator, added to the running sum in registers.
+//                    Two fragment sets: the next k-tile (of this tile or the next) is split while the current one's
+//                    MMAs run.  A finished tile goes through a shared-memory staging buffer to TMA stores, which drain
+//                    while the consumer computes its next tile.
 // Persistence matters for the tall products with a shallow reduction (K = 32, 64: the data gradients of the 1e / 2e
 // linears): they are bound by their output stores, and a CTA per tile would wait for a TMA round trip before each store.
 // Weight gradient: the same roles over the CTA's slice of the R rows.  Both operands are "MN-major" (the reduction runs
 // along the strided dimension), which tf32 wgmma cannot read from shared memory: A^T is read as register fragments
-// straight from its swizzled TMA boxes, and the consumers transpose + split each G tile into K-major hi / lo tiles first.
+// straight from its swizzled TMA boxes, and the consumers transpose + split each G tile into K-major hi / lo tiles -
+// the next stage's while the current stage's MMAs run.
+// Every k-tile's MMAs start from a zero accumulator (scale-d 0) and nothing but wgmma writes it between fence and wait,
+// so ptxas keeps the MMA chains asynchronous (no injected warpgroup.arrive / wait).
 #include <cuda.h>
 #include <cuda_runtime.h>
 
@@ -46,29 +52,96 @@ struct Smem {
   static constexpr int kABytes = BM * kRowBytes;
   static constexpr int kBBytes = BN * kRowBytes;
   static constexpr int kStageBytes = kABytes + 2 * kBBytes;       // A raw | B hi | B lo
-  static constexpr int kStagesRaw = (kSmemBudget - 2048) / kStageBytes;
+  static constexpr int kOutBytes = 64 * BN * 4;                   // one consumer's C tile: BN / 32 boxes of [64 x 32]
+  static constexpr int kStagesRaw = (kSmemBudget - 2048 - 2 * kOutBytes) / kStageBytes;
   static constexpr int kStages = kStagesRaw > kMaxStages ? kMaxStages : kStagesRaw;
   static_assert(kStages >= 2, "tile does not fit shared memory");
-  static constexpr int kTotal = kStages * kStageBytes + 1024 /* barriers */ + 1024 /* alignment slack */;
+  static constexpr int kTotal = kStages * kStageBytes + 2 * kOutBytes + 1024 /* barriers */ + 1024 /* alignment slack */;
 };
 
 struct Params {
-  float* C;
-  long long M, ldc;
   long long n_tiles;      // m_blocks * n_blocks, m-block major (the n-blocks of one m-block run side by side: A is
   int n_blocks;           // read from HBM once and from L2 for the other column tiles)
   int N, K;
 };
 
+// The consumer's warpgroup tile [64 x BN] into its staging buffer: BN / 32 boxes of [64 rows x 32 columns], 128-byte
+// rows, SWIZZLE_128B (the layout the C tensor map stores from).  A warp's float2 writes of one accumulator pair cover
+// eight rows x two 16-byte chunks, which the swizzle spreads over all 32 banks: two wavefronts, no conflict.
+template <int BN>
+__device__ __forceinline__ void stage_acc(const float* acc, uint32_t out, int row_w, int lane) {
+#pragma unroll
+  for (int i = 0; i < BN / 2; i += 2) {
+    const int r = row_w + acc_row(i, lane), c = acc_col(i, lane), cc = c & 31;
+    const uint32_t addr = out + (uint32_t)(c >> 5) * 8192u + (uint32_t)r * 128u + (uint32_t)((((cc >> 2) ^ (r & 7)) << 4) + (cc & 3) * 4);
+    asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(acc[i]), "f"(acc[i + 1]) : "memory");
+  }
+}
+
+// One consumer step: issue the MMAs of the current k-tile (fragments hc / lc), split the next k-tile into hn / ln while
+// they run, then retire the stage and promote the k-tile sum; at the last k-tile of a tile, hand the tile to a TMA store.
+// Returns false after the consumer's last k-tile.
+template <int BN>
+struct Consumer {
+  using S = Smem<BN>;
+  uint8_t* smem;
+  uint64_t *full, *empty;
+  const CUtensorMap* map_c;
+  uint32_t out;                            // this warpgroup's staging buffer
+  long long tile, n_tiles;
+  int kt, k_tiles, n_blocks, s, row_w, row_wg, lane, wg;
+  uint32_t ph;
+  bool leader;
+  float acc[BN / 2], part[BN / 2];         // running sum, this k-tile's tensor-core sum
+
+  __device__ __forceinline__ bool step(const uint32_t (&hc)[16], const uint32_t (&lc)[16], uint32_t (&hn)[16],
+                                       uint32_t (&ln)[16]) {
+    const uint32_t st = smem_u32(smem + s * S::kStageBytes);
+    mma_ktile_3xtf32<BN, true>(part, hc, lc, st + S::kABytes, st + S::kABytes + S::kBBytes);
+    const int s_cur = s;
+    const int kt_cur = kt;
+    const long long tile_cur = tile;
+    if (++s == S::kStages) { s = 0; ph ^= 1; }
+    if (++kt == k_tiles) { kt = 0; tile += gridDim.x; }
+    const bool more = tile < n_tiles;
+    if (more) {
+      mbar_wait_hint(&full[s], ph);
+      load_a_split(smem_u32(smem + s * S::kStageBytes), row_wg, lane, hn, ln);
+    }
+    wgmma_wait<0>();
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[s_cur]);
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = kt_cur == 0 ? part[i] : acc[i] + part[i];
+    if (kt_cur == k_tiles - 1) {
+      // the staging buffer is free once the previous tile's store has read it
+      if (leader) bulk_wait_read();
+      named_barrier(wg, 128);
+      stage_acc<BN>(acc, out, row_w, lane);
+      fence_async_smem();
+      named_barrier(wg, 128);
+      if (leader) {
+        const int m0 = (int)(tile_cur / n_blocks) * BM + (wg - 1) * 64;
+        const int n0 = (int)(tile_cur % n_blocks) * BN;
+#pragma unroll
+        for (int b = 0; b < BN / 32; ++b) tma_store_2d(map_c, n0 + 32 * b, m0, out + (uint32_t)b * 8192u);
+        bulk_commit();
+      }
+    }
+    return more;
+  }
+};
+
 template <int BN>
 __global__ void __launch_bounds__(kThreads, 1)
 gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_bhi,
-                   const __grid_constant__ CUtensorMap map_blo, Params p) {
+                   const __grid_constant__ CUtensorMap map_blo, const __grid_constant__ CUtensorMap map_c, Params p) {
   using S = Smem<BN>;
   constexpr int kStages = S::kStages;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + kStages * S::kStageBytes);
+  uint8_t* out_base = smem + kStages * S::kStageBytes;
+  uint64_t* full = reinterpret_cast<uint64_t*>(out_base + 2 * S::kOutBytes);
   uint64_t* empty = full + kStages;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2;
@@ -101,32 +174,22 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_const
     }
   } else {
     reg_alloc<232>();
-    const int row_wg = (wg - 1) * 64 + (warp & 3) * 16;      // first of this warp's 16 rows inside the tile
-    int s = 0;
-    uint32_t ph = 0;
-    for (long long tile = blockIdx.x; tile < p.n_tiles; tile += gridDim.x) {
-      const long long m0 = (tile / p.n_blocks) * BM;
-      const int n0 = (int)(tile % p.n_blocks) * BN;
-      float acc[BN / 2], part[BN / 2];     // running sum, this k-tile's tensor-core sum
-#pragma unroll
-      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-      for (int kt = 0; kt < k_tiles; ++kt) {
-        mbar_wait_hint(&full[s], ph);
-        const uint32_t st = smem_u32(smem + s * S::kStageBytes);
-        uint32_t hi[16], lo[16];
-        load_a_split(st, row_wg, lane, hi, lo);
-#pragma unroll
-        for (int i = 0; i < BN / 2; ++i) part[i] = 0.f;
-        mma_ktile_3xtf32<BN>(part, hi, lo, st + S::kABytes, st + S::kABytes + S::kBBytes);
-        wgmma_wait<0>();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&empty[s]);
-#pragma unroll
-        for (int i = 0; i < BN / 2; ++i) acc[i] += part[i];
-        if (++s == kStages) { s = 0; ph ^= 1; }
-      }
-      store_acc<BN>(acc, p.C, p.ldc, m0 + row_wg, p.M, n0, p.N, lane, false);
-    }
+    if ((long long)blockIdx.x >= p.n_tiles) return;
+    Consumer<BN> c;
+    c.smem = smem; c.full = full; c.empty = empty; c.map_c = &map_c;
+    c.out = smem_u32(out_base + (wg - 1) * S::kOutBytes);
+    c.tile = blockIdx.x; c.n_tiles = p.n_tiles; c.kt = 0; c.k_tiles = k_tiles; c.n_blocks = p.n_blocks;
+    c.s = 0; c.ph = 0; c.lane = lane; c.wg = wg;
+    c.row_w = (warp & 3) * 16;
+    c.row_wg = (wg - 1) * 64 + c.row_w;                     // first of this warp's 16 rows inside the tile
+    c.leader = (threadIdx.x & 127) == 0;
+    if (c.leader) prefetch_map(&map_c);
+    // two fragment sets: the split of the next k-tile runs while the MMAs of the current one are in flight
+    uint32_t h0[16], l0[16], h1[16], l1[16];
+    mbar_wait_hint(&full[0], 0);
+    load_a_split(smem_u32(smem), c.row_wg, lane, h0, l0);
+    while (c.step(h0, l0, h1, l1) && c.step(h1, l1, h0, l0)) {}
+    if (c.leader) bulk_wait();
   }
 }
 
@@ -154,8 +217,8 @@ __global__ void split_transpose_kernel(const float* __restrict__ w, long long ld
 }
 
 template <int BN>
-static int launch(const CUtensorMap& ma, const CUtensorMap& mh, const CUtensorMap& ml, const Params& p, long long m_blocks,
-                  int n_blocks, cudaStream_t s) {
+static int launch(const CUtensorMap& ma, const CUtensorMap& mh, const CUtensorMap& ml, const CUtensorMap& mc, const Params& p,
+                  long long m_blocks, int n_blocks, cudaStream_t s) {
   static std::once_flag once;
   static cudaError_t attr_err = cudaSuccess;
   std::call_once(once, [] {
@@ -167,7 +230,7 @@ static int launch(const CUtensorMap& ma, const CUtensorMap& mh, const CUtensorMa
   q.n_tiles = m_blocks * n_blocks;
   const long long sms = device_sms();
   const unsigned grid = (unsigned)(q.n_tiles < sms ? q.n_tiles : sms);
-  gemm_tf32x3_kernel<BN><<<grid, kThreads, Smem<BN>::kTotal, s>>>(ma, mh, ml, q);
+  gemm_tf32x3_kernel<BN><<<grid, kThreads, Smem<BN>::kTotal, s>>>(ma, mh, ml, mc, q);
   return check_cuda(cudaGetLastError(), "gemm_tf32x3_kernel launch");
 }
 
@@ -258,15 +321,10 @@ wgrad_tf32x3_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_cons
     reg_alloc<232>();
     const int ct = threadIdx.x - 128;                          // 0 .. 255
     const int row_wg = (wgi - 1) * 64 + (warp & 3) * 16;
-    float acc[BN / 2], part[BN / 2];       // running sum, this k-tile's tensor-core sum
-#pragma unroll
-    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-    for (int kt = 0; kt < k_tiles; ++kt) {
-      const int s = kt % kStages;
-      mbar_wait_hint(&full[s], (kt / kStages) & 1);
-      const uint32_t st = smem_u32(smem + s * S::kStageBytes);
-      const uint32_t g_raw = st + S::kABytes, g_hi = g_raw + S::kGRawBytes, g_lo = g_hi + S::kGBytes;
-      // G tile [BKR][BN] -> G^T hi / lo [BN][BKR]: item (n, 4 reduction rows) = one 16-byte chunk of each plane
+    // G tile [BKR][BN] of stage s -> G^T hi / lo [BN][BKR]: item (n, 4 reduction rows) = one 16-byte chunk of each plane
+    auto transpose_split = [&](int s) {
+      const uint32_t g_raw = smem_u32(smem + s * S::kStageBytes) + S::kABytes, g_hi = g_raw + S::kGRawBytes,
+                     g_lo = g_hi + S::kGBytes;
       for (int i = ct; i < BN * (BKR / 4); i += kConsumerThreads) {
         const int n = i % BN, rq = i / BN;
         float4 v;
@@ -282,18 +340,38 @@ wgrad_tf32x3_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_cons
                                        tf32_rn_fast(v.w - h.w)));
       }
       fence_async_smem();
-      named_barrier(1, kConsumerThreads);
-      uint32_t hi[16], lo[16];
-      load_at_split(st, row_wg, lane, hi, lo);
-#pragma unroll
-      for (int i = 0; i < BN / 2; ++i) part[i] = 0.f;
-      mma_ktile_3xtf32<BN>(part, hi, lo, g_hi, g_lo);
+    };
+    float acc[BN / 2], part[BN / 2];       // running sum, this k-tile's tensor-core sum
+    // One k-tile: its MMAs (fragments hc / lc, G^T planes of its stage) run while the consumers wait for the next stage,
+    // transpose + split its G tile and split its A^T fragments into hn / ln; then the k-tile sum is promoted.
+    int kt = 0;
+    auto step = [&](const uint32_t (&hc)[16], const uint32_t (&lc)[16], uint32_t (&hn)[16], uint32_t (&ln)[16]) {
+      const int s = kt % kStages;
+      const uint32_t g_hi = smem_u32(smem + s * S::kStageBytes) + S::kABytes + S::kGRawBytes;
+      mma_ktile_3xtf32<BN, true>(part, hc, lc, g_hi, g_hi + S::kGBytes);
+      const bool more = kt + 1 < k_tiles;
+      if (more) {
+        const int s1 = (kt + 1) % kStages;
+        mbar_wait_hint(&full[s1], ((kt + 1) / kStages) & 1);
+        transpose_split(s1);
+        load_at_split(smem_u32(smem + s1 * S::kStageBytes), row_wg, lane, hn, ln);
+      }
       wgmma_wait<0>();
       __syncwarp();
       if (lane == 0) mbar_arrive(&empty[s]);
 #pragma unroll
-      for (int i = 0; i < BN / 2; ++i) acc[i] += part[i];
-    }
+      for (int i = 0; i < BN / 2; ++i) acc[i] = kt == 0 ? part[i] : acc[i] + part[i];
+      // every consumer's share of the next G^T planes is written before any warpgroup's MMAs read them
+      if (more) named_barrier(1, kConsumerThreads);
+      ++kt;
+      return more;
+    };
+    uint32_t h0[16], l0[16], h1[16], l1[16];
+    mbar_wait_hint(&full[0], 0);
+    transpose_split(0);
+    load_at_split(smem_u32(smem), row_wg, lane, h0, l0);
+    named_barrier(1, kConsumerThreads);
+    while (step(h0, l0, h1, l1) && step(h1, l1, h0, l0)) {}
     float* out = p.reduce ? p.out : p.out + (long long)blockIdx.z * p.K1 * p.N;
     store_acc<BN>(acc, out, p.N, m0 + row_wg, p.K1, n0, p.N, lane, p.reduce != 0);
   }
@@ -370,17 +448,19 @@ extern "C" int eqf_gemm_tf32x3(const float* A, const float* Bt, float* C, int64_
   const int bn = per <= 32 ? 32 : per <= 64 ? 64 : per <= 96 ? 96 : 128;
   const int n_blocks = (int)((N + bn - 1) / bn);
   const long long m_blocks = (M + BM - 1) / BM;
+  if (M > 0x7fffffffLL) { set_error("eqf_gemm_tf32x3: M too large"); return EQF_ERR_UNSUPPORTED; }
   Params p;
-  p.C = C; p.M = M; p.ldc = ldc; p.N = (int)N; p.K = (int)K;
-  CUtensorMap ma, mh, ml;
+  p.N = (int)N; p.K = (int)K;
+  CUtensorMap ma, mh, ml, mc;
   if ((rc = make_map_2d(&ma, A, M, K, lda, BM, BK)) != EQF_OK) return rc;
   if ((rc = make_map_2d(&mh, hi, N, K, K, bn, BK)) != EQF_OK) return rc;
   if ((rc = make_map_2d(&ml, lo, N, K, K, bn, BK)) != EQF_OK) return rc;
+  if ((rc = make_map_2d(&mc, C, M, N, ldc, 64, 32)) != EQF_OK) return rc;     // the TMA store clips to [M, N]
   switch (bn) {
-    case 32: return launch<32>(ma, mh, ml, p, m_blocks, n_blocks, s);
-    case 64: return launch<64>(ma, mh, ml, p, m_blocks, n_blocks, s);
-    case 96: return launch<96>(ma, mh, ml, p, m_blocks, n_blocks, s);
-    default: return launch<128>(ma, mh, ml, p, m_blocks, n_blocks, s);
+    case 32: return launch<32>(ma, mh, ml, mc, p, m_blocks, n_blocks, s);
+    case 64: return launch<64>(ma, mh, ml, mc, p, m_blocks, n_blocks, s);
+    case 96: return launch<96>(ma, mh, ml, mc, p, m_blocks, n_blocks, s);
+    default: return launch<128>(ma, mh, ml, mc, p, m_blocks, n_blocks, s);
   }
 }
 

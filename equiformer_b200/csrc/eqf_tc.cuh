@@ -55,6 +55,16 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, i
   asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
                ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(smem_u32(bar)) : "memory");
 }
+// shared -> global tensor store of one box (bulk-group completion: commit, then wait before the source is reused)
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, int c0, int c1, uint32_t src) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%1, %2}], [%3];"
+               ::"l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(src) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// every committed bulk store has finished reading its shared-memory source
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// every committed bulk store has completed
+__device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 __device__ __forceinline__ void prefetch_map(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
 }
@@ -107,21 +117,24 @@ __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.a
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
-// D[64 x 32] (+)= A[64 x 8] (registers, tf32 fragment) x B[8 x 32] (shared memory, K-major SWIZZLE_128B)
+// D[64 x 32] (+)= A[64 x 8] (registers, tf32 fragment) x B[8 x 32] (shared memory, K-major SWIZZLE_128B); kScaleD = 0
+// overwrites D instead of adding to it
+template <int kScaleD = 1>
 __device__ __forceinline__ void wgmma_rs_n32(float* d, const uint32_t* a, uint64_t b_desc) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
       "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
       "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
       "{%16, %17, %18, %19}, %20, p, 1, 1;\n\t}"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
         "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc));
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "n"(kScaleD));
 }
 // D[64 x 64] (+)= A[64 x 8] (registers, tf32 fragment) x B[8 x 64] (shared memory, K-major SWIZZLE_128B)
+template <int kScaleD = 1>
 __device__ __forceinline__ void wgmma_rs_n64(float* d, const uint32_t* a, uint64_t b_desc) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
       "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
       "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
       "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
@@ -130,7 +143,49 @@ __device__ __forceinline__ void wgmma_rs_n64(float* d, const uint32_t* a, uint64
         "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
         "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
         "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc));
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "n"(kScaleD));
+}
+
+// D[64 x 96] (+)= A[64 x 8] x B[8 x 96]: one instruction for the whole tile width (same accumulator layout as
+// consecutive 64-column chunks)
+template <int kScaleD = 1>
+__device__ __forceinline__ void wgmma_rs_n96(float* d, const uint32_t* a, uint64_t b_desc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %53, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n96k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, "
+      "{%48, %49, %50, %51}, %52, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "n"(kScaleD));
+}
+// D[64 x 128] (+)= A[64 x 8] x B[8 x 128]: one instruction for the whole tile width (same accumulator layout as
+// consecutive 64-column chunks)
+template <int kScaleD = 1>
+__device__ __forceinline__ void wgmma_rs_n128(float* d, const uint32_t* a, uint64_t b_desc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "{%64, %65, %66, %67}, %68, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "n"(kScaleD));
 }
 
 constexpr int kKTile = 32;            // reduction depth of one shared-memory stage: 32 tf32 = one 128-byte row
@@ -160,10 +215,13 @@ __device__ __forceinline__ void load_a_split(uint32_t tile, int row0, int lane, 
 }
 
 // acc[64 x BN] += A[64 x 32] B[32 x BN] in 3xTF32: B hi / lo planes are [BN][32] K-major SWIZZLE_128B tiles at b_hi / b_lo.
-// hi / lo hold the fragments of N4 / 4 k-steps from k-step kb0 on (load_a_split).  Column chunks of 64 (and one of 32 when
-// BN % 64 == 32); chunk j's accumulators are acc[32 j ..].  Issues the MMAs and commits them as one group; the caller
-// waits (wgmma_wait) before touching acc, hi, lo or the B tiles again.
-template <int BN, int N4>
+// hi / lo hold the fragments of N4 / 4 k-steps from k-step kb0 on (load_a_split).  BN = 96, 128: one instruction per
+// product; other widths: column chunks of 64 (and one of 32 when BN % 64 == 32), chunk j's accumulators at acc[32 j ..]
+// (the same layout).  Issues the MMAs and commits them as one group; the caller
+// waits (wgmma_wait) before touching acc, hi, lo or the B tiles again.  kFresh: the first MMA of each chunk overwrites acc
+// (scale-d 0) instead of adding to it, so a k-tile sum needs no zeroing by ordinary instructions - register writes between
+// wgmma.fence and the MMAs would make ptxas serialise the chain.
+template <int BN, bool kFresh = false, int N4>
 __device__ __forceinline__ void mma_ktile_3xtf32(float* acc, const uint32_t (&hi)[N4], const uint32_t (&lo)[N4], uint32_t b_hi,
                                                  uint32_t b_lo, int kb0 = 0) {
   static_assert(BN % 32 == 0 && BN >= 32 && BN <= 256, "BN must be a multiple of 32 up to 256");
@@ -171,19 +229,37 @@ __device__ __forceinline__ void mma_ktile_3xtf32(float* acc, const uint32_t (&hi
 #pragma unroll
   for (int kb = 0; kb < N4 / 4; ++kb) {
     const uint64_t adv = (uint64_t)(((kb0 + kb) * 32) >> 4);
+    if constexpr (BN == 96 || BN == 128) {
+      // the whole width in one instruction per product: the A fragment is read once per k-step instead of per chunk
+      const uint64_t dh = smem_desc_sw128(b_hi) + adv, dl = smem_desc_sw128(b_lo) + adv;
+      if constexpr (BN == 96) {
+        if (kFresh && kb == 0) wgmma_rs_n96<0>(acc, &lo[kb * 4], dh);
+        else wgmma_rs_n96(acc, &lo[kb * 4], dh);
+        wgmma_rs_n96(acc, &hi[kb * 4], dl);
+        wgmma_rs_n96(acc, &hi[kb * 4], dh);
+      } else {
+        if (kFresh && kb == 0) wgmma_rs_n128<0>(acc, &lo[kb * 4], dh);
+        else wgmma_rs_n128(acc, &lo[kb * 4], dh);
+        wgmma_rs_n128(acc, &hi[kb * 4], dl);
+        wgmma_rs_n128(acc, &hi[kb * 4], dh);
+      }
+    } else {
 #pragma unroll
-    for (int j = 0; j < BN / 64; ++j) {
-      const uint64_t dh = smem_desc_sw128(b_hi + (uint32_t)j * 8192u) + adv, dl = smem_desc_sw128(b_lo + (uint32_t)j * 8192u) + adv;
-      wgmma_rs_n64(acc + 32 * j, &lo[kb * 4], dh);
-      wgmma_rs_n64(acc + 32 * j, &hi[kb * 4], dl);
-      wgmma_rs_n64(acc + 32 * j, &hi[kb * 4], dh);
-    }
-    if constexpr (BN % 64 == 32) {
-      constexpr int j = BN / 64;
-      const uint64_t dh = smem_desc_sw128(b_hi + (uint32_t)j * 8192u) + adv, dl = smem_desc_sw128(b_lo + (uint32_t)j * 8192u) + adv;
-      wgmma_rs_n32(acc + 32 * j, &lo[kb * 4], dh);
-      wgmma_rs_n32(acc + 32 * j, &hi[kb * 4], dl);
-      wgmma_rs_n32(acc + 32 * j, &hi[kb * 4], dh);
+      for (int j = 0; j < BN / 64; ++j) {
+        const uint64_t dh = smem_desc_sw128(b_hi + (uint32_t)j * 8192u) + adv, dl = smem_desc_sw128(b_lo + (uint32_t)j * 8192u) + adv;
+        if (kFresh && kb == 0) wgmma_rs_n64<0>(acc + 32 * j, &lo[kb * 4], dh);
+        else wgmma_rs_n64(acc + 32 * j, &lo[kb * 4], dh);
+        wgmma_rs_n64(acc + 32 * j, &hi[kb * 4], dl);
+        wgmma_rs_n64(acc + 32 * j, &hi[kb * 4], dh);
+      }
+      if constexpr (BN % 64 == 32) {
+        constexpr int j = BN / 64;
+        const uint64_t dh = smem_desc_sw128(b_hi + (uint32_t)j * 8192u) + adv, dl = smem_desc_sw128(b_lo + (uint32_t)j * 8192u) + adv;
+        if (kFresh && kb == 0) wgmma_rs_n32<0>(acc + 32 * j, &lo[kb * 4], dh);
+        else wgmma_rs_n32(acc + 32 * j, &lo[kb * 4], dh);
+        wgmma_rs_n32(acc + 32 * j, &hi[kb * 4], dl);
+        wgmma_rs_n32(acc + 32 * j, &hi[kb * 4], dh);
+      }
     }
   }
   wgmma_commit();
