@@ -13,7 +13,11 @@ blocks of ``irreps_feature`` such as ``512x0e+256x1e`` feed only the auxiliary h
 ``GraphAttention`` (attribute ``auxiliary_head``) over the frame's edges, reading the normed final features before
 ``out_dropout`` and predicting one vector per atom (``1x1o`` if ``irreps_feature`` has a ``1o`` block, else ``1x1e``).
 ``forward`` then returns ``(energy [G, 1], aux [N, 3])``; its per-edge work runs on the same kernels as the blocks.  The
-training objective that goes with it is in ``equiformer_b200.oc20_objective``.  The attention head
+training objective that goes with it is in ``equiformer_b200.oc20_objective``.
+
+The named configurations below restate the ``model:`` blocks of the shipped IS2RE yml files: ``OC20_L1_256_NONLINEAR``,
+its auxiliary-head variants, the linear-message ``OC20_L1_256`` and the E(3) ``OC20_L1_256_E3_NONLINEAR``, whose node
+features carry ``0o`` / ``1o`` blocks and whose spherical harmonics are ``1x0e+1x1o``.  The attention head
 (``use_attention_head``), learned node attributes and atom-pair edge attributes are not implemented and raise.
 """
 from __future__ import annotations
@@ -222,3 +226,11 @@ OC20_L1_256_BLOCKS18_NONLINEAR_AUX = dict(OC20_L1_256_NONLINEAR_AUX, num_layers=
 # configuration (its attention runs on ops.MlpSoftmaxAggregate).  The model blocks of all/.../l1_256_g@4_local.yml and
 # 100k/.../l1_256_g@2_local.yml are identical.
 OC20_L1_256 = dict(OC20_L1_256_NONLINEAR, num_layers=8, nonlinear_message=False)
+
+# the model block of oc20/configs/is2re/all/graph_attention_transformer/l1_256_e3_nonlinear_g@2_local.yml:5-31, the E(3)
+# configuration: odd-parity blocks next to the even ones.  Its depth-wise products (edge-degree embedding, sep_act and
+# sep_value of every block) share the plan 256x0e+64x0o+64x1e+64x1o x 1x0e+1x1o, generated as codegen tag "oc20_l1_e3".
+OC20_L1_256_E3_NONLINEAR = dict(
+    OC20_L1_256_NONLINEAR, irreps_node_embedding="256x0e+64x0o+64x1e+64x1o", irreps_sh="1x0e+1x1o",
+    irreps_head="32x0e+8x0o+8x1e+8x1o", irreps_pre_attn="256x0e+64x0o+64x1e+64x1o",
+    irreps_mlp_mid="768x0e+192x0o+192x1e+192x1o")

@@ -1,6 +1,6 @@
 """Operator-boundary microbenchmark of the DTP kernels (SURVEY.md section 8d): GB/s vs the measured HBM peak.
 
-usage: python tools/dtp_microbench.py [config] [E] [iters]      config in {qm9_l2, md17_l3, oc20_l1}
+usage: python tools/dtp_microbench.py [config] [E] [iters]      config in {qm9_l2, md17_l3, oc20_l1, oc20_l1_e3}
 Times each kernel with CUDA events on the launching stream after warm-up; operands (>= 0.5 GB) exceed the 126 MB L2.
 """
 import json
@@ -16,7 +16,8 @@ from equiformer_b200.nets.graph_attention_transformer import DepthwiseTensorProd
 
 CONFIGS = {"qm9_l2": ("128x0e+64x1e+32x2e", "1x0e+1x1e+1x2e"),
            "md17_l3": ("128x0e+64x1e+64x2e+32x3e", "1x0e+1x1e+1x2e+1x3e"),
-           "oc20_l1": ("256x0e+128x1e", "1x0e+1x1e")}
+           "oc20_l1": ("256x0e+128x1e", "1x0e+1x1e"),
+           "oc20_l1_e3": ("256x0e+64x0o+64x1e+64x1o", "1x0e+1x1o")}      # OC20_L1_256_E3_NONLINEAR
 
 
 def main():
@@ -58,7 +59,7 @@ def main():
     rows["grad_xw(shared w)"] = timeit(lambda: ops.dtp_grad_xw_raw(plan, xs, y, ws, gs), ops._dtp_bytes(plan, E, True, "grad_xw"))
     rows["grad_x"] = timeit(lambda: ops.dtp_grad_x_raw(plan, gs, y, w), ops._dtp_bytes(plan, E, False, "grad_x"))
     rows["grad_y"] = timeit(lambda: ops.dtp_grad_y_raw(plan, xs, w, gs, y), ops._dtp_bytes(plan, E, False, "grad_y"))
-    out = {"config": name, "E": E, "variant": os.environ.get("EQF_DTP_VARIANT", "tma"), "tile": os.environ.get("EQF_TILE_EDGES", "8"),
+    out = {"config": name, "E": E, "generated": bool(plan.generated), "variant": os.environ.get("EQF_DTP_VARIANT", "tma"), "tile": os.environ.get("EQF_TILE_EDGES", "8"),
            "peak_gbs": peak}
     for k, (us, gbs) in rows.items():
         out[k] = {"us": round(us, 1), "gb_s": round(gbs, 1), "frac": round(gbs / peak, 3)}
