@@ -118,9 +118,13 @@ __global__ void __launch_bounds__(256) radius_graph_pbc_kernel(const float* __re
       ia = img / (nb * nc) - rep_a;
       ib = (img / nc) % nb - rep_b;
       ic = img % nc - rep_c;
-      const float ox = ia * cm[0] + ib * cm[3] + ic * cm[6];
-      const float oy = ia * cm[1] + ib * cm[4] + ic * cm[7];
-      const float oz = ia * cm[2] + ib * cm[5] + ic * cm[8];
+      // image offset ia a + ib b + ic c as separately rounded products summed in that order, the arithmetic of the torch
+      // statement: left to the compiler the sum becomes an FMA chain, which rounds differently and so keeps or drops
+      // some pairs within an ulp of r^2 that the statement decides the other way
+      const float fa = (float)ia, fb = (float)ib, fc = (float)ic;
+      const float ox = __fadd_rn(__fadd_rn(__fmul_rn(fa, cm[0]), __fmul_rn(fb, cm[3])), __fmul_rn(fc, cm[6]));
+      const float oy = __fadd_rn(__fadd_rn(__fmul_rn(fa, cm[1]), __fmul_rn(fb, cm[4])), __fmul_rn(fc, cm[7]));
+      const float oz = __fadd_rn(__fadd_rn(__fmul_rn(fa, cm[2]), __fmul_rn(fb, cm[5])), __fmul_rn(fc, cm[8]));
       const float dx = __ldg(pos + 3 * j) + ox - xi, dy = __ldg(pos + 3 * j + 1) + oy - yi, dz = __ldg(pos + 3 * j + 2) + oz - zi;
       d2 = __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
       hit = d2 <= r2 && d2 > 1e-4f;          // ocpmodels' masks: distance_sqr <= r^2 and distance_sqr > 0.0001 (the atom itself)

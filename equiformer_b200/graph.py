@@ -118,7 +118,10 @@ def radius_graph_pbc_torch(pos, batch, cell, r: float, max_neighbors: int = 500)
     for f in range(int(batch.max()) + 1 if batch.numel() else 0):
         idx = (batch == f).nonzero().flatten()
         p = pos[idx].float()
-        shift = (imgs.to(pos.dtype) @ cell[f].to(pos.dtype)).float()                       # [n_img, 3]
+        # n_a a + n_b b + n_c c as separately rounded products summed in that order, as the kernels form it (a matmul
+        # leaves the rounding order to the library)
+        n, c = imgs.to(pos.dtype), cell[f].to(pos.dtype)
+        shift = ((n[:, 0:1] * c[0] + n[:, 1:2] * c[1]) + n[:, 2:3] * c[2]).float()           # [n_img, 3]
         d = p[None, :, None, :] + shift[None, None, :, :] - p[:, None, None, :]             # [i, j, img, 3]
         d2 = (d[..., 0] * d[..., 0] + d[..., 1] * d[..., 1]) + d[..., 2] * d[..., 2]
         hit = (d2 <= r * r) & (d2 > 1e-4)
@@ -129,13 +132,17 @@ def radius_graph_pbc_torch(pos, batch, cell, r: float, max_neighbors: int = 500)
 
 
 def _cap_neighbours(edge, offsets, d2, n, max_neighbors):
-    """Keep the ``max_neighbors`` nearest hits of every centre (ocpmodels ``get_max_neighbors_mask``); order preserved."""
+    """Keep the ``max_neighbors`` nearest hits of every centre (ocpmodels ``get_max_neighbors_mask``), exact on the
+    given ``d2``; of equal ``d2`` the earlier hit in the list is kept.  Order preserved."""
     deg = torch.bincount(edge[1], minlength=n)
     if max_neighbors is None or edge.shape[1] == 0 or int(deg.max()) <= max_neighbors:
         return edge, offsets, d2
     row_ptr = torch.zeros(n + 1, dtype=torch.long, device=edge.device)
     torch.cumsum(deg, 0, out=row_ptr[1:])
-    order = torch.argsort(d2 + edge[1].to(d2.dtype) * (float(d2.max()) + 1.0), stable=True)   # by centre, then distance
+    # by centre, then distance, then list position: two stable sorts, so that no combined float key rounds near-equal
+    # distances of high-index centres into ties
+    order = torch.argsort(d2, stable=True)
+    order = order[torch.argsort(edge[1][order], stable=True)]
     rank = torch.empty_like(order)
     rank[order] = torch.arange(order.numel(), device=order.device) - row_ptr[edge[1][order]]
     keep = rank < max_neighbors

@@ -26,6 +26,7 @@ import math
 from dataclasses import dataclass
 from typing import Dict, Optional, Tuple
 
+import numpy as np
 import torch
 import torch.nn.functional as F
 
@@ -402,6 +403,66 @@ def pbc_edge_vectors(pos, cell, batch, edge_src, edge_dst, cell_offsets):
     cells = cell.to(pos.dtype).index_select(0, batch.index_select(0, edge_dst))
     offsets = torch.bmm(cell_offsets.to(pos.dtype).view(-1, 1, 3), cells).view(-1, 3)
     return pos.index_select(0, edge_src) - pos.index_select(0, edge_dst) + offsets
+
+
+def nearest_neighbours_mask(centre, d2, max_neighbors):
+    """ocpmodels ``get_max_neighbors_mask``: keep the ``max_neighbors`` smallest ``d2`` of every centre; equal ``d2``
+    keep list order.  An exact lexicographic sort on (centre, d2, list position)."""
+    centre_np = centre.cpu().numpy()
+    d2_np = d2.detach().cpu().double().numpy()
+    keep = np.ones(centre_np.shape[0], dtype=bool)
+    if max_neighbors is None or centre_np.size == 0:
+        return torch.from_numpy(keep)
+    order = np.lexsort((np.arange(centre_np.size), d2_np, centre_np))
+    sorted_centre = centre_np[order]
+    first = np.searchsorted(sorted_centre, sorted_centre, side="left")
+    keep[order] = np.arange(order.size) - first < max_neighbors
+    return torch.from_numpy(keep)
+
+
+def radius_graph_pbc(pos, batch, cell, r, max_neighbors=None, budget=2 ** 25):
+    """ocpmodels ``radius_graph_pbc`` (as consumed at nets/graph_attention_transformer_oc20.py:267-302) in float64, on
+    the device of ``pos``: every (centre i, atom j, image n) of one frame with ``1e-4 < |pos_j + n . cell - pos_i|^2 <=
+    r^2``; rows of ``cell [n_frames, 3, 3]`` are the lattice vectors.
+
+    Each frame enumerates ``ceil(r / height) + 1`` images per lattice vector, one shell more than can hold a neighbour
+    of an atom inside the cell, so that a short repetition count elsewhere shows up as missing pairs.  Hits are ordered
+    by centre, then j, then image (a slowest, c fastest); with ``max_neighbors`` each centre keeps its nearest hits by
+    exact ``d2`` (``nearest_neighbours_mask``).  Centres are evaluated in chunks of about ``budget`` float64 elements.
+    Returns ``(edge_index [2, E] = (j, i), cell_offsets [E, 3] int64, d2 [E] float64)``."""
+    pos, cell = pos.detach().double(), cell.detach().to(pos.device, torch.float64)
+    r2 = float(r) ** 2
+    srcs, dsts, offs, d2s = [], [], [], []
+    for f in range(cell.shape[0]):
+        idx = (batch == f).nonzero().flatten()
+        if idx.numel() == 0:
+            continue
+        a, b, c = cell[f]
+        volume = float(torch.dot(a, torch.linalg.cross(b, c)).abs())
+        heights = [volume / float(torch.linalg.cross(u, v).norm()) for u, v in ((b, c), (c, a), (a, b))]
+        reps = [math.ceil(float(r) / h) + 1 for h in heights]
+        imgs = torch.tensor([(na, nb, nc) for na in range(-reps[0], reps[0] + 1) for nb in range(-reps[1], reps[1] + 1)
+                             for nc in range(-reps[2], reps[2] + 1)], dtype=torch.int64, device=pos.device)
+        shift = imgs.double() @ cell[f]                                                         # [n_img, 3]
+        p = pos[idx]
+        image_pos = (p[:, None, :] + shift[None, :, :]).reshape(-1, 3)                        # [(j, img), 3]
+        chunk = max(1, budget // (3 * image_pos.shape[0]))
+        for i0 in range(0, idx.numel(), chunk):
+            centres = p[i0:i0 + chunk]
+            d2 = (image_pos[None, :, :] - centres[:, None, :]).pow(2).sum(-1)                  # [i, (j, img)]
+            i, t = ((d2 > 1e-4) & (d2 <= r2)).nonzero(as_tuple=True)
+            srcs.append(idx[t // imgs.shape[0]])
+            dsts.append(idx[i0 + i])
+            offs.append(imgs[t % imgs.shape[0]])
+            d2s.append(d2[i, t])
+    if not srcs:
+        return (torch.zeros(2, 0, dtype=torch.int64, device=pos.device), torch.zeros(0, 3, dtype=torch.int64, device=pos.device),
+                torch.zeros(0, dtype=torch.float64, device=pos.device))
+    src, dst, off, d2 = torch.cat(srcs), torch.cat(dsts), torch.cat(offs), torch.cat(d2s)
+    order = torch.argsort(dst, stable=True)                                                     # frames in any order
+    src, dst, off, d2 = src[order], dst[order], off[order], d2[order]
+    keep = nearest_neighbours_mask(dst, d2, max_neighbors).to(pos.device)
+    return torch.stack([src[keep], dst[keep]]), off[keep], d2[keep]
 
 
 def model_forward_oc20(params: Params, cfg: Config, pos, cell, batch, atomic_numbers, tags, n_graphs: int, edge_src,
