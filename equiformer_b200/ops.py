@@ -2141,6 +2141,38 @@ def _sh_couplings(device):
     return _coupling_tensor(1, torch.float32, device).contiguous(), _coupling_tensor(2, torch.float32, device).contiguous()
 
 
+def edge_geom_fwd_raw(pos, graph: "Graph", lmax: int, offsets):
+    """(edge_vec [E, 3], length [E], sh [E, (lmax + 1)^2]) of ``pos[src] - pos[dst] (+ offsets)`` (``eqf_edge_geom_fwd``)."""
+    pos = _require_cuda(pos, "pos")
+    E = graph.n_edges
+    a1, a2 = _sh_couplings(pos.device)
+    vec = torch.empty((E, 3), device=pos.device, dtype=torch.float32)
+    length = torch.empty(E, device=pos.device, dtype=torch.float32)
+    sh = torch.empty((E, (lmax + 1) ** 2), device=pos.device, dtype=torch.float32)
+    with torch.cuda.device(pos.device), _kernel("edge_geom_fwd", 4 * E * (6 + 4 + (lmax + 1) ** 2)):
+        rc = _lib.load().eqf_edge_geom_fwd(pos.data_ptr(), graph.src.data_ptr(), graph.dst.data_ptr(),
+                                           offsets.data_ptr() if offsets is not None else None, a1.data_ptr(), a2.data_ptr(),
+                                           E, lmax, vec.data_ptr(), length.data_ptr(), sh.data_ptr(), _stream())
+    _lib.check(rc, "eqf_edge_geom_fwd")
+    return vec, length, sh
+
+
+def edge_geom_bwd_raw(vec, lmax: int, g_sh, g_len):
+    """``[E, 3]`` gradient of the edge vectors from the cotangents of the harmonics and of the length (either may be
+    None; ``eqf_edge_geom_bwd``)."""
+    E = vec.shape[0]
+    a1, a2 = _sh_couplings(vec.device)
+    gv = torch.empty((E, 3), device=vec.device, dtype=torch.float32)
+    gs = g_sh.contiguous() if g_sh is not None else None
+    gl = g_len.contiguous() if g_len is not None else None
+    with torch.cuda.device(vec.device), _kernel("edge_geom_bwd", 4 * E * (6 + (lmax + 1) ** 2)):
+        rc = _lib.load().eqf_edge_geom_bwd(vec.data_ptr(), a1.data_ptr(), a2.data_ptr(), E, lmax,
+                                           gs.data_ptr() if gs is not None else None,
+                                           gl.data_ptr() if gl is not None else None, gv.data_ptr(), _stream())
+    _lib.check(rc, "eqf_edge_geom_bwd")
+    return gv
+
+
 class EdgeGeometry(torch.autograd.Function):
     """(edge_vec, length, sh) of ``pos[src] - pos[dst] (+ offsets)`` in one kernel; backward = one kernel + two segment sums
     to the positions (destination-sorted CSR and its CSC).  apply(pos, graph, lmax, offsets_or_None)."""
@@ -2148,16 +2180,7 @@ class EdgeGeometry(torch.autograd.Function):
     @staticmethod
     def forward(ctx, pos, graph: "Graph", lmax: int, offsets):
         pos = _require_cuda(pos, "pos")
-        E = graph.n_edges
-        a1, a2 = _sh_couplings(pos.device)
-        vec = torch.empty((E, 3), device=pos.device, dtype=torch.float32)
-        length = torch.empty(E, device=pos.device, dtype=torch.float32)
-        sh = torch.empty((E, (lmax + 1) ** 2), device=pos.device, dtype=torch.float32)
-        with torch.cuda.device(pos.device), _kernel("edge_geom_fwd", 4 * E * (6 + 4 + (lmax + 1) ** 2)):
-            rc = _lib.load().eqf_edge_geom_fwd(pos.data_ptr(), graph.src.data_ptr(), graph.dst.data_ptr(),
-                                               offsets.data_ptr() if offsets is not None else None, a1.data_ptr(), a2.data_ptr(),
-                                               E, lmax, vec.data_ptr(), length.data_ptr(), sh.data_ptr(), _stream())
-        _lib.check(rc, "eqf_edge_geom_fwd")
+        vec, length, sh = edge_geom_fwd_raw(pos, graph, lmax, offsets)
         ctx.graph, ctx.lmax, ctx.has_off = graph, lmax, offsets is not None
         ctx.save_for_backward(pos, vec, *([offsets] if offsets is not None else []))
         return vec, length, sh
@@ -2172,15 +2195,7 @@ class EdgeGeometry(torch.autograd.Function):
             gp, go = _higher_order_grads(fn, (pos, offsets), (g_vec_out, g_len, g_sh))
             return gp, None, None, go
         E = graph.n_edges
-        a1, a2 = _sh_couplings(pos.device)
-        gv = torch.empty((E, 3), device=pos.device, dtype=torch.float32)
-        gs = g_sh.contiguous() if g_sh is not None else None
-        gl = g_len.contiguous() if g_len is not None else None
-        with torch.cuda.device(pos.device), _kernel("edge_geom_bwd", 4 * E * (6 + (lmax + 1) ** 2)):
-            rc = _lib.load().eqf_edge_geom_bwd(vec.data_ptr(), a1.data_ptr(), a2.data_ptr(), E, lmax,
-                                               gs.data_ptr() if gs is not None else None,
-                                               gl.data_ptr() if gl is not None else None, gv.data_ptr(), _stream())
-        _lib.check(rc, "eqf_edge_geom_bwd")
+        gv = edge_geom_bwd_raw(vec, lmax, g_sh, g_len)
         if g_vec_out is not None:
             gv = gv + g_vec_out
         lay = HeadLayout([1], [3], 1)
@@ -2203,18 +2218,37 @@ def expnorm_torch(dist, means, betas, alpha: float, cutoff_upper: float):
     return cut * torch.exp(-betas * (torch.exp(-alpha * d) - means) ** 2)
 
 
+def expnorm_fwd_raw(dist, means, betas, alpha: float, hi: float):
+    """``[E, B]`` exp-normal basis of the distances (``eqf_expnorm_fwd``)."""
+    dist = _require_cuda(dist, "expnorm dist")
+    E, B = dist.shape[0], means.numel()
+    out = torch.empty((E, B), device=dist.device, dtype=torch.float32)
+    with torch.cuda.device(dist.device), _kernel("expnorm_fwd", 4 * (E + E * B)):
+        rc = _lib.load().eqf_expnorm_fwd(dist.data_ptr(), means.data_ptr(), betas.data_ptr(), alpha, hi, E, B,
+                                         out.data_ptr(), _stream())
+    _lib.check(rc, "eqf_expnorm_fwd")
+    return out
+
+
+def expnorm_bwd_raw(dist, means, betas, alpha: float, hi: float, g):
+    """``[E]`` distance gradient of the exp-normal basis for the cotangent ``g`` ``[E, B]`` (``eqf_expnorm_bwd``)."""
+    E, B = g.shape
+    gd = torch.empty(E, device=g.device, dtype=torch.float32)
+    g = g.contiguous()
+    with torch.cuda.device(g.device), _kernel("expnorm_bwd", 4 * (2 * E + E * B)):
+        rc = _lib.load().eqf_expnorm_bwd(dist.data_ptr(), means.data_ptr(), betas.data_ptr(), alpha, hi, E, B,
+                                         g.data_ptr(), gd.data_ptr(), _stream())
+    _lib.check(rc, "eqf_expnorm_bwd")
+    return gd
+
+
 class ExpNormalRbf(torch.autograd.Function):
     """Exp-normal radial basis on ``[E]`` distances -> ``[E, B]`` (fixed means / betas); one kernel each way."""
 
     @staticmethod
     def forward(ctx, dist, means, betas, alpha: float, hi: float):
         dist = _require_cuda(dist, "expnorm dist")
-        E, B = dist.shape[0], means.numel()
-        out = torch.empty((E, B), device=dist.device, dtype=torch.float32)
-        with torch.cuda.device(dist.device), _kernel("expnorm_fwd", 4 * (E + E * B)):
-            rc = _lib.load().eqf_expnorm_fwd(dist.data_ptr(), means.data_ptr(), betas.data_ptr(), alpha, hi, E, B,
-                                             out.data_ptr(), _stream())
-        _lib.check(rc, "eqf_expnorm_fwd")
+        out = expnorm_fwd_raw(dist, means, betas, alpha, hi)
         ctx.alpha, ctx.hi = alpha, hi
         ctx.save_for_backward(dist, means, betas)
         return out
@@ -2226,14 +2260,7 @@ class ExpNormalRbf(torch.autograd.Function):
             fn = lambda d, m, b: expnorm_torch(d, m, b, ctx.alpha, ctx.hi)
             gd, gm, gb = _higher_order_grads(fn, (dist, means, betas), (g,))
             return gd, gm, gb, None, None
-        E, B = g.shape
-        gd = torch.empty(E, device=g.device, dtype=torch.float32)
-        g = g.contiguous()
-        with torch.cuda.device(g.device), _kernel("expnorm_bwd", 4 * (2 * E + E * B)):
-            rc = _lib.load().eqf_expnorm_bwd(dist.data_ptr(), means.data_ptr(), betas.data_ptr(), ctx.alpha, ctx.hi, E, B,
-                                             g.data_ptr(), gd.data_ptr(), _stream())
-        _lib.check(rc, "eqf_expnorm_bwd")
-        return gd, None, None, None, None
+        return expnorm_bwd_raw(dist, means, betas, ctx.alpha, ctx.hi, g), None, None, None, None
 
 
 def expnorm_rbf(dist, means, betas, alpha: float, cutoff_upper: float):

@@ -97,42 +97,38 @@ def dtp_grad_xw_raw(plan, xs, y, w, gs, gather=None, w_offset=None):
     return dtp_grad_x_raw(plan, gs, y, w), dtp_grad_w_raw(plan, xs, y, gs, w.dim() == 1)
 
 
-def seg_softmax_bwd_raw(alpha, ga, graph):
-    t = alpha * ga
-    s = torch.zeros((graph.n_nodes, alpha.shape[1]), dtype=alpha.dtype).index_add(0, graph.dst, t)
+def seg_softmax_bwd_raw(alpha, ga, graph, keep=None):
+    t = alpha * (ga if keep is None else ga * keep)
+    s = alpha.new_zeros((graph.n_nodes, alpha.shape[1])).index_add(0, graph.dst, t)
     return t - alpha * s.index_select(0, graph.dst)
 
 
-def _head_of(lay, g):
+def _head_of(lay, g, device=None):
     C = lay.Cs[g]
-    return torch.arange(C) // (C // lay.n_heads)
+    return torch.arange(C, device=device) // (C // lay.n_heads)
 
 
 def seg_softmax_raw(z, graph):
-    out = torch.empty_like(z)
-    rp = graph.row_ptr.tolist()
-    for t in range(graph.n_nodes):
-        a, b = rp[t], rp[t + 1]
-        if b > a:
-            seg = z[a:b]
-            e = (seg - seg.max(dim=0, keepdim=True).values).exp()
-            out[a:b] = e / (e.sum(dim=0, keepdim=True) + 1e-16)
-    return out
+    """Segment softmax over destination segments, vectorised (segment maxima by ``index_reduce``)."""
+    m = z.new_full((graph.n_nodes, z.shape[1]), float("-inf")).index_reduce(0, graph.dst, z, "amax")
+    e = (z - m.index_select(0, graph.dst)).exp()
+    s = z.new_zeros((graph.n_nodes, z.shape[1])).index_add(0, graph.dst, e)
+    return e / (s.index_select(0, graph.dst) + 1e-16)
 
 
 def attn_aggregate_raw(lay, alpha, Vs, graph, by_src=False):
     outs = []
     index = graph.src if by_src else graph.dst
     for g, V in enumerate(Vs):
-        val = V if alpha is None else V * alpha[:, _head_of(lay, g)][:, None, :]
+        val = V if alpha is None else V * alpha[:, _head_of(lay, g, V.device)][:, None, :]
         out = V.new_zeros((graph.n_nodes,) + tuple(V.shape[1:]))
         outs.append(out.index_add(0, index, val))
     return outs
 
 
-def softmax_aggregate_raw(lay, z, Vs, graph):
+def softmax_aggregate_raw(lay, z, Vs, graph, keep=None):
     alpha = seg_softmax_raw(z, graph)
-    return attn_aggregate_raw(lay, alpha, Vs, graph), alpha
+    return attn_aggregate_raw(lay, alpha if keep is None else alpha * keep, Vs, graph), alpha
 
 
 def attn_edge_dot_raw(lay, Vs, Gs, graph):
@@ -140,18 +136,69 @@ def attn_edge_dot_raw(lay, Vs, Gs, graph):
     out = Vs[0].new_zeros((E, lay.n_heads))
     for g, (V, G) in enumerate(zip(Vs, Gs)):
         prod = (V * G.index_select(0, graph.dst)).sum(dim=1)  # [E, C]
-        out = out.index_add(1, _head_of(lay, g), prod)
+        out = out.index_add(1, _head_of(lay, g, V.device), prod)
     return out
 
 
-def attn_edge_scale_raw(lay, alpha, Gs, graph):
+def attn_edge_scale_raw(lay, alpha, Gs, graph, keep=None):
+    if keep is not None:
+        alpha = alpha * keep
     outs = []
     for g, G in enumerate(Gs):
         val = G.index_select(0, graph.dst)
         if alpha is not None:
-            val = val * alpha[:, _head_of(lay, g)][:, None, :]
+            val = val * alpha[:, _head_of(lay, g, G.device)][:, None, :]
         outs.append(val)
     return outs
+
+
+def kv_halves(lay, kvs):
+    """Keys ``[..., :C]`` and values ``[..., C:]`` of the key / value blocks of the dot-product attention."""
+    return ([t[..., :C] for t, C in zip(kvs, lay.Cs)], [t[..., C:] for t, C in zip(kvs, lay.Cs)])
+
+
+def dot_softmax_aggregate_raw(lay, qs, kvs, graph, keep=None):
+    k, v = kv_halves(lay, kvs)
+    alpha = seg_softmax_raw(attn_edge_dot_raw(lay, k, qs, graph), graph)
+    return attn_aggregate_raw(lay, alpha if keep is None else alpha * keep, v, graph), alpha
+
+
+def dot_softmax_aggregate_bwd_raw(lay, Gs, qs, kvs, alpha, graph, keep=None):
+    """The formulas the backward kernel implements, stated on whole tensors."""
+    k, v = kv_halves(lay, kvs)
+    keep = torch.ones_like(alpha) if keep is None else keep
+    ga = attn_edge_dot_raw(lay, v, Gs, graph)
+    s = alpha.new_zeros((graph.n_nodes, lay.n_heads)).index_add(0, graph.dst, alpha * keep * ga)
+    gz = alpha * (keep * ga - s.index_select(0, graph.dst))
+    gk = attn_edge_scale_raw(lay, gz, qs, graph)
+    gv = attn_edge_scale_raw(lay, alpha * keep, Gs, graph)
+    gq = attn_aggregate_raw(lay, gz, k, graph)
+    return gq, [torch.cat([a, b], dim=2) for a, b in zip(gk, gv)]
+
+
+def mlp_softmax_aggregate_raw(lay, t0, Vs, alpha_dot, graph, keep=None):
+    alpha = seg_softmax_raw(ops.mlp_logits_torch(lay, t0, alpha_dot), graph)
+    vals = [ops.mlp_value_scalars(lay, t0), *Vs]
+    return attn_aggregate_raw(lay.head, alpha if keep is None else alpha * keep, vals, graph), alpha
+
+
+def mlp_softmax_aggregate_bwd_raw(lay, Gs, t0, Vs, alpha_dot, alpha, graph, keep=None):
+    """The formulas the backward kernel implements, stated on whole tensors."""
+    hl = lay.head
+    E, H, A, R_ = t0.shape[0], hl.n_heads, lay.n_alpha, lay.n_scalars
+    keep = torch.ones_like(alpha) if keep is None else keep
+    vals = [ops.mlp_value_scalars(lay, t0), *Vs]
+    ga = attn_edge_dot_raw(hl, vals, Gs, graph)
+    s = alpha.new_zeros((graph.n_nodes, H)).index_add(0, graph.dst, alpha * keep * ga)
+    gz = alpha * (keep * ga - s.index_select(0, graph.dst))
+    gv = attn_edge_scale_raw(hl, alpha * keep, Gs, graph)
+    a = t0.reshape(E, H, A + R_)[:, :, :A]
+    sg = torch.sigmoid(a)
+    k1, k2 = 0.5 * (1 + lay.slope), 0.5 * (1 - lay.slope)
+    act = lay.c_slr * (k1 * a + k2 * a * (2 * sg - 1))
+    dact = lay.c_slr * (k1 + k2 * ((2 * sg - 1) + 2 * a * sg * (1 - sg)))
+    gt0 = torch.cat([gz[:, :, None] * alpha_dot.reshape(1, H, A) * dact, gv[0].reshape(E, H, R_)], dim=2).reshape(E, -1)
+    return gt0, gv[1:], (gz[:, :, None] * act).sum(0).reshape(-1)
 
 
 def gemm_raw(mode, A, B):

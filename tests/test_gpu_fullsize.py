@@ -17,7 +17,7 @@ from __future__ import annotations
 import pytest
 import torch
 
-from tests.helpers import rel_err
+from tests.helpers import assert_same_grad_presence, rel_err
 
 pytestmark = pytest.mark.gpu
 
@@ -46,7 +46,7 @@ def _worst_grad_err(named_grads, ref_grads):
     worst, where = 0.0, None
     for k, g in named_grads.items():
         gref = ref_grads.get(k)
-        if g is None or gref is None:
+        if not assert_same_grad_presence(k, g, gref):
             continue
         e = ((g.double().cpu() - gref).abs().max() / gref.abs().max().clamp_min(1e-12)).item()
         if e > worst:

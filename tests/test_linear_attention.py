@@ -164,38 +164,11 @@ def test_mirror_with_emulated_kernels_matches_reference_linear_message_model_fil
 
 
 # ------------------------------------------------------------------------------------------------ host logic (float64)
-def _fwd64(lay, t0, Vs, alpha_dot, graph, keep=None):
-    from equiformer_b200 import ops
-    alpha = emu.seg_softmax_raw(ops.mlp_logits_torch(lay, t0, alpha_dot), graph)
-    vals = [ops.mlp_value_scalars(lay, t0), *Vs]
-    return emu.attn_aggregate_raw(lay.head, alpha if keep is None else alpha * keep, vals, graph), alpha
-
-
-def _bwd64(lay, Gs, t0, Vs, alpha_dot, alpha, graph, keep=None):
-    """The formulas the backward kernel implements, stated on whole tensors."""
-    from equiformer_b200 import ops
-    hl = lay.head
-    E, H, A, R_ = t0.shape[0], hl.n_heads, lay.n_alpha, lay.n_scalars
-    keep = torch.ones_like(alpha) if keep is None else keep
-    vals = [ops.mlp_value_scalars(lay, t0), *Vs]
-    ga = emu.attn_edge_dot_raw(hl, vals, Gs, graph)
-    s = torch.zeros((graph.n_nodes, H), dtype=alpha.dtype).index_add(0, graph.dst, alpha * keep * ga)
-    gz = alpha * (keep * ga - s.index_select(0, graph.dst))
-    gv = emu.attn_edge_scale_raw(hl, alpha * keep, Gs, graph)
-    a = t0.reshape(E, H, A + R_)[:, :, :A]
-    sg = torch.sigmoid(a)
-    k1, k2 = 0.5 * (1 + lay.slope), 0.5 * (1 - lay.slope)
-    act = lay.c_slr * (k1 * a + k2 * a * (2 * sg - 1))
-    dact = lay.c_slr * (k1 + k2 * ((2 * sg - 1) + 2 * a * sg * (1 - sg)))
-    gt0 = torch.cat([gz[:, :, None] * alpha_dot.reshape(1, H, A) * dact, gv[0].reshape(E, H, R_)], dim=2).reshape(E, -1)
-    return gt0, gv[1:], (gz[:, :, None] * act).sum(0).reshape(-1)
-
-
 @pytest.fixture
 def stand_ins(monkeypatch):
     from equiformer_b200 import ops
-    monkeypatch.setattr(ops, "mlp_softmax_aggregate_raw", _fwd64)
-    monkeypatch.setattr(ops, "mlp_softmax_aggregate_bwd_raw", _bwd64)
+    monkeypatch.setattr(ops, "mlp_softmax_aggregate_raw", emu.mlp_softmax_aggregate_raw)
+    monkeypatch.setattr(ops, "mlp_softmax_aggregate_bwd_raw", emu.mlp_softmax_aggregate_bwd_raw)
     with emu.emulated_kernels():
         yield ops
 

@@ -163,34 +163,14 @@ def test_mirror_with_emulated_kernels_matches_reference_dp_oc20_model_file():
 
 
 # ------------------------------------------------------------------------------------------------ host logic (float64)
-def _halves(lay, kvs):
-    return ([t[..., :C] for t, C in zip(kvs, lay.Cs)], [t[..., C:] for t, C in zip(kvs, lay.Cs)])
-
-
-def _fwd64(lay, qs, kvs, graph, keep=None):
-    k, v = _halves(lay, kvs)
-    alpha = emu.seg_softmax_raw(emu.attn_edge_dot_raw(lay, k, qs, graph), graph)
-    return emu.attn_aggregate_raw(lay, alpha if keep is None else alpha * keep, v, graph), alpha
-
-
-def _bwd64(lay, Gs, qs, kvs, alpha, graph, keep=None):
-    """The formulas the backward kernel implements, stated on whole tensors."""
-    k, v = _halves(lay, kvs)
-    keep = torch.ones_like(alpha) if keep is None else keep
-    ga = emu.attn_edge_dot_raw(lay, v, Gs, graph)
-    s = torch.zeros((graph.n_nodes, lay.n_heads), dtype=alpha.dtype).index_add(0, graph.dst, alpha * keep * ga)
-    gz = alpha * (keep * ga - s.index_select(0, graph.dst))
-    gk = emu.attn_edge_scale_raw(lay, gz, qs, graph)
-    gv = emu.attn_edge_scale_raw(lay, alpha * keep, Gs, graph)
-    gq = emu.attn_aggregate_raw(lay, gz, k, graph)
-    return gq, [torch.cat([a, b], dim=2) for a, b in zip(gk, gv)]
+_halves = emu.kv_halves
 
 
 @pytest.fixture
 def stand_ins(monkeypatch):
     from equiformer_b200 import ops
-    monkeypatch.setattr(ops, "dot_softmax_aggregate_raw", _fwd64)
-    monkeypatch.setattr(ops, "dot_softmax_aggregate_bwd_raw", _bwd64)
+    monkeypatch.setattr(ops, "dot_softmax_aggregate_raw", emu.dot_softmax_aggregate_raw)
+    monkeypatch.setattr(ops, "dot_softmax_aggregate_bwd_raw", emu.dot_softmax_aggregate_bwd_raw)
     with emu.emulated_kernels():
         yield ops
 

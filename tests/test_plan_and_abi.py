@@ -65,6 +65,21 @@ def test_generated_kernel_signatures_match_the_shipped_plans():
             assert codegen.plan_signature(plan) == sigs[tag], (name, tag)
 
 
+def _known_tags():
+    from equiformer_b200 import codegen
+    return [tag for tag, _irreps, _sh in codegen.KNOWN_CONFIGS]
+
+
+@pytest.mark.parametrize("tag", _known_tags())
+def test_committed_generated_file_is_what_the_generator_emits(tag):
+    """``build()`` regenerates ``csrc/gen`` before it compiles: a committed file that the generator no longer emits
+    byte for byte would be reviewed as one kernel and compiled as another."""
+    from equiformer_b200 import codegen
+    irreps, sh = next((i, s) for t, i, s in codegen.KNOWN_CONFIGS if t == tag)
+    committed = (codegen.GEN_DIR / f"dtp_gen_{tag}.cu").read_text()
+    assert codegen.generate(codegen.plan_for(irreps, sh), tag) == committed, tag
+
+
 def test_plan_info_and_bytes(built_lib):
     from equiformer_b200.nets.graph_attention_transformer import DepthwiseTensorProduct
     irreps = "128x0e+64x1e+32x2e"

@@ -19,7 +19,7 @@ import torch
 
 from oracle import e3nn_ref as e3
 from oracle import equiformer_ref as R
-from tests.helpers import rel_err
+from tests.helpers import assert_same_grad_presence, rel_err
 
 FIXTURE = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_modules.npz")
 LN_CASES = ["qm9_l2", "md17_l3", "oc20_l1", "ffn_mid"]
@@ -353,9 +353,9 @@ def test_cuda_small_model_gradients_through_tcgen05_gemms_match_oracle(cuda_devi
     assert rel_err(out, ref) < 1e-4
     errs = []
     for k, p in model.named_parameters():
-        if p.grad is None or params[k].grad is None:
-            continue
         gref = params[k].grad
+        if not assert_same_grad_presence(k, p.grad, gref):
+            continue
         errs.append((((p.grad.double().cpu() - gref).abs().max() / gref.abs().max().clamp_min(1e-12)).item(), k))
     errs.sort(reverse=True)
     assert errs[0][0] < 1e-3, errs[:5]
