@@ -19,7 +19,7 @@ PKG_DIR = Path(__file__).resolve().parent
 CSRC_DIR = PKG_DIR / "csrc"
 INCLUDE_DIR = PKG_DIR.parent / "include"
 LIB_PATH = PKG_DIR / "libeqf_b200.so"
-SOURCES = ("eqf_abi.cu", "eqf_dtp.cu", "eqf_dtp_vec.cu", "eqf_dtp_v3.cu", "eqf_attn.cu", "eqf_pointwise.cu", "eqf_gemm_tf32x3.cu", "eqf_graph.cu",
+SOURCES = ("eqf_abi.cu", "eqf_dtp.cu", "eqf_dtp_vec.cu", "eqf_attn.cu", "eqf_pointwise.cu", "eqf_gemm_tf32x3.cu", "eqf_graph.cu",
            "eqf_fused.cu", "eqf_edge.cu", "eqf_gemm_small.cu")
 
 EQF_COLSUM_COUNTERS = 16384

@@ -145,9 +145,8 @@ extern "C" int eqf_plan_create(const EqfPathDesc* paths, int32_t n_paths, const 
   h.n_wtasks = (int)wtasks.size() / 2;
   h.n_xtasks = (int)xtasks.size() / 2;
 
-  // tile size: largest of {8,4,2,1} edges whose scratch fits comfortably beside the tables (env override for tuning)
+  // tile size: largest of {8,4,2,1} edges whose scratch fits comfortably beside the tables
   int te = 8;
-  if (const char* env = std::getenv("EQF_TILE_EDGES")) { int v = std::atoi(env); if (v == 1 || v == 2 || v == 4 || v == 8 || v == 16) te = v; }
   const size_t fixed_words = (size_t)n_paths * (sizeof(PathDev) / 4) + cg_len + m_size + 4 * (size_t)n_paths + 64;
   auto scalar_smem = [&](int t) {
     size_t extra = (size_t)std::max(weight_numel, t * m_size);

@@ -79,12 +79,8 @@ struct GeneratedKernels {
 };
 int register_generated(const GeneratedKernels* k);
 const GeneratedKernels* find_generated(unsigned long long signature);
-int dtp_variant();                        // 0 scalar, 1 vec, 2 vec + TMA weights, 3 pipelined v3, 4 generated (env EQF_DTP_VARIANT)
 int launch_forward_vec(const EqfPlan* plan, const EdgeArgs& a, bool tma, cudaStream_t stream);
 int launch_grad_x_vec(const EqfPlan* plan, const EdgeArgs& a, bool with_w, cudaStream_t stream);
-int launch_forward_v3(const EqfPlan* plan, const EdgeArgs& a, cudaStream_t stream);
-int launch_backward_v3(const EqfPlan* plan, const EdgeArgs& a, bool with_w, cudaStream_t stream);
-int backward_v3_grid(const EqfPlan* plan, long long E);
 
 }  // namespace eqf
 

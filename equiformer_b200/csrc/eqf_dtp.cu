@@ -385,7 +385,7 @@ static int fill_args(const EqfPlan* plan, const EqfEdgeOperands* op, long long E
   a.dst = reinterpret_cast<const long long*>(op->dst);
   a.y = op->y; a.w = op->w; a.w_off = op->w_offset; a.w_shared = op->w_shared; a.gw = nullptr; a.gy = nullptr; a.E = E;
   if (E == 0) return EQF_OK;
-  if (a.w_off != nullptr && !(plan->gen != nullptr && dtp_variant() == 4)) {
+  if (a.w_off != nullptr && plan->gen == nullptr) {
     set_error("w_offset is only supported by the plan-specialised kernels");
     return EQF_ERR_UNSUPPORTED;
   }
@@ -429,10 +429,9 @@ using namespace eqf;
 
 extern "C" int eqf_plan_partial_rows(const EqfPlan* plan, int64_t n_edges) {
   if (plan == nullptr) return EQF_ERR_INVALID;
-  // upper bound over the kernel generations that may write the shared-weight partial buffer
+  // upper bound over the grids that may write the shared-weight partial buffer: the table-driven kernels (scalar and
+  // float4 share grid_for; grad_w always runs the scalar one) and, for a known plan, the generated backward
   int rows = grid_for(plan, n_edges);
-  const int b = backward_v3_grid(plan, n_edges);
-  if (b > rows) rows = b;
   if (plan->gen != nullptr) { const int c = plan->gen->partial_rows(plan, n_edges); if (c > rows) rows = c; }
   return rows;
 }
@@ -446,10 +445,9 @@ extern "C" int eqf_dtp_forward(const EqfPlan* plan, const EqfEdgeOperands* op, i
     if (out_groups == nullptr || out_groups[g] == nullptr) { set_error("null output group"); return EQF_ERR_INVALID; }
     a.out[g] = out_groups[g];
   }
-  if (plan->gen != nullptr && dtp_variant() == 4) return plan->gen->forward(plan, a, (cudaStream_t)stream);
-  if (plan->hdr.vec_ok && dtp_variant() == 3) return launch_forward_v3(plan, a, (cudaStream_t)stream);
-  if (plan->hdr.vec_ok && dtp_variant() > 0)
-    return launch_forward_vec(plan, a, dtp_variant() == 2 && !a.w_shared, (cudaStream_t)stream);
+  if (plan->gen != nullptr) return plan->gen->forward(plan, a, (cudaStream_t)stream);
+  // float4 lanes; per-edge weights stream through the TMA ring, shared weights are read in place
+  if (plan->hdr.vec_ok) return launch_forward_vec(plan, a, !a.w_shared, (cudaStream_t)stream);
   const size_t smem = plan->smem_bytes;
   if ((rc = set_smem(dtp_forward_kernel, smem)) != EQF_OK) return rc;
   dtp_forward_kernel<<<grid_for(plan, n_edges), kThreads, smem, (cudaStream_t)stream>>>(plan->hdr, plan->d_blob, a);
@@ -478,9 +476,8 @@ extern "C" int eqf_dtp_grad_x(const EqfPlan* plan, const EqfEdgeOperands* op, in
     if (gx_blocks == nullptr || gx_blocks[b] == nullptr) { set_error("null gx block"); return EQF_ERR_INVALID; }
     a.gx[b] = gx_blocks[b];
   }
-  if (plan->gen != nullptr && dtp_variant() == 4) return plan->gen->backward(plan, a, false, (cudaStream_t)stream);
-  if (plan->hdr.vec_ok && dtp_variant() == 3) return launch_backward_v3(plan, a, false, (cudaStream_t)stream);
-  if (plan->hdr.vec_ok && dtp_variant() > 0) return launch_grad_x_vec(plan, a, false, (cudaStream_t)stream);
+  if (plan->gen != nullptr) return plan->gen->backward(plan, a, false, (cudaStream_t)stream);
+  if (plan->hdr.vec_ok) return launch_grad_x_vec(plan, a, false, (cudaStream_t)stream);
   const size_t smem = plan->smem_bytes;
   if ((rc = set_smem(dtp_grad_x_kernel<false>, smem)) != EQF_OK) return rc;
   dtp_grad_x_kernel<false><<<grid_for(plan, n_edges), kThreads, smem, (cudaStream_t)stream>>>(plan->hdr, plan->d_blob, a);
@@ -498,9 +495,8 @@ extern "C" int eqf_dtp_grad_xw(const EqfPlan* plan, const EqfEdgeOperands* op, i
     a.gx[b] = gx_blocks[b];
   }
   a.gw = gw;
-  if (plan->gen != nullptr && dtp_variant() == 4) return plan->gen->backward(plan, a, true, (cudaStream_t)stream);
-  if (plan->hdr.vec_ok && dtp_variant() == 3) return launch_backward_v3(plan, a, true, (cudaStream_t)stream);
-  if (plan->hdr.vec_ok && dtp_variant() > 0) return launch_grad_x_vec(plan, a, true, (cudaStream_t)stream);
+  if (plan->gen != nullptr) return plan->gen->backward(plan, a, true, (cudaStream_t)stream);
+  if (plan->hdr.vec_ok) return launch_grad_x_vec(plan, a, true, (cudaStream_t)stream);
   const size_t smem = plan->smem_bytes;
   if ((rc = set_smem(dtp_grad_x_kernel<true>, smem)) != EQF_OK) return rc;
   dtp_grad_x_kernel<true><<<grid_for(plan, n_edges), kThreads, smem, (cudaStream_t)stream>>>(plan->hdr, plan->d_blob, a);
@@ -514,7 +510,7 @@ extern "C" int eqf_dtp_grad_y(const EqfPlan* plan, const EqfEdgeOperands* op, in
   if (rc != EQF_OK || n_edges == 0) return rc;
   if (gy == nullptr) { set_error("null gy"); return EQF_ERR_INVALID; }
   a.gy = gy;
-  if (plan->gen != nullptr && dtp_variant() == 4) return plan->gen->grad_y(plan, a, (cudaStream_t)stream);
+  if (plan->gen != nullptr) return plan->gen->grad_y(plan, a, (cudaStream_t)stream);
   const size_t smem = plan->smem_bytes;
   if ((rc = set_smem(dtp_grad_y_kernel, smem)) != EQF_OK) return rc;
   dtp_grad_y_kernel<<<grid_for(plan, n_edges), kThreads, smem, (cudaStream_t)stream>>>(plan->hdr, plan->d_blob, a);

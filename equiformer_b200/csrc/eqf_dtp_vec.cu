@@ -11,8 +11,6 @@
 //     destination-sorted edge list (fuses graph_attention_transformer.py:487 into the operand load).
 // Requires every multiplicity to be a multiple of 4 (true for all shipped configs); otherwise the scalar
 // kernels of eqf_dtp.cu are used.
-#include <cstdlib>
-
 #include <mutex>
 #include <unordered_map>
 
@@ -318,18 +316,6 @@ __global__ void __launch_bounds__(kThreads) dtp_grad_x_vec_kernel(PlanHdr h, con
 }
 
 // ---------------------------------------------------------------------------------------------- host side
-int dtp_variant() {
-  // EQF_DTP_VARIANT = scalar | vec | tma | v3 | gen (default gen: plan-specialised kernels when the plan is known,
-  // otherwise the fastest generic variant, tma); read once
-  static int v = -1;
-  if (v < 0) {
-    const char* e = std::getenv("EQF_DTP_VARIANT");
-    std::string s = e ? e : "gen";
-    v = (s == "scalar") ? 0 : (s == "vec") ? 1 : (s == "v3") ? 3 : (s == "tma") ? 2 : 4;
-  }
-  return v;
-}
-
 // forward: persistent CTAs sized to what fits per SM (each CTA pipelines several tiles through the TMA ring)
 static int vgrid_fwd(const EqfPlan* plan, long long E) {
   const long long n_tiles = (E + plan->hdr.te - 1) / plan->hdr.te;

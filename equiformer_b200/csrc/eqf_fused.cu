@@ -27,7 +27,6 @@
 #include <cuda_runtime.h>
 
 #include <cstdint>
-#include <cstdlib>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -82,8 +81,6 @@ struct FArgs {
   int d_y, W, w_shared, d3, n_paths, m_row, K, N;
   int n_tile, n_blocks;
   long long m_blocks;
-  int dbg_skip;          // measurement aid: bit 0 skips the DTP math, bit 1 the MMAs (garbage results); bit 3 (8) turns off
-                         // the suspend-time hint of the barrier waits (results unchanged)
   long long* dbg;        // optional clock64 timeline of CTA 0: dbg[role * 2048 + n] (eqf_fused_set_timeline)
   // shared-memory layout (bytes), fixed by the host: n_op operand slots (B hi | B lo | weight box) | n_raw raw A tiles |
   // 2 x (M rows + harmonics + node rows) | descriptors | barriers
@@ -125,11 +122,10 @@ struct Ring {
 
 // One k-tile (32 channels `ch0 ..` of path p) of the raw A tile: thread t of the set's 256 handles edge t / 8 (+32 ...)
 // and the four channels 4 (t % 8) of the chunk.  The coupling block of (edge, path) is read with ceil(D1 D3 / 4) 128-bit
-// shared loads from its 16-byte aligned slot and contracted densely, i outermost (v3 used D1 D3 generic scalar loads, each
-// behind a structural-zero test: 2/3 of the producer's instructions were not arithmetic); DIAG = the l2 = 0 paths, whose
-// block is m_i delta_ik.  The first pass's gathers are issued BEFORE the warp waits for its raw slot and the weight box, so
+// shared loads from its 16-byte aligned slot and contracted densely, i outermost; DIAG = the l2 = 0 paths, whose block is
+// m_i delta_ik.  The first pass's gathers are issued BEFORE the warp waits for its raw slot and the weight box, so
 // the L2 round trip overlaps the handshake.  `w_tile`: shared-memory address of the [n_e][32] weight box or 0 (shared w).
-struct KtWaits { uint64_t* raw_free; uint32_t raw_ph; uint64_t* op_full; uint32_t op_ph; bool hint; };
+struct KtWaits { uint64_t* raw_free; uint32_t raw_ph; uint64_t* op_full; uint32_t op_ph; };
 
 template <int D1, int D3, bool DIAG>
 __device__ __forceinline__ void dtp_ktile(const FArgs& a, const FPath& p, int ch0, int t, long long e0, int n_e, long long row0,
@@ -166,10 +162,10 @@ __device__ __forceinline__ void dtp_ktile(const FArgs& a, const FPath& p, int ch
     }
     if (!waited) {
       waited = true;
-      if (wt.hint) { mbar_wait_hint(wt.raw_free, wt.raw_ph); if (wt.op_full) mbar_wait_hint(wt.op_full, wt.op_ph); }
-      else { mbar_wait(wt.raw_free, wt.raw_ph); if (wt.op_full) mbar_wait(wt.op_full, wt.op_ph); }
+      mbar_wait_hint(wt.raw_free, wt.raw_ph);
+      if (wt.op_full) mbar_wait_hint(wt.op_full, wt.op_ph);
     }
-    if (!active || (a.dbg_skip & 1)) break;
+    if (!active) break;
     float4 wv = w_tile != 0 ? lds128(w_tile + (uint32_t)el * 128u + (uint32_t)c8 * 16u) : ld4(a.w + p.w_off + ch);
     addv(wv, woff);
     float m[NM * 4];
@@ -251,8 +247,6 @@ dtp_gemm_fwd_kernel(const __grid_constant__ CUtensorMap map_bhi, const __grid_co
   constexpr int d3 = D3;        // compile-time output degree: one kernel per degree
   const long long n_tiles_total = a.m_blocks * a.n_blocks;
   const bool w_tma = !a.w_shared;
-  const bool hint = (a.dbg_skip & 8) == 0;         // try_wait with the long suspend-time hint (bit 3 turns it off: A/B)
-  auto wait = [hint](uint64_t* bar, uint32_t parity) { if (hint) mbar_wait_hint(bar, parity); else mbar_wait(bar, parity); };
 
   if (threadIdx.x == kProducerWarp * 32) {
     prefetch_map(&map_bhi); prefetch_map(&map_blo);
@@ -285,8 +279,8 @@ dtp_gemm_fwd_kernel(const __grid_constant__ CUtensorMap map_bhi, const __grid_co
 #pragma unroll
       for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
       for (int kt = 0; kt < k_tiles; ++kt, op.next(), raw.next()) {
-        wait(&op_full[op.idx], op.ph);
-        wait(&raw_ready[raw.idx], raw.ph);
+        mbar_wait_hint(&op_full[op.idx], op.ph);
+        mbar_wait_hint(&raw_ready[raw.idx], raw.ph);
         if (stamper) stamp(a, 1, n_stamp);
         // the k-tile in two halves of two 8-deep k-steps: the accumulator and one half's split fragments fit the
         // 72-register launch budget of the 896-thread CTA, so ptxas keeps the MMAs of a half asynchronous
@@ -300,10 +294,8 @@ dtp_gemm_fwd_kernel(const __grid_constant__ CUtensorMap map_bhi, const __grid_co
             __syncwarp();
             if (lane == 0) mbar_arrive(&raw_free[raw.idx]);
           }
-          if (!(a.dbg_skip & 2)) {
-            mma_ktile_3xtf32<BN>(acc, hi, lo, st, st + S::kBBytes, 2 * half);
-            wgmma_wait<0>();
-          }
+          mma_ktile_3xtf32<BN>(acc, hi, lo, st, st + S::kBBytes, 2 * half);
+          wgmma_wait<0>();
         }
         __syncwarp();
         if (lane == 0) mbar_arrive(&op_empty[op.idx]);
@@ -325,7 +317,7 @@ dtp_gemm_fwd_kernel(const __grid_constant__ CUtensorMap map_bhi, const __grid_co
           const int nb = (int)(tile % a.n_blocks);
           const int e0 = (int)((mb * BM) / d3);
           for (int kt = 0; kt < k_tiles; ++kt, op.next()) {
-            wait(&op_empty[op.idx], op.ph ^ 1);
+            mbar_wait_hint(&op_empty[op.idx], op.ph ^ 1);
             stamp(a, 0, n_stamp);
             uint8_t* st = op_base + (size_t)op.idx * a.op_bytes;
             mbar_expect_tx(&op_full[op.idx], tx);
@@ -342,8 +334,7 @@ dtp_gemm_fwd_kernel(const __grid_constant__ CUtensorMap map_bhi, const __grid_co
       // ------------------------------------------------------------------------------------- table helpers (warps 6, 7)
       // One row block AHEAD of the DTP warps: the block's edges (src / dst rows, harmonics) into shared memory, then the
       // coupling blocks M_p[e] = CG_p . y_e, one thread per entry q of the edge's M row (its CG column in registers)
-      // walking the block's edges.  (v3 did this inside the DTP warps between two 512-thread barriers: ~7 k cycles per row
-      // block during which the whole pipeline drained - 23 % of the kernel.)
+      // walking the block's edges.
       const int ht = threadIdx.x - kHelperWarp0 * 32;          // 0 .. 63
       const int m_row = a.m_row, d_y = a.d_y;
       {
@@ -377,7 +368,7 @@ dtp_gemm_fwd_kernel(const __grid_constant__ CUtensorMap map_bhi, const __grid_co
         if (e1 > a.E) e1 = a.E;
         const int n_e = (int)(e1 - e0);
         const int b = tile_it & 1;
-        wait(&tab_free[b], ((tile_it >> 1) & 1) ^ 1);
+        mbar_wait_hint(&tab_free[b], ((tile_it >> 1) & 1) ^ 1);
         if (ht == 0) stamp(a, 5, n_stamp);
         float* mw = reinterpret_cast<float*>(tab_base + b * a.tab_bytes);
         float* ybuf = mw + a.m_buf_floats;
@@ -429,7 +420,7 @@ dtp_gemm_fwd_kernel(const __grid_constant__ CUtensorMap map_bhi, const __grid_co
       if (e1 > a.E) e1 = a.E;
       const int n_e = (int)(e1 - e0);
       const int b = tile_it & 1;
-      wait(&tab_ready[b], (tile_it >> 1) & 1);            // the helper warps built this row block's tables
+      mbar_wait_hint(&tab_ready[b], (tile_it >> 1) & 1);            // the helper warps built this row block's tables
       if (stamper) stamp(a, 4, n_stamp);
       const float* mw = reinterpret_cast<const float*>(tab_base + b * a.tab_bytes);
       const float* ybuf = mw + a.m_buf_floats;
@@ -444,7 +435,7 @@ dtp_gemm_fwd_kernel(const __grid_constant__ CUtensorMap map_bhi, const __grid_co
         const uint32_t w_tile = w_tma ? smem_u32(op_base + (size_t)op.idx * a.op_bytes) + (uint32_t)a.w_tile_off : 0u;
         KtWaits wt;
         wt.raw_free = &raw_free[raw.idx]; wt.raw_ph = raw.ph ^ 1;
-        wt.op_full = w_tma ? &op_full[op.idx] : nullptr; wt.op_ph = op.ph; wt.hint = hint;
+        wt.op_full = w_tma ? &op_full[op.idx] : nullptr; wt.op_ph = op.ph;
         if (stamper) stamp(a, 4, n_stamp);
         dtp_ktile_d1<D3>(a, p, ch0, t, e0, n_e, row0, src_s, dst_s, m_addr, raw_addr, w_tile, wt);
         __syncwarp();
@@ -694,7 +685,6 @@ static int fill_fargs(const EqfPlan* plan, const EqfEdgeOperands* op, int64_t n_
   if (a.M > 0x7fffffffLL) { set_error(std::string(who) + ": too many rows"); return EQF_ERR_UNSUPPORTED; }
   a.n_tile = a.n_blocks = 0; a.m_blocks = 0;
   a.n_op = a.n_raw = a.op_bytes = a.w_tile_off = a.w_box_rows = a.tab_bytes = a.m_buf_floats = a.y_buf_floats = a.cg_floats = 0;
-  { const char* e = std::getenv("EQF_FUSED_DBG_SKIP"); a.dbg_skip = e ? std::atoi(e) : 0; }
   a.dbg = g_fused_dbg;
   return EQF_OK;
 }

@@ -1,4 +1,4 @@
-// eqf_gemm_small.cu - grouped fp32 GEMM for the SMALL products of the path (sm_90a, CUDA cores, exact fp32 FMA).
+// eqf_gemm_small.cu - grouped fp32 GEMM for the SMALL products of the path (sm_90a, warp-level MMA, 3xTF32).
 //
 // Node-level linears (nets/graph_attention_transformer.py:430-431 merge_src / merge_dst, :515 proj, the FeedForwardNetwork's
 // two FCTPs, nets/tensor_product_rescale.py LinearRS) are one [atoms * (2l+1), mul_in] x [mul_in, mul_out] product per degree:
@@ -11,12 +11,14 @@
 //     data gradient  g[M, N'] W[K', N']^T       A k-contiguous, B k-contiguous
 //     weight grad.   x[R, K']^T g[R, N]         A m-contiguous, B n-contiguous, the long reduction over R split across CTAs
 //                                               (fp32 atomic adds into a zeroed output, like the reference's scatter)
-// 64 x 64 output tile per CTA, 256 threads x (4 x 4) accumulators, 16-deep k-chunks double-buffered in shared memory,
-// 128-bit global loads along the contiguous dimension.
+// 64 x 64 output tile per CTA on the tensor cores' warp-level path (mma.sync m16n8k8, tf32 inputs, fp32 accumulate) with
+// the 3xTF32 split done in registers: a = a_hi + a_lo, b = b_hi + b_lo, acc += a_lo b_hi + a_hi b_lo + a_hi b_hi (the
+// error of the dropped a_lo b_lo term is ~2^-22 relative, like the wgmma kernels of eqf_gemm_tf32x3.cu).  A k-step of 8
+// costs a warp 24 MMAs + 16 shared loads + 48 split instructions for its 32 x 32 sub-tile; 16-deep k-chunks arrive through
+// a four-stage cp.async ring, 128-bit along the contiguous dimension.
 #include <cuda_runtime.h>
 
 #include <cstdint>
-#include <cstdlib>
 #include <string>
 
 #include "eqf_common.cuh"
@@ -24,7 +26,7 @@
 namespace eqf {
 namespace small {
 
-constexpr int BM = 64, BN = 64, BK = 16, kThreadsG = 256, kPad = 4;
+constexpr int BM = 64, BN = 64, BK = 16;
 
 struct Prob {
   const float* A;
@@ -43,120 +45,6 @@ struct Args {
   Prob p[EQF_GROUP_MAX];
 };
 
-template <bool AKC, bool BKC>
-__device__ __forceinline__ void load_tiles(const Prob& p, int m0, int n0, int k0, int k_end, float4& ra, float4& rb) {
-  const int t = threadIdx.x;
-  ra = make_float4(0.f, 0.f, 0.f, 0.f);
-  rb = make_float4(0.f, 0.f, 0.f, 0.f);
-  if constexpr (AKC) {           // A[m * lda + k]: thread = (row t / 4, k-quad t % 4)
-    const int m = m0 + (t >> 2), k = k0 + (t & 3) * 4;
-    if (m < p.M && k < k_end) ra = __ldg(reinterpret_cast<const float4*>(p.A + (size_t)m * p.lda + k));
-  } else {                       // A[k * lda + m]: thread = (k t / 16, m-quad t % 16)
-    const int k = k0 + (t >> 4), m = m0 + (t & 15) * 4;
-    if (k < k_end && m < p.M) ra = __ldg(reinterpret_cast<const float4*>(p.A + (size_t)k * p.lda + m));
-  }
-  if constexpr (BKC) {           // B[n * ldb + k]
-    const int n = n0 + (t >> 2), k = k0 + (t & 3) * 4;
-    if (n < p.N && k < k_end) rb = __ldg(reinterpret_cast<const float4*>(p.B + (size_t)n * p.ldb + k));
-  } else {                       // B[k * ldb + n]
-    const int k = k0 + (t >> 4), n = n0 + (t & 15) * 4;
-    if (k < k_end && n < p.N) rb = __ldg(reinterpret_cast<const float4*>(p.B + (size_t)k * p.ldb + n));
-  }
-}
-
-template <bool AKC, bool BKC>
-__device__ __forceinline__ void store_tiles(float (*As)[BM + kPad], float (*Bs)[BN + kPad], const float4& ra, const float4& rb) {
-  const int t = threadIdx.x;
-  if constexpr (AKC) {
-    const int m = t >> 2, k = (t & 3) * 4;
-    As[k][m] = ra.x; As[k + 1][m] = ra.y; As[k + 2][m] = ra.z; As[k + 3][m] = ra.w;
-  } else {
-    *reinterpret_cast<float4*>(&As[t >> 4][(t & 15) * 4]) = ra;
-  }
-  if constexpr (BKC) {
-    const int n = t >> 2, k = (t & 3) * 4;
-    Bs[k][n] = rb.x; Bs[k + 1][n] = rb.y; Bs[k + 2][n] = rb.z; Bs[k + 3][n] = rb.w;
-  } else {
-    *reinterpret_cast<float4*>(&Bs[t >> 4][(t & 15) * 4]) = rb;
-  }
-}
-
-template <bool AKC, bool BKC>
-__device__ __forceinline__ void tile(const Prob& p, int tm, int tn, int split, float (*As)[BK][BM + kPad], float (*Bs)[BK][BN + kPad]) {
-  const int m0 = tm * BM, n0 = tn * BN;
-  const int k_begin = split * p.k_per_split;
-  const int k_end = (k_begin + p.k_per_split) < p.K ? (k_begin + p.k_per_split) : p.K;
-  const int t = threadIdx.x, ty = t >> 4, tx = t & 15;      // rows 4 ty .., columns 4 tx ..
-  float acc[4][4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
-  float4 ra, rb;
-  load_tiles<AKC, BKC>(p, m0, n0, k_begin, k_end, ra, rb);
-  store_tiles<AKC, BKC>(As[0], Bs[0], ra, rb);
-  __syncthreads();
-  int buf = 0;
-  for (int k0 = k_begin; k0 < k_end; k0 += BK) {
-    const bool more = (k0 + BK) < k_end;
-    if (more) load_tiles<AKC, BKC>(p, m0, n0, k0 + BK, k_end, ra, rb);
-#pragma unroll
-    for (int k = 0; k < BK; ++k) {
-      const float4 a = *reinterpret_cast<const float4*>(&As[buf][k][ty * 4]);
-      const float4 b = *reinterpret_cast<const float4*>(&Bs[buf][k][tx * 4]);
-      const float av[4] = {a.x, a.y, a.z, a.w}, bv[4] = {b.x, b.y, b.z, b.w};
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(av[i], bv[j], acc[i][j]);
-    }
-    if (more) {
-      store_tiles<AKC, BKC>(As[buf ^ 1], Bs[buf ^ 1], ra, rb);
-      __syncthreads();
-      buf ^= 1;
-    }
-  }
-  const int n = n0 + tx * 4;
-  if (n >= p.N) return;
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int m = m0 + ty * 4 + i;
-    if (m >= p.M) break;
-    float* c = p.C + (size_t)m * p.ldc + n;
-    if (!p.atomic) {
-      *reinterpret_cast<float4*>(c) = make_float4(p.alpha * acc[i][0], p.alpha * acc[i][1], p.alpha * acc[i][2], p.alpha * acc[i][3]);
-    } else {
-#pragma unroll
-      for (int j = 0; j < 4; ++j) atomicAdd(c + j, p.alpha * acc[i][j]);
-    }
-  }
-}
-
-__global__ void __launch_bounds__(kThreadsG) grouped_gemm_kernel(const __grid_constant__ Args g) {
-  __shared__ __align__(16) float As[2][BK][BM + kPad];
-  __shared__ __align__(16) float Bs[2][BK][BN + kPad];
-  int pi = 0;
-  for (int i = 1; i < g.n; ++i) if ((int)blockIdx.x >= g.p[i].tile0) pi = i;
-  const Prob& p = g.p[pi];
-  int local = (int)blockIdx.x - p.tile0;
-  const int tn = local % p.tiles_n; local /= p.tiles_n;
-  const int tm = local % p.tiles_m;
-  const int split = local / p.tiles_m;
-  if (p.a_kc) {
-    if (p.b_kc) tile<true, true>(p, tm, tn, split, As, Bs);
-    else tile<true, false>(p, tm, tn, split, As, Bs);
-  } else {
-    if (p.b_kc) tile<false, true>(p, tm, tn, split, As, Bs);
-    else tile<false, false>(p, tm, tn, split, As, Bs);
-  }
-}
-
-// ---------------------------------------------------------------------------------------------- warp-MMA variant
-// The same tiles on the tensor cores' warp-level path (mma.sync m16n8k8, tf32 inputs, fp32 accumulate) with the 3xTF32
-// split done in registers: a = a_hi + a_lo, b = b_hi + b_lo, acc += a_lo b_hi + a_hi b_lo + a_hi b_hi (the error of the
-// dropped a_lo b_lo term is ~2^-22 relative, like the wgmma kernels of eqf_gemm_tf32x3.cu).  The CUDA-core kernel
-// above is bound by FMA issue (a 64 x 64 x 128 tile is 16 k warp-FMAs); here a k-step of 8 costs a
-// warp 24 MMAs + 16 shared loads + 48 split instructions for its 32 x 32 sub-tile instead of 256 FMAs + 32 loads.
 // 128 threads = 4 warps (2 x 2) per 64 x 64 tile; operands in shared memory in whichever orientation makes the global
 // load a 128-bit access AND the fragment loads conflict-free: k-contiguous operands as [row][16 + 4], the others as
 // [k][64 + 8].
@@ -315,7 +203,7 @@ using namespace eqf;
 
 // n (<= EQF_GROUP_MAX) independent products in one launch.  Problem i:  C[M, N] = alpha * op(A) op(B)  with
 //   mode 0: A[M, K] (lda) x B[K, N] (ldb);   mode 1: A[M, K] x B[N, K]^T;   mode 2: A[K, M]^T x B[K, N]   (gemm_raw's modes)
-// fp32 FMA accumulation.  `accumulate` != 0: the reduction is split across CTAs and ADDED into C with fp32 atomics (C must
+// 3xTF32 products, fp32 accumulation.  `accumulate` != 0: the reduction is split across CTAs and ADDED into C with fp32 atomics (C must
 // hold the initial value, normally zero; used for the long reductions of the weight gradients); 0: C is overwritten.
 // Pointers 16-byte aligned, leading dimensions and the extent of every contiguous dimension multiples of 4.
 extern "C" int eqf_gemm_grouped(const EqfGemmProblem* problems, int32_t n, void* stream) {
@@ -367,9 +255,6 @@ extern "C" int eqf_gemm_grouped(const EqfGemmProblem* problems, int32_t n, void*
     ++g.n;
   }
   if (g.n == 0) return EQF_OK;
-  // EQF_SMALL_MMA=0: the CUDA-core (exact fp32 FMA) kernel instead of the warp-MMA 3xTF32 one
-  static const bool use_mma = [] { const char* e = std::getenv("EQF_SMALL_MMA"); return e == nullptr || e[0] != '0'; }();
-  if (use_mma) small::grouped_gemm_mma_kernel<<<tiles, kThreadsM, 0, (cudaStream_t)stream>>>(g);
-  else small::grouped_gemm_kernel<<<tiles, kThreadsG, 0, (cudaStream_t)stream>>>(g);
-  return check_cuda(cudaGetLastError(), "grouped_gemm_kernel launch");
+  small::grouped_gemm_mma_kernel<<<tiles, kThreadsM, 0, (cudaStream_t)stream>>>(g);
+  return check_cuda(cudaGetLastError(), "grouped_gemm_mma_kernel launch");
 }

@@ -32,14 +32,7 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t done;
-  do {
-    asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                 : "=r"(done) : "r"(smem_u32(bar)), "r"(parity) : "memory");
-  } while (!done);
-}
-// the same wait with a suspend-time hint (ticks): the warp sleeps in hardware until the phase completes or the limit
+// phase wait with a suspend-time hint (ticks): the warp sleeps in hardware until the phase completes or the limit
 // expires, instead of returning after the short default limit and being re-issued
 __device__ __forceinline__ void mbar_wait_hint(uint64_t* bar, uint32_t parity) {
   asm volatile(

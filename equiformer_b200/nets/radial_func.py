@@ -6,13 +6,9 @@
 from __future__ import annotations
 
 import math
-import os
 
 import torch
 from torch import nn
-
-# EQF_RAD_HOIST=0: every radial MLP runs its own first Linear (A/B switch)
-_HOIST = os.environ.get("EQF_RAD_HOIST", "1") != "0"
 
 
 def hoist_first_layers(modules, x: torch.Tensor):
@@ -25,7 +21,7 @@ def hoist_first_layers(modules, x: torch.Tensor):
     ``forward`` (same parameters, same ``state_dict``).  Returns the modules it served.  The QM9 and OC20 steps gain from
     it; the MD17 energy + force step (2 100 edges, second-order graph) got slower, so the MD17 / DeNS models do not hoist."""
     from .. import ops
-    if not _HOIST or not ops.fused_ok(x) or x.dim() != 2:
+    if not ops.fused_ok(x) or x.dim() != 2:
         return []
     mods = []
     for m in modules:

@@ -243,7 +243,7 @@ def dtp_grad_x_raw(plan: DtpPlan, gs, y, w) -> List[torch.Tensor]:
 
 def _gw_buffer(plan: DtpPlan, E: int, shared: bool, device) -> torch.Tensor:
     if shared:
-        # upper bound on the CTAs of whichever kernel generation runs; rows a launch does not write must read as zero
+        # upper bound on the CTAs of whichever kernel runs; rows a launch does not write must read as zero
         rows = _lib.load().eqf_plan_partial_rows(plan.handle, E)
         return torch.zeros((max(rows, 1), plan.weight_numel), device=device, dtype=torch.float32)
     return torch.empty((E, plan.weight_numel), device=device, dtype=torch.float32)
@@ -560,13 +560,13 @@ def depthwise_tensor_product_gathered(plan: DtpPlan, graph: "Graph", As, Bs, y, 
 
 # ----------------------------------------------------------------------------- K1: DTP fused into the per-degree linear
 
-# EQF_FUSED: "1" fused forward everywhere, "0" the round-1 pipeline (DTP -> [E, 3136] in HBM -> GEMMs), "auto" (default) by
-# size.  The fused forward keeps the [E, 3136] products out of HBM and out of the saved activations - what lets large
+# _FUSED_MODE: "1" fused forward everywhere, "0" the unfused pipeline (DTP -> [E, 3136] in HBM -> GEMMs), "auto" by size.
+# The fused forward keeps the [E, 3136] products out of HBM and out of the saved activations - what lets large
 # periodic cells (E ~ 5e5) train at all - but its producer warps are latency bound (gathers + per-k-tile handshakes), so
 # below _FUSED_MIN_EDGES the unfused pipeline is kept.
-_FUSED_MODE = os.environ.get("EQF_FUSED", "auto")
-_FUSED = _FUSED_MODE != "0"
-_FUSED_MIN_EDGES = int(os.environ.get("EQF_FUSED_MIN_EDGES", "200000"))
+_FUSED_MODE = "auto"
+_FUSED = True
+_FUSED_MIN_EDGES = 200000
 _FUSED_SPLIT = {}
 
 
@@ -621,7 +621,7 @@ def dtp_linear_fwd_raw(plan: DtpPlan, group: int, xs, y, w, Wt: torch.Tensor, ga
 # registers), and a wider linear would recompute the product once per tile, so its group is written to HBM once
 # (eqf_dtp_group_forward) and read by the wgmma GEMM.  On the stress workload (H100) fusing the 128-column linears as
 # well measured about 1 % slower per step.
-_FUSED_MAX_N = int(os.environ.get("EQF_FUSED_MAX_N", "64"))
+_FUSED_MAX_N = 64
 
 
 def dtp_group_forward_raw(plan: DtpPlan, group: int, xs, y, w, gather=None, w_offset=None) -> torch.Tensor:
@@ -1371,26 +1371,10 @@ def segment_softmax(z: torch.Tensor, graph: Graph) -> torch.Tensor:
 
 # ----------------------------------------------------------------------------- fp32-accurate tensor-core GEMM
 
-_GEMM_MODE = None
-
-
 def gemm_backend() -> str:
-    """Which kernel carries the fp32-accurate edge-level products:
-
-    * ``'tf32x3'`` (default) - the hand-written wgmma 3xTF32 kernels of ``libeqf_b200.so`` (``eqf_gemm_tf32x3*``);
-    * ``'torch'`` - cuBLAS SGEMM everywhere (``EQF_GEMM=torch``)."""
-    global _GEMM_MODE
-    if _GEMM_MODE is None:
-        want = os.environ.get("EQF_GEMM", "tf32x3")
-        if want not in ("tf32x3", "torch"):
-            raise ValueError(f"EQF_GEMM={want!r}: expected 'tf32x3' or 'torch'")
-        _GEMM_MODE = want
-    return _GEMM_MODE
-
-
-def gemm_backend_forced() -> bool:
-    """EQF_GEMM_FORCE=1: every aligned product goes to the hand-written 3xTF32 kernels, whatever its size (tests)."""
-    return os.environ.get("EQF_GEMM_FORCE", "0") == "1"
+    """The kernels that carry the fp32-accurate edge-level products: the hand-written wgmma 3xTF32 kernels of
+    ``libeqf_b200.so`` (``eqf_gemm_tf32x3*``)."""
+    return "tf32x3"     # bench.py prints it in its result line
 
 
 def _gemm_operand(t: torch.Tensor):
@@ -1404,19 +1388,17 @@ def _gemm_operand(t: torch.Tensor):
 
 # reduction length from which the weight gradient runs as the sliced 3xTF32 launch (node-level products of 2 324 atoms x
 # (2l+1) rows included)
-_WGRAD_MIN_K = int(os.environ.get("EQF_WGRAD_MIN_K", "2048"))
-# rows from which forward / data-gradient products leave the small-product kernel for the 3xTF32 kernels; EQF_GEMM_MIN_M=1 sends the small
-# reference-run fixtures (tests/golden/reference_model_*.npz) through the hand-written kernels as well
-_GEMM_MIN_M = int(os.environ.get("EQF_GEMM_MIN_M", "16384"))
-# ... or this many flops (EQF_GEMM_MIN_FLOP; off by default): the 3xTF32 route costs a weight-split + GEMM launch pair
-# per degree where the grouped small-product kernel takes all degrees - and, in the backward, data and weight gradients -
-# in one launch.
-_GEMM_MIN_FLOP = float(os.environ.get("EQF_GEMM_MIN_FLOP", "inf"))
+_WGRAD_MIN_K = 2048
+# rows from which forward / data-gradient products leave the small-product kernel for the 3xTF32 kernels: that route costs
+# a weight-split + GEMM launch pair per degree where the grouped small-product kernel takes all degrees - and, in the
+# backward, data and weight gradients - in one launch.  smoke() and the reference-run parity tests set both thresholds to 1,
+# which sends their small fixtures through the wgmma kernels as well
+_GEMM_MIN_M = 16384
 
 
 def _use_tensor_cores(M: int, N: int, K: int) -> bool:
     """Forward / data-gradient product [M, K] x [K, N]: the wgmma 3xTF32 kernels (True) or the small-product kernel."""
-    return M >= _GEMM_MIN_M or (M >= 1024 and 2.0 * M * N * K >= _GEMM_MIN_FLOP)
+    return M >= _GEMM_MIN_M
 
 
 def gemm_raw(mode: int, A: torch.Tensor, B: torch.Tensor) -> torch.Tensor:
@@ -1433,22 +1415,19 @@ def gemm_raw(mode: int, A: torch.Tensor, B: torch.Tensor) -> torch.Tensor:
     if not ok:
         raise ValueError(f"gemm mode {mode}: incompatible shapes {tuple(A.shape)} {tuple(B.shape)}")
     aligned = all(v % 4 == 0 for v in (A.shape[1], B.shape[1], N)) and min(M, N, K) > 0
-    fast = A.is_cuda and A.dtype == torch.float32 and aligned
-    backend = gemm_backend() if fast else "torch"
-    forced = fast and gemm_backend_forced()
-    # policy: the tensor-core kernels take the tall edge-level products (forward / data gradient from _GEMM_MIN_M rows,
-    # weight gradient from _WGRAD_MIN_K reduction rows); below that the exact-fp32 small-product kernel
-    if backend == "tf32x3":
-        if mode != 2 and (forced or _use_tensor_cores(M, N, K)):
+    if A.is_cuda and A.dtype == torch.float32 and aligned:
+        # policy: the wgmma kernels take the tall edge-level products (forward / data gradient from _GEMM_MIN_M rows,
+        # weight gradient from _WGRAD_MIN_K reduction rows); below that (the whole MD17 regime, node-level leftovers) the
+        # warp-MMA 3xTF32 small-product kernel
+        if mode != 2 and _use_tensor_cores(M, N, K):
             return gemm_tf32x3_raw(A, B, b_is_kn=(mode == 0))
-        if mode == 2 and (forced or K >= _WGRAD_MIN_K):
+        if mode == 2 and K >= _WGRAD_MIN_K:
             return gemm_tf32x3_wgrad_raw(A, B)
-    if fast and backend != "torch" and _SMALL_OWN:
-        # small products (the whole MD17 regime, node-level leftovers): the exact-fp32 CUDA-core kernel, not cuBLAS
         split = mode == 2 and K >= 1024 and not _DETERMINISTIC   # long reduction, small output: split across CTAs, atomic adds
         C = (torch.zeros if split else torch.empty)((M, N), device=A.device, dtype=torch.float32)
         grouped_gemm_raw([(mode, A, B, C, 1.0, split)])
         return C
+    # operands that are not CUDA fp32 or not 4-aligned
     if mode == 0:
         return A @ B
     return A @ B.t() if mode == 1 else A.t() @ B
@@ -1570,12 +1549,9 @@ def linear_f32(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tenso
 
 
 # ----------------------------------------------------------------------------- grouped small products
-# All degrees of a node-level linear in one launch of the exact-fp32 CUDA-core kernel (csrc/eqf_gemm_small.cu): forward,
-# data gradients and weight gradients (the two gradient sets share a launch in a first-order backward).  Round 1 sent each
-# of these 30-80 MFLOP products to cuBLAS separately (~180 SIMT SGEMM launches per QM9 step).
-_GROUPED = os.environ.get("EQF_GROUPED_GEMM", "1") != "0"
-# EQF_SMALL_GEMM=cublas hands single small products (below the tensor-core thresholds) back to torch / cuBLAS (A/B switch)
-_SMALL_OWN = os.environ.get("EQF_SMALL_GEMM", "own") != "cublas"
+# All degrees of a node-level linear in one launch of the warp-MMA 3xTF32 kernel (csrc/eqf_gemm_small.cu): forward, data
+# gradients and weight gradients (the two gradient sets share a launch in a first-order backward), instead of ~180 separate
+# 30-80 MFLOP launches per QM9 step.
 
 
 class LinearSpec:
@@ -1735,8 +1711,8 @@ def planar_linear_grouped_ok(spec: LinearSpec, w: torch.Tensor, xs) -> bool:
     """All paths in one launch of the small-product kernel: CUDA fp32, aligned channels, every product below the row count
     from which the tensor-core kernels take over.  ``EQF_DETERMINISTIC=1`` keeps the per-degree route (the grouped weight
     gradients meet in ``gw`` through fp32 atomics, whose order is not fixed)."""
-    if not (_GROUPED and not _DETERMINISTIC and w.is_cuda and w.dtype == torch.float32 and w.dim() == 1 and w.is_contiguous()
-            and w.data_ptr() % 16 == 0 and spec.aligned() and gemm_backend() != "torch"):
+    if not (not _DETERMINISTIC and w.is_cuda and w.dtype == torch.float32 and w.dim() == 1 and w.is_contiguous()
+            and w.data_ptr() % 16 == 0 and spec.aligned()):
         return False
     return all(x.is_cuda and x.dtype == torch.float32 and x.dim() == 3 and x.shape[2] == p[3]
                and not _use_tensor_cores(x.shape[0] * x.shape[1], max(p[3], p[4]), min(p[3], p[4])) for p, x in zip(spec.paths, xs))

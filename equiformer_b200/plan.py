@@ -145,8 +145,7 @@ class DtpPlan:
         """True when the plan-specialised kernels (codegen.py) will run for this plan."""
         g = getattr(self, "_generated", None)
         if g is None:
-            import os
-            g = bool(self.info()["generated"]) and os.environ.get("EQF_DTP_VARIANT", "gen") not in ("scalar", "vec", "v3", "tma")
+            g = bool(self.info()["generated"])
             self._generated = g
         return g
 

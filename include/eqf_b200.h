@@ -309,7 +309,7 @@ int eqf_colsum(const float* x, int64_t rows, int64_t cols, int64_t ld, float* ou
 /* Grouped fp32 GEMM for the SMALL products of the path: all degrees of a node-level linear (reference
  * nets/tensor_product_rescale.py:LinearRS -> e3nn 'uvw' with a scalar second operand = one [rows * (2l+1), mul_in] x
  * [mul_in, mul_out] product per degree; nets/graph_attention_transformer.py:430-431, :515, FeedForwardNetwork) - forward,
- * data gradients and weight gradients - in ONE launch of exact-fp32 CUDA-core tiles (replaces the per-degree cuBLAS calls).
+ * data gradients and weight gradients - in ONE launch of warp-MMA 3xTF32 tiles (replaces the per-degree cuBLAS calls).
  * Problem i: C[M, N] = alpha * op(A) op(B); mode 0: A[M, K] B[K, N], 1: A[M, K] B[N, K]^T, 2: A[K, M]^T B[K, N];
  * accumulate != 0: the reduction is split across CTAs and ADDED into C with fp32 atomics (C holds the initial value).
  * 16-byte aligned pointers; leading dimensions and every contiguous extent multiples of 4. */

@@ -178,7 +178,9 @@ def test_unsorted_edges_are_sorted_once(cuda_device):
 def test_fast_fp32_gemm_all_layouts(cuda_device, M, N, K, monkeypatch):
     """Fast-fp32 GEMM entry point (gemm_raw) vs fp64 matmul: forward, data-grad and weight-grad layouts."""
     from equiformer_b200 import ops
-    monkeypatch.setenv("EQF_GEMM_FORCE", "1")   # exercise the 3xTF32 kernels for every layout / size, not just the policy's picks
+    # exercise the 3xTF32 kernels for every layout / size, not just the policy's picks
+    monkeypatch.setattr(ops, "_GEMM_MIN_M", 1)
+    monkeypatch.setattr(ops, "_WGRAD_MIN_K", 1)
     g = torch.Generator().manual_seed(M + N + K)
     A = torch.randn(M, K, generator=g)
     B = torch.randn(K, N, generator=g)
@@ -754,7 +756,7 @@ def test_planar_linear_grouped_matches_per_path_products(cuda_device, monkeypatc
     cots = [torch.randn(R, 2 * l + 1, m, generator=g).to(cuda_device) for l, m in ((0, 64), (1, 64), (2, 16))]
 
     def run(grouped):
-        monkeypatch.setattr(ops, "_GROUPED", grouped)
+        monkeypatch.setattr(ops, "_DETERMINISTIC", not grouped)      # the deterministic mode keeps the per-degree route
         prof = ops.KernelProfile(time_events=False)
         xs = [x.clone().requires_grad_(True) for x in xs0]
         monkeypatch.setattr(ops, "PROFILE", prof)

@@ -242,7 +242,7 @@ def test_bucketed_stream_of_batches_matches_eager(cuda_device):
 
 
 def test_fused_forward_model_matches_unfused_model(cuda_device, monkeypatch):
-    """K1 on (EQF_FUSED=1: every depth-wise product feeds its linears on chip, backward recomputes) against K1 off on the
+    """K1 on (``ops._FUSED_MODE = "1"``: every depth-wise product feeds its linears on chip, backward recomputes) against K1 off on the
     same model and batch: energies and every parameter gradient."""
     from equiformer_b200 import ops
     model = _build("graph_attention_transformer_nonlinear_l2", cuda_device)

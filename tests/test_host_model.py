@@ -215,15 +215,16 @@ def test_bucketed_step_padding_leaves_loss_and_gradients_unchanged():
 
 def test_radial_first_layers_run_as_one_product(monkeypatch):
     """The first Linear of the 7 radial MLPs of the QM9 model is ONE stacked product (``radial_func.hoist_first_layers``);
-    outputs and gradients equal the per-module evaluation (``EQF_RAD_HOIST=0``)."""
+    outputs and gradients equal the per-module evaluation (the model with nothing hoisted)."""
     from equiformer_b200 import ops
-    from equiformer_b200.nets import radial_func
+    from equiformer_b200.nets import graph_attention_transformer
     model = _build("graph_attention_transformer_nonlinear_l2")
     pos, batch, z = molecules([5, 7], seed=3, dtype=torch.float64)
     real = ops.linear_f32
     results = {}
     for hoist in (True, False):
-        monkeypatch.setattr(radial_func, "_HOIST", hoist)
+        if not hoist:
+            monkeypatch.setattr(graph_attention_transformer, "hoist_first_layers", lambda modules, x: [])
         calls = []
         monkeypatch.setattr(ops, "linear_f32", lambda x, w, b=None: (calls.append(tuple(w.shape)), real(x, w, b))[1])
         model.zero_grad(set_to_none=True)

@@ -295,8 +295,7 @@ def test_cuda_headline_model_matches_reference_model_file(cuda_device):
 
 @pytest.fixture
 def tensor_core_gemms_everywhere():
-    """Lower the row thresholds of the GEMM policy (``ops._GEMM_MIN_M`` / ``_WGRAD_MIN_K``; env EQF_GEMM_MIN_M /
-    EQF_WGRAD_MIN_K) so that even the 16-atom reference-run fixtures go through the hand-written wgmma kernels instead
+    """Lower the row thresholds of the GEMM policy (``ops._GEMM_MIN_M`` / ``_WGRAD_MIN_K``) so that even the 16-atom reference-run fixtures go through the hand-written wgmma kernels instead
     of cuBLAS (VERDICT r1: at these sizes ``M = E (2l+1) << 16 384`` and every product used to be a cuBLAS call)."""
     from equiformer_b200 import ops
     old = ops._GEMM_MIN_M, ops._WGRAD_MIN_K

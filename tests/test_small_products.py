@@ -9,11 +9,9 @@ from equiformer_b200 import _lib, ops
 
 def test_tcgen05_dispatch_thresholds(monkeypatch):
     monkeypatch.setattr(ops, "_GEMM_MIN_M", 16384)
-    monkeypatch.setattr(ops, "_GEMM_MIN_FLOP", float("inf"))
     assert ops._use_tensor_cores(32560, 64, 128) and not ops._use_tensor_cores(11620, 32, 32)
     assert not ops._use_tensor_cores(14700, 32, 576)              # the MD17 edge-level products stay on the grouped kernel
-    monkeypatch.setattr(ops, "_GEMM_MIN_FLOP", 4e8)
-    assert ops._use_tensor_cores(14700, 32, 576) and not ops._use_tensor_cores(2324, 128, 128)
+    assert not ops._use_tensor_cores(2324, 128, 128)
     assert not ops._use_tensor_cores(512, 4096, 4096)             # a flop-heavy product with too few rows for 128-row tiles
     monkeypatch.setattr(ops, "_GEMM_MIN_M", 1)               # smoke() / the tensor-core-forced parity tests
     assert ops._use_tensor_cores(7, 4, 4)

@@ -59,8 +59,7 @@ def main():
     rows["grad_xw(shared w)"] = timeit(lambda: ops.dtp_grad_xw_raw(plan, xs, y, ws, gs), ops._dtp_bytes(plan, E, True, "grad_xw"))
     rows["grad_x"] = timeit(lambda: ops.dtp_grad_x_raw(plan, gs, y, w), ops._dtp_bytes(plan, E, False, "grad_x"))
     rows["grad_y"] = timeit(lambda: ops.dtp_grad_y_raw(plan, xs, w, gs, y), ops._dtp_bytes(plan, E, False, "grad_y"))
-    out = {"config": name, "E": E, "generated": bool(plan.generated), "variant": os.environ.get("EQF_DTP_VARIANT", "tma"), "tile": os.environ.get("EQF_TILE_EDGES", "8"),
-           "peak_gbs": peak}
+    out = {"config": name, "E": E, "generated": bool(plan.generated), "peak_gbs": peak}
     for k, (us, gbs) in rows.items():
         out[k] = {"us": round(us, 1), "gb_s": round(gbs, 1), "frac": round(gbs / peak, 3)}
     print(json.dumps(out))

@@ -80,7 +80,6 @@ def main():
             tot_u += us_gemm
         row["fused_total_us"] = round(tot_f, 1)
         row["unfused_total_us"] = round(tot_u + us_dtp, 1)
-        row["dbg_skip"] = os.environ.get("EQF_FUSED_DBG_SKIP", "0")
         print(json.dumps(row), flush=True)
 
 
