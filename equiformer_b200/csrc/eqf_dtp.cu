@@ -509,6 +509,7 @@ extern "C" int eqf_dtp_grad_y(const EqfPlan* plan, const EqfEdgeOperands* op, in
   int rc = fill_args(plan, op, n_edges, a, true, true, true);
   if (rc != EQF_OK || n_edges == 0) return rc;
   if (gy == nullptr) { set_error("null gy"); return EQF_ERR_INVALID; }
+  if (a.src != nullptr) { set_error("eqf_dtp_grad_y: x is read per edge (no gather)"); return EQF_ERR_UNSUPPORTED; }
   a.gy = gy;
   if (plan->gen != nullptr) return plan->gen->grad_y(plan, a, (cudaStream_t)stream);
   const size_t smem = plan->smem_bytes;

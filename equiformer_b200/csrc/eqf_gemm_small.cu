@@ -187,12 +187,12 @@ __global__ void __launch_bounds__(kThreadsM) grouped_gemm_mma_kernel(const __gri
   const int tn = local % p.tiles_n; local /= p.tiles_n;
   const int tm = local % p.tiles_m;
   const int split = local / p.tiles_m;
+  // the three modes of eqf_gemm_grouped; no mode reads A along M and B along k, so <false, true> is not instantiated
   if (p.a_kc) {
     if (p.b_kc) mma_tile<true, true>(p, tm, tn, split, As, Bs);
     else mma_tile<true, false>(p, tm, tn, split, As, Bs);
   } else {
-    if (p.b_kc) mma_tile<false, true>(p, tm, tn, split, As, Bs);
-    else mma_tile<false, false>(p, tm, tn, split, As, Bs);
+    mma_tile<false, false>(p, tm, tn, split, As, Bs);
   }
 }
 

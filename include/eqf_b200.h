@@ -97,7 +97,8 @@ int eqf_dtp_grad_x(const EqfPlan* plan, const EqfEdgeOperands* op, int64_t n_edg
 int eqf_dtp_grad_w(const EqfPlan* plan, const EqfEdgeOperands* op, int64_t n_edges,
                    float* gw, void* stream);
 
-/* d/dy: gy[E][d_y] (needed for MD17 forces, graph_attention_transformer_md17.py:318-325). */
+/* d/dy: gy[E][d_y] (needed for MD17 forces, graph_attention_transformer_md17.py:318-325).  x is read per edge: op->src
+ * must be NULL (EQF_ERR_UNSUPPORTED otherwise). */
 int eqf_dtp_grad_y(const EqfPlan* plan, const EqfEdgeOperands* op, int64_t n_edges,
                    float* gy, void* stream);
 
