@@ -19,6 +19,10 @@ PKG_DIR = Path(__file__).resolve().parent
 CSRC_DIR = PKG_DIR / "csrc"
 INCLUDE_DIR = PKG_DIR.parent / "include"
 LIB_PATH = PKG_DIR / "libeqf_b200.so"
+# depth-wise plans with an in1 / output degree of 4: the plan and table-walk DTP sources built once more with
+# -DEQF_MAX_DEGREE=4, so that the degree-4 branches stay out of the kernels of the main library
+L4_LIB_PATH = PKG_DIR / "libeqf_b200_l4.so"
+L4_SOURCES = ("eqf_abi.cu", "eqf_dtp.cu", "eqf_dtp_vec.cu")
 SOURCES = ("eqf_abi.cu", "eqf_dtp.cu", "eqf_dtp_vec.cu", "eqf_attn.cu", "eqf_pointwise.cu", "eqf_gemm_tf32x3.cu", "eqf_graph.cu",
            "eqf_fused.cu", "eqf_edge.cu", "eqf_gemm_small.cu")
 
@@ -157,9 +161,10 @@ SIGNATURES = {
                                              c_void_p, c_void_p]),
     "eqf_radius_graph_pbc_fill": (c_int32, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_float, c_int32, c_int32, c_int32,
                                             c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
-    "eqf_edge_geom_fwd": (c_int32, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int32, c_void_p,
-                                    c_void_p, c_void_p, c_void_p]),
-    "eqf_edge_geom_bwd": (c_int32, [c_void_p, c_void_p, c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "eqf_edge_geom_fwd": (c_int32, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int32,
+                                    c_void_p, c_void_p, c_void_p, c_void_p]),
+    "eqf_edge_geom_bwd": (c_int32, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_void_p,
+                                    c_void_p]),
     "eqf_expnorm_fwd": (c_int32, [c_void_p, c_void_p, c_void_p, c_float, c_float, c_int64, c_int32, c_void_p, c_void_p]),
     "eqf_expnorm_bwd": (c_int32, [c_void_p, c_void_p, c_void_p, c_float, c_float, c_int64, c_int32, c_void_p, c_void_p, c_void_p]),
     "eqf_bessel_fwd": (c_int32, [c_void_p, c_void_p, c_float, c_int64, c_int32, c_void_p, c_void_p]),
@@ -205,15 +210,16 @@ def generate_sources():
 
 
 def needs_build() -> bool:
-    if not LIB_PATH.exists():
+    if not LIB_PATH.exists() or not L4_LIB_PATH.exists():
         return True
-    mtime = LIB_PATH.stat().st_mtime
+    mtime = min(LIB_PATH.stat().st_mtime, L4_LIB_PATH.stat().st_mtime)
     deps = sources() + list(CSRC_DIR.glob("*.cuh")) + [INCLUDE_DIR / "eqf_b200.h"]
     return any(p.stat().st_mtime > mtime for p in deps)
 
 
 def build(force: bool = False, verbose: bool = False) -> Path:
-    """Compile ``csrc/*.cu`` for sm_90a into ``equiformer_b200/libeqf_b200.so`` (in-tree)."""
+    """Compile ``csrc/*.cu`` for sm_90a into ``equiformer_b200/libeqf_b200.so`` and ``L4_SOURCES`` with
+    ``-DEQF_MAX_DEGREE=4`` into ``equiformer_b200/libeqf_b200_l4.so`` (in-tree)."""
     generate_sources()
     if not force and not needs_build():
         return LIB_PATH
@@ -221,36 +227,75 @@ def build(force: bool = False, verbose: bool = False) -> Path:
     if not os.path.exists(nvcc):
         raise EqfError("nvcc not found: cannot build libeqf_b200.so")
     # one nvcc per source file, in parallel (the plan-specialised files take a minute each), then one
-    # link step; objects live in a scratch directory next to the library
+    # link step per library; objects live in a scratch directory next to the libraries
     from concurrent.futures import ThreadPoolExecutor
     obj_dir = PKG_DIR / "build" / ("obj%d" % os.getpid())
     obj_dir.mkdir(parents=True, exist_ok=True)
     compile_flags = [f for f in NVCC_FLAGS if f != "--shared"]
+    jobs = [(src, "", []) for src in sources()] + [(CSRC_DIR / s, "_l4", ["-DEQF_MAX_DEGREE=4"]) for s in L4_SOURCES]
 
-    def compile_one(src: Path):
-        obj = obj_dir / (src.stem + ".o")
-        cmd = [nvcc, *compile_flags, "-I", str(INCLUDE_DIR), "-c", "-o", str(obj), str(src)]
+    def compile_one(job):
+        src, suffix, defines = job
+        obj = obj_dir / (src.stem + suffix + ".o")
+        cmd = [nvcc, *compile_flags, *defines, "-I", str(INCLUDE_DIR), "-c", "-o", str(obj), str(src)]
         if verbose:
             cmd.insert(1, "-Xptxas=-v")
-        return obj, subprocess.run(cmd, capture_output=True, text=True)
+        return obj, suffix, subprocess.run(cmd, capture_output=True, text=True)
+
+    def link(path: Path, objs):
+        tmp = path.with_suffix(".so.tmp%d" % os.getpid())
+        proc = subprocess.run([nvcc, "--shared", "-Xcompiler", "-fPIC", "-gencode", "arch=compute_90a,code=sm_90a",
+                               "-o", str(tmp), *[str(o) for o in objs]], capture_output=True, text=True)
+        if proc.returncode != 0:
+            raise EqfError("nvcc link failed:\n" + proc.stdout + proc.stderr)
+        os.replace(tmp, path)
 
     try:
         with ThreadPoolExecutor(max_workers=min(8, os.cpu_count() or 1)) as pool:
-            results = list(pool.map(compile_one, sources()))
-        for _obj, proc in results:
+            results = list(pool.map(compile_one, jobs))
+        for _obj, _suffix, proc in results:
             if proc.returncode != 0:
                 raise EqfError("nvcc failed:\n" + proc.stdout + proc.stderr)
             if verbose:
                 print(proc.stderr)
-        tmp = LIB_PATH.with_suffix(".so.tmp%d" % os.getpid())
-        link = subprocess.run([nvcc, "--shared", "-Xcompiler", "-fPIC", "-gencode", "arch=compute_90a,code=sm_90a",
-                               "-o", str(tmp), *[str(o) for o, _ in results]], capture_output=True, text=True)
-        if link.returncode != 0:
-            raise EqfError("nvcc link failed:\n" + link.stdout + link.stderr)
-        os.replace(tmp, LIB_PATH)
+        link(LIB_PATH, [o for o, suffix, _ in results if suffix == ""])
+        link(L4_LIB_PATH, [o for o, suffix, _ in results if suffix == "_l4"])
     finally:
         shutil.rmtree(obj_dir, ignore_errors=True)
     return LIB_PATH
+
+
+def _open(path: Path, required: bool):
+    if not path.exists():
+        raise EqfError(
+            f"{path} is missing: run `python -c 'import __graft_entry__ as g; g.build()'` "
+            "(the sm_90a kernels are the only implementation of the edge path)")
+    lib = ctypes.CDLL(str(path))
+    for name, (restype, argtypes) in SIGNATURES.items():
+        try:
+            fn = getattr(lib, name)
+        except AttributeError as exc:  # stale build (the degree-4 library exports the plan and DTP entry points only)
+            if required:
+                raise EqfError(f"{path.name} does not export {name}; rebuild it") from exc
+            continue
+        fn.restype = restype
+        fn.argtypes = argtypes
+    return lib
+
+
+_lib_l4 = None
+
+
+def load_l4():
+    """Return the loaded degree-4 library (plan creation and the table-walk DTP kernels with in1 / output degree <= 4)."""
+    global _lib_l4
+    with _lock:
+        if _lib_l4 is None:
+            lib = _open(L4_LIB_PATH, required=False)
+            if not hasattr(lib, "eqf_dtp_forward"):
+                raise EqfError(f"{L4_LIB_PATH.name} does not export eqf_dtp_forward; rebuild it")
+            _lib_l4 = lib
+    return _lib_l4
 
 
 def load():
@@ -261,23 +306,13 @@ def load():
     with _lock:
         if _lib is not None:
             return _lib
-        if not LIB_PATH.exists():
-            raise EqfError(
-                f"{LIB_PATH} is missing: run `python -c 'import __graft_entry__ as g; g.build()'` "
-                "(the sm_90a kernels are the only implementation of the edge path)")
-        lib = ctypes.CDLL(str(LIB_PATH))
-        for name, (restype, argtypes) in SIGNATURES.items():
-            try:
-                fn = getattr(lib, name)
-            except AttributeError as exc:  # stale build
-                raise EqfError(f"libeqf_b200.so does not export {name}; rebuild it") from exc
-            fn.restype = restype
-            fn.argtypes = argtypes
-        _lib = lib
+        _lib = _open(LIB_PATH, required=True)
     return _lib
 
 
-def check(rc: int, what: str) -> None:
+def check(rc: int, what: str, lib=None) -> None:
+    """Raise with the library's last error message when ``rc`` is not ``EQF_OK`` (``lib``: the library that returned it,
+    default the main one)."""
     if rc != 0:
-        msg = load().eqf_last_error()
+        msg = (lib if lib is not None else load()).eqf_last_error()
         raise EqfError(f"{what} failed (code {rc}): {msg.decode() if msg else '?'}")

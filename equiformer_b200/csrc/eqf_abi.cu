@@ -90,14 +90,16 @@ extern "C" int eqf_plan_create(const EqfPathDesc* paths, int32_t n_paths, const 
   std::memset(&h, 0, sizeof(h));
   h.n_paths = n_paths; h.n_in1 = n_in1; h.n_out = n_out; h.d_y = d_y; h.w_numel = weight_numel; h.cg_len = cg_len;
   for (int b = 0; b < n_in1; ++b) {
-    if (in1_l[b] < 0 || 2 * in1_l[b] + 1 > kMaxD || in1_mul[b] < 1) {
-      delete plan; set_error("in1 degree must be 0..3 and mul >= 1"); return EQF_ERR_UNSUPPORTED;
+    if (in1_l[b] < 0 || 2 * in1_l[b] + 1 > kMaxDtpD || in1_mul[b] < 1) {
+      delete plan; set_error("in1 degree must be 0.." + std::to_string(EQF_MAX_DEGREE) + " and mul >= 1");
+      return EQF_ERR_UNSUPPORTED;
     }
     h.in1_d[b] = 2 * in1_l[b] + 1; h.in1_mul[b] = in1_mul[b];
   }
   for (int g = 0; g < n_out; ++g) {
-    if (out_l[g] < 0 || 2 * out_l[g] + 1 > kMaxD || out_mul[g] < 1) {
-      delete plan; set_error("output degree must be 0..3 and mul >= 1"); return EQF_ERR_UNSUPPORTED;
+    if (out_l[g] < 0 || 2 * out_l[g] + 1 > kMaxDtpD || out_mul[g] < 1) {
+      delete plan; set_error("output degree must be 0.." + std::to_string(EQF_MAX_DEGREE) + " and mul >= 1");
+      return EQF_ERR_UNSUPPORTED;
     }
     h.out_d[g] = 2 * out_l[g] + 1; h.out_mul[g] = out_mul[g];
   }
@@ -108,7 +110,9 @@ extern "C" int eqf_plan_create(const EqfPathDesc* paths, int32_t n_paths, const 
     const EqfPathDesc& s = paths[p];
     PathDev& d = pd[p];
     const bool tri = s.l3 >= std::abs(s.l1 - s.l2) && s.l3 <= s.l1 + s.l2;
-    if (s.l1 < 0 || s.l2 < 0 || s.l3 < 0 || !tri || 2 * s.l1 + 1 > kMaxD || 2 * s.l3 + 1 > kMaxD || 2 * s.l2 + 1 > 15) {
+    // d1, d3 <= kMaxDtpD: the table-walk kernels dispatch on them at compile time (EQF_DISPATCH_D); up to 9 they also fit
+    // mdesc's 4-bit fields
+    if (s.l1 < 0 || s.l2 < 0 || s.l3 < 0 || !tri || 2 * s.l1 + 1 > kMaxDtpD || 2 * s.l3 + 1 > kMaxDtpD || 2 * s.l2 + 1 > 15) {
       delete plan; set_error("path degrees unsupported or violate the triangle rule"); return EQF_ERR_UNSUPPORTED;
     }
     d.d1 = 2 * s.l1 + 1; d.d2 = 2 * s.l2 + 1; d.d3 = 2 * s.l3 + 1;

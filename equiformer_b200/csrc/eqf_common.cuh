@@ -13,7 +13,19 @@ namespace eqf {
 
 constexpr int kThreads = 256;           // threads per CTA for the edge kernels
 constexpr int kWarps = kThreads / 32;
-constexpr int kMaxD = 7;                // degrees 0..3  (2l+1 <= 7)
+constexpr int kMaxD = 7;                // degrees 0..3  (2l+1 <= 7): fused DTP -> linear kernel (eqf_fused.cu)
+// Largest in1 / output degree of a depth-wise plan.  libeqf_b200.so keeps 3; the table-walk DTP sources (eqf_abi.cu,
+// eqf_dtp.cu, eqf_dtp_vec.cu) are built a second time with -DEQF_MAX_DEGREE=4 into libeqf_b200_l4.so, so the degree-4
+// branches never enter the kernels (and the register allocation) of the l <= 3 library.
+#ifndef EQF_MAX_DEGREE
+#define EQF_MAX_DEGREE 3
+#endif
+constexpr int kMaxDtpD = 2 * EQF_MAX_DEGREE + 1;
+#if EQF_MAX_DEGREE >= 4
+#define EQF_CASE_D9(NAME, ...) case 9: { constexpr int NAME = 9; __VA_ARGS__; } break;
+#else
+#define EQF_CASE_D9(NAME, ...)
+#endif
 
 // Device-side path record (one Clebsch-Gordan path); mirrors EqfPathDesc + derived fields.
 struct PathDev {
@@ -29,6 +41,32 @@ struct PathDev {
   int pad;
 };
 static_assert(sizeof(PathDev) == 48, "PathDev layout");
+
+// One path's per-edge coupling matrix M_p[i, k] (i < D1, k < D3) as the table-walk DTP kernels read it.  Up to 7 x 7 it is
+// copied to registers once per task.  A degree-4 side would make that up to 9 x 9 = 81 registers, and since a kernel's
+// register count is the maximum over all of its branches, it would raise the count (or spill) for every l <= 3 plan too;
+// so a path with a degree-4 input or output reads each entry from shared memory where it is used (a broadcast load), and
+// its task loops over the output components k one at a time (`#pragma unroll 1`), so that neither the tile nor a row of
+// cotangents is ever live in registers at once.
+template <int D1, int D3, bool IN_REGS = (D1 <= 7 && D3 <= 7)>
+struct MTile {
+  static constexpr bool kInRegs = true;
+  float v[D1][D3];
+  __device__ __forceinline__ explicit MTile(const float* __restrict__ Mp) {
+#pragma unroll
+    for (int i = 0; i < D1; ++i)
+#pragma unroll
+      for (int k = 0; k < D3; ++k) v[i][k] = Mp[i * D3 + k];
+  }
+  __device__ __forceinline__ float operator()(int i, int k) const { return v[i][k]; }
+};
+template <int D1, int D3>
+struct MTile<D1, D3, false> {
+  static constexpr bool kInRegs = false;
+  const float* __restrict__ p;
+  __device__ __forceinline__ explicit MTile(const float* __restrict__ Mp) : p(Mp) {}
+  __device__ __forceinline__ float operator()(int i, int k) const { return p[i * D3 + k]; }
+};
 
 // Header passed by value to every edge kernel; offsets index the int/float blob in global memory.
 struct PlanHdr {

@@ -85,6 +85,7 @@ __device__ __forceinline__ void stage_tile(const PlanHdr& h, const Smem& s, cons
     case 3: { constexpr int NAME = 3; __VA_ARGS__; } break;  \
     case 5: { constexpr int NAME = 5; __VA_ARGS__; } break;  \
     case 7: { constexpr int NAME = 7; __VA_ARGS__; } break;  \
+    EQF_CASE_D9(NAME, __VA_ARGS__)                           \
     default: break;                                          \
   }
 
@@ -102,14 +103,6 @@ __device__ __forceinline__ void load_x(const EdgeArgs& a, int xb, int mul, long 
   }
 }
 
-template <int D1, int D3>
-__device__ __forceinline__ void load_M(const float* __restrict__ Mp, float (&M)[D1][D3]) {
-#pragma unroll
-  for (int i = 0; i < D1; ++i)
-#pragma unroll
-    for (int k = 0; k < D3; ++k) M[i][k] = Mp[i * D3 + k];
-}
-
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -121,20 +114,29 @@ __device__ __forceinline__ float warp_sum(float v) {
 template <int D1, int D3>
 __device__ __forceinline__ void fwd_task(const PlanHdr& h, const EdgeArgs& a, const PathDev& P, const float* Mp,
                                          long long e, int u) {
-  float M[D1][D3];
-  load_M<D1, D3>(Mp, M);
+  const MTile<D1, D3> M(Mp);
   if (u >= P.mul) return;
   float xi[D1];
   load_x<D1>(a, P.xb, P.mul, e, u, xi);
   const float wv = __ldg(a.w + (a.w_shared ? 0 : e * h.w_numel) + P.w_off + u);
   const int K = h.out_mul[P.og];
   float* o = a.out[P.og] + (e * D3) * K + P.koff + u;
+  if constexpr (MTile<D1, D3>::kInRegs) {
 #pragma unroll
-  for (int k = 0; k < D3; ++k) {
-    float acc = 0.f;
+    for (int k = 0; k < D3; ++k) {
+      float acc = 0.f;
 #pragma unroll
-    for (int i = 0; i < D1; ++i) acc = fmaf(xi[i], M[i][k], acc);
-    o[(long long)k * K] = wv * acc;
+      for (int i = 0; i < D1; ++i) acc = fmaf(xi[i], M(i, k), acc);
+      o[(long long)k * K] = wv * acc;
+    }
+  } else {
+#pragma unroll 1
+    for (int k = 0; k < D3; ++k) {
+      float acc = 0.f;
+#pragma unroll
+      for (int i = 0; i < D1; ++i) acc = fmaf(xi[i], M(i, k), acc);
+      o[(long long)k * K] = wv * acc;
+    }
   }
 }
 
@@ -166,21 +168,31 @@ __global__ void __launch_bounds__(kThreads) dtp_forward_kernel(PlanHdr h, const 
 template <int D1, int D3>
 __device__ __forceinline__ float gw_value(const PlanHdr& h, const EdgeArgs& a, const PathDev& P, const float* Mp,
                                           long long e, int u) {
-  float M[D1][D3];
-  load_M<D1, D3>(Mp, M);
+  const MTile<D1, D3> M(Mp);
   if (u >= P.mul) return 0.f;
   float xi[D1];
   load_x<D1>(a, P.xb, P.mul, e, u, xi);
   const int K = h.out_mul[P.og];
   const float* gp = a.g[P.og] + (e * D3) * K + P.koff + u;
   float acc = 0.f;
+  if constexpr (MTile<D1, D3>::kInRegs) {
 #pragma unroll
-  for (int k = 0; k < D3; ++k) {
-    const float gk = __ldg(gp + (long long)k * K);
-    float t = 0.f;
+    for (int k = 0; k < D3; ++k) {
+      const float gk = __ldg(gp + (long long)k * K);
+      float t = 0.f;
 #pragma unroll
-    for (int i = 0; i < D1; ++i) t = fmaf(xi[i], M[i][k], t);
-    acc = fmaf(t, gk, acc);
+      for (int i = 0; i < D1; ++i) t = fmaf(xi[i], M(i, k), t);
+      acc = fmaf(t, gk, acc);
+    }
+  } else {
+#pragma unroll 1
+    for (int k = 0; k < D3; ++k) {
+      const float gk = __ldg(gp + (long long)k * K);
+      float t = 0.f;
+#pragma unroll
+      for (int i = 0; i < D1; ++i) t = fmaf(xi[i], M(i, k), t);
+      acc = fmaf(t, gk, acc);
+    }
   }
   return acc;
 }
@@ -225,22 +237,34 @@ __global__ void __launch_bounds__(kThreads) dtp_grad_w_kernel(PlanHdr h, const u
 template <int D1, int D3, bool WITH_W>
 __device__ __forceinline__ void gx_path(const PlanHdr& h, const EdgeArgs& a, const PathDev& P, const float* Mp,
                                         long long e, int u, const float (&xi)[D1], float (&acc)[D1], float* wacc) {
-  float M[D1][D3];
-  load_M<D1, D3>(Mp, M);
+  const MTile<D1, D3> M(Mp);
   const int K = h.out_mul[P.og];
   const float* gp = a.g[P.og] + (e * D3) * K + P.koff + u;
-  float gk[D3];
-#pragma unroll
-  for (int k = 0; k < D3; ++k) gk[k] = __ldg(gp + (long long)k * K);
   const float wv = __ldg(a.w + (a.w_shared ? 0 : e * h.w_numel) + P.w_off + u);
   float gwv = 0.f;
+  if constexpr (MTile<D1, D3>::kInRegs) {
+    float gk[D3];
 #pragma unroll
-  for (int i = 0; i < D1; ++i) {
-    float t = 0.f;
+    for (int k = 0; k < D3; ++k) gk[k] = __ldg(gp + (long long)k * K);
 #pragma unroll
-    for (int k = 0; k < D3; ++k) t = fmaf(gk[k], M[i][k], t);
-    acc[i] = fmaf(wv, t, acc[i]);
-    if (WITH_W) gwv = fmaf(xi[i], t, gwv);
+    for (int i = 0; i < D1; ++i) {
+      float t = 0.f;
+#pragma unroll
+      for (int k = 0; k < D3; ++k) t = fmaf(gk[k], M(i, k), t);
+      acc[i] = fmaf(wv, t, acc[i]);
+      if (WITH_W) gwv = fmaf(xi[i], t, gwv);
+    }
+  } else {                    // one cotangent component at a time (acc[] stays indexed by compile-time i)
+#pragma unroll 1
+    for (int k = 0; k < D3; ++k) {
+      const float gk = __ldg(gp + (long long)k * K);
+#pragma unroll
+      for (int i = 0; i < D1; ++i) {
+        const float t = gk * M(i, k);
+        acc[i] = fmaf(wv, t, acc[i]);
+        if (WITH_W) gwv = fmaf(xi[i], t, gwv);
+      }
+    }
   }
   if (WITH_W) {
     if (a.w_shared) atomicAdd(wacc + P.w_off + u, gwv);
@@ -308,6 +332,24 @@ __device__ __forceinline__ void gy_task(const PlanHdr& h, const EdgeArgs& a, con
   for (int i = 0; i < D1; ++i) xi[i] = 0.f;
 #pragma unroll
   for (int k = 0; k < D3; ++k) gk[k] = 0.f;
+  if constexpr (!MTile<D1, D3>::kInRegs) {   // degree 4: one cotangent component at a time, as in gx_path
+    const int K = h.out_mul[P.og];
+    const float* gp = a.g[P.og] + (e * D3) * K + P.koff + u;
+    if (u < P.mul) {
+      load_x<D1>(a, P.xb, P.mul, e, u, xi);
+      wv = __ldg(a.w + (a.w_shared ? 0 : e * h.w_numel) + P.w_off + u);
+    }
+#pragma unroll 1
+    for (int k = 0; k < D3; ++k) {
+      const float g = u < P.mul ? __ldg(gp + (long long)k * K) : 0.f;
+#pragma unroll
+      for (int i = 0; i < D1; ++i) {
+        const float r = warp_sum(wv * xi[i] * g);
+        if (lane == 0) atomicAdd(Np + i * D3 + k, r);
+      }
+    }
+    return;
+  }
   if (u < P.mul) {
     load_x<D1>(a, P.xb, P.mul, e, u, xi);
     const int K = h.out_mul[P.og];

@@ -82,6 +82,7 @@ __device__ __forceinline__ void vstage_tile(const PlanHdr& h, const VSmem& s, co
     case 3: { constexpr int NAME = 3; __VA_ARGS__; } break;  \
     case 5: { constexpr int NAME = 5; __VA_ARGS__; } break;  \
     case 7: { constexpr int NAME = 7; __VA_ARGS__; } break;  \
+    EQF_CASE_D9(NAME, __VA_ARGS__)                           \
     default: break;                                          \
   }
 
@@ -113,14 +114,6 @@ __device__ __forceinline__ void load_x4(const EdgeArgs& a, int xb, int mul, long
       xi[i].x += t.x; xi[i].y += t.y; xi[i].z += t.z; xi[i].w += t.w;
     }
   }
-}
-
-template <int D1, int D3>
-__device__ __forceinline__ void vload_M(const float* __restrict__ Mp, float (&M)[D1][D3]) {
-#pragma unroll
-  for (int i = 0; i < D1; ++i)
-#pragma unroll
-    for (int k = 0; k < D3; ++k) M[i][k] = Mp[i * D3 + k];
 }
 
 // lane -> (edge inside the tile, first channel) for a vector task
@@ -169,8 +162,7 @@ __device__ __forceinline__ void vfwd_task(const PlanHdr& h, const EdgeArgs& a, c
                                           const LaneMap& lm, long long e0, const float* wtile) {
   if (!lm.ok) return;
   const long long e = e0 + lm.te;
-  float M[D1][D3];
-  vload_M<D1, D3>(s.M + lm.te * h.m_size + P.m_off, M);
+  const MTile<D1, D3> M(s.M + lm.te * h.m_size + P.m_off);
   float4 xi[D1];
   load_x4<D1>(a, P.xb, P.mul, e, lm.u, xi);
   float4 wv;
@@ -178,12 +170,22 @@ __device__ __forceinline__ void vfwd_task(const PlanHdr& h, const EdgeArgs& a, c
   else wv = ldg4(a.w + (a.w_shared ? 0 : e * h.w_numel) + P.w_off + lm.u);
   const int K = h.out_mul[P.og];
   float* o = a.out[P.og] + (e * D3) * K + P.koff + lm.u;
+  if constexpr (MTile<D1, D3>::kInRegs) {
 #pragma unroll
-  for (int k = 0; k < D3; ++k) {
-    float4 acc = f4zero();
+    for (int k = 0; k < D3; ++k) {
+      float4 acc = f4zero();
 #pragma unroll
-    for (int i = 0; i < D1; ++i) fma4(acc, xi[i], M[i][k]);
-    stg4(o + (long long)k * K, mul44(acc, wv));
+      for (int i = 0; i < D1; ++i) fma4(acc, xi[i], M(i, k));
+      stg4(o + (long long)k * K, mul44(acc, wv));
+    }
+  } else {
+#pragma unroll 1
+    for (int k = 0; k < D3; ++k) {
+      float4 acc = f4zero();
+#pragma unroll
+      for (int i = 0; i < D1; ++i) fma4(acc, xi[i], M(i, k));
+      stg4(o + (long long)k * K, mul44(acc, wv));
+    }
   }
 }
 
@@ -243,22 +245,35 @@ template <int D1, int D3, bool WITH_W>
 __device__ __forceinline__ void vgx_path(const PlanHdr& h, const EdgeArgs& a, const VSmem& s, const PathDev& P,
                                          const LaneMap& lm, long long e, const float4 (&xi)[D1], float4 (&acc)[D1],
                                          float* wacc) {
-  float M[D1][D3];
-  vload_M<D1, D3>(s.M + lm.te * h.m_size + P.m_off, M);
+  const MTile<D1, D3> M(s.M + lm.te * h.m_size + P.m_off);
   const int K = h.out_mul[P.og];
   const float* gp = a.g[P.og] + (e * D3) * K + P.koff + lm.u;
-  float4 gk[D3];
-#pragma unroll
-  for (int k = 0; k < D3; ++k) gk[k] = ldg4(gp + (long long)k * K);
   const float4 wv = ldg4(a.w + (a.w_shared ? 0 : e * h.w_numel) + P.w_off + lm.u);
   float4 gwv = f4zero();
+  if constexpr (MTile<D1, D3>::kInRegs) {
+    float4 gk[D3];
 #pragma unroll
-  for (int i = 0; i < D1; ++i) {
-    float4 t = f4zero();
+    for (int k = 0; k < D3; ++k) gk[k] = ldg4(gp + (long long)k * K);
 #pragma unroll
-    for (int k = 0; k < D3; ++k) fma4(t, gk[k], M[i][k]);
-    fma44(acc[i], wv, t);
-    if (WITH_W) fma44(gwv, xi[i], t);
+    for (int i = 0; i < D1; ++i) {
+      float4 t = f4zero();
+#pragma unroll
+      for (int k = 0; k < D3; ++k) fma4(t, gk[k], M(i, k));
+      fma44(acc[i], wv, t);
+      if (WITH_W) fma44(gwv, xi[i], t);
+    }
+  } else {                    // one cotangent component at a time (acc[] stays indexed by compile-time i)
+#pragma unroll 1
+    for (int k = 0; k < D3; ++k) {
+      const float4 gk = ldg4(gp + (long long)k * K);
+      const float4 wg = mul44(wv, gk);
+#pragma unroll
+      for (int i = 0; i < D1; ++i) {
+        const float c = M(i, k);
+        fma4(acc[i], wg, c);
+        if (WITH_W) fma44(gwv, xi[i], make_float4(gk.x * c, gk.y * c, gk.z * c, gk.w * c));
+      }
+    }
   }
   if (WITH_W) {
     if (a.w_shared) {

@@ -1,5 +1,5 @@
 // eqf_edge.cu - edge-feature producers of the hot path (SURVEY.md rows a11, a12, f-2): one kernel for the edge geometry
-// (edge vector, length, real spherical harmonics up to l = 3) with its first-order backward to the edge vector, and the
+// (edge vector, length, real spherical harmonics up to l = 4) with its first-order backward to the edge vector, and the
 // exp-normal radial basis of the MD17 models.
 //
 // Reference work replaced:
@@ -12,8 +12,8 @@
 //                                                      envelope (p = 5) * sqrt(2 / c^3) sin(f_k d / c) / (d / c)
 // One thread per edge for the geometry (a few hundred flops, ~100 bytes), one warp per edge row for the bases.  The
 // harmonics follow e3nn's coupling recurrence  Y_{l+1,k} = sum_ji A_l[k,j,i] x_j Y_{l,i}  ('norm' normalisation, y polar,
-// Y_1 = (x, y, z)); the host passes the coupling tensors A_1, A_2 (equiformer_b200/o3/sh.py computes them from the real
-// Wigner 3j), so kernel and torch statement share one table.  Second derivatives (MD17 force training) go through the
+// Y_1 = (x, y, z)); the host passes the coupling tensors A_1, A_2, A_3 (equiformer_b200/o3/sh.py computes them from the
+// real Wigner 3j), so kernel and torch statement share one table.  Second derivatives (MD17 force training) go through the
 // torch statement (ops._higher_order_grads), like the other fused pointwise ops.
 #include <cuda_runtime.h>
 
@@ -30,17 +30,19 @@ struct EdgeGeomArgs {
   const float* offsets;        // optional [E, 3] added to pos[src] - pos[dst] (periodic images)
   const float* a1;             // coupling 1 -> 2: [5][3][3]
   const float* a2;             // coupling 2 -> 3: [7][3][5]
+  const float* a3;             // coupling 3 -> 4: [9][3][7]
   long long E;
-  int lmax;                    // 0 .. 3
+  int lmax;                    // 0 .. 4
   int n_sh;                    // (lmax + 1)^2
 };
 
 // forward: vec [E, 3], len [E], sh [E, n_sh] ('component' normalisation: Y_l * sqrt(2l+1)), harmonics of the UNIT vector
 __global__ void __launch_bounds__(256) edge_geom_fwd_kernel(EdgeGeomArgs a, float* __restrict__ vec, float* __restrict__ len,
                                                             float* __restrict__ sh) {
-  __shared__ float c1[45], c2[105];
+  __shared__ float c1[45], c2[105], c3[189];
   for (int i = threadIdx.x; i < 45; i += blockDim.x) c1[i] = a.lmax >= 2 ? a.a1[i] : 0.f;
   for (int i = threadIdx.x; i < 105; i += blockDim.x) c2[i] = a.lmax >= 3 ? a.a2[i] : 0.f;
+  for (int i = threadIdx.x; i < 189; i += blockDim.x) c3[i] = a.lmax >= 4 ? a.a3[i] : 0.f;
   __syncthreads();
   const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= a.E) return;
@@ -73,6 +75,7 @@ __global__ void __launch_bounds__(256) edge_geom_fwd_kernel(EdgeGeomArgs a, floa
     o[4 + k] = 2.23606797749979f * acc;
   }
   if (a.lmax < 3) return;
+  float y3[7];
 #pragma unroll
   for (int k = 0; k < 7; ++k) {
     float acc = 0.f;
@@ -80,7 +83,18 @@ __global__ void __launch_bounds__(256) edge_geom_fwd_kernel(EdgeGeomArgs a, floa
     for (int j = 0; j < 3; ++j)
 #pragma unroll
       for (int i = 0; i < 5; ++i) acc = fmaf(c2[(k * 3 + j) * 5 + i] * x[j], y2[i], acc);
+    y3[k] = acc;
     o[9 + k] = 2.6457513110645907f * acc;
+  }
+  if (a.lmax < 4) return;
+#pragma unroll
+  for (int k = 0; k < 9; ++k) {
+    float acc = 0.f;
+#pragma unroll
+    for (int j = 0; j < 3; ++j)
+#pragma unroll
+      for (int i = 0; i < 7; ++i) acc = fmaf(c3[(k * 3 + j) * 7 + i] * x[j], y3[i], acc);
+    o[16 + k] = 3.f * acc;
   }
 }
 
@@ -88,9 +102,10 @@ __global__ void __launch_bounds__(256) edge_geom_fwd_kernel(EdgeGeomArgs a, floa
 __global__ void __launch_bounds__(256) edge_geom_bwd_kernel(EdgeGeomArgs a, const float* __restrict__ vec,
                                                             const float* __restrict__ g_sh, const float* __restrict__ g_len,
                                                             float* __restrict__ g_vec) {
-  __shared__ float c1[45], c2[105];
+  __shared__ float c1[45], c2[105], c3[189];
   for (int i = threadIdx.x; i < 45; i += blockDim.x) c1[i] = a.lmax >= 2 ? a.a1[i] : 0.f;
   for (int i = threadIdx.x; i < 105; i += blockDim.x) c2[i] = a.lmax >= 3 ? a.a2[i] : 0.f;
+  for (int i = threadIdx.x; i < 189; i += blockDim.x) c3[i] = a.lmax >= 4 ? a.a3[i] : 0.f;
   __syncthreads();
   const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= a.E) return;
@@ -102,6 +117,7 @@ __global__ void __launch_bounds__(256) edge_geom_bwd_kernel(EdgeGeomArgs a, cons
   if (g_sh != nullptr && a.lmax >= 1) {
     const float* g = g_sh + e * a.n_sh;
     float y2[5] = {0.f, 0.f, 0.f, 0.f, 0.f}, g1[3], g2[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
+    float y3[7] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f}, g3[7] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
 #pragma unroll
     for (int q = 0; q < 3; ++q) g1[q] = 1.7320508075688772f * __ldg(g + 1 + q);
     if (a.lmax >= 2) {
@@ -116,10 +132,36 @@ __global__ void __launch_bounds__(256) edge_geom_bwd_kernel(EdgeGeomArgs a, cons
         g2[k] = 2.23606797749979f * __ldg(g + 4 + k);
       }
     }
+    if (a.lmax >= 3) {
+#pragma unroll
+      for (int k = 0; k < 7; ++k) {
+        float acc = 0.f;
+#pragma unroll
+        for (int j = 0; j < 3; ++j)
+#pragma unroll
+          for (int i = 0; i < 5; ++i) acc = fmaf(c2[(k * 3 + j) * 5 + i] * x[j], y2[i], acc);
+        y3[k] = acc;
+        g3[k] = 2.6457513110645907f * __ldg(g + 9 + k);
+      }
+    }
+    if (a.lmax >= 4) {                                  // Y_4 = A_3 . (x (x) Y_3): adjoints of x and of Y_3
+#pragma unroll 1                                        // one Y_4 component at a time (fully unrolled: 72 registers)
+      for (int k = 0; k < 9; ++k) {
+        const float gk = 3.f * __ldg(g + 16 + k);
+#pragma unroll
+        for (int j = 0; j < 3; ++j)
+#pragma unroll
+          for (int i = 0; i < 7; ++i) {
+            const float c = c3[(k * 3 + j) * 7 + i] * gk;
+            xb[j] = fmaf(c, y3[i], xb[j]);
+            g3[i] = fmaf(c, x[j], g3[i]);
+          }
+      }
+    }
     if (a.lmax >= 3) {                                  // Y_3 = A_2 . (x (x) Y_2): adjoints of x and of Y_2
 #pragma unroll
       for (int k = 0; k < 7; ++k) {
-        const float gk = 2.6457513110645907f * __ldg(g + 9 + k);
+        const float gk = g3[k];
 #pragma unroll
         for (int j = 0; j < 3; ++j)
 #pragma unroll
@@ -279,34 +321,36 @@ __global__ void __launch_bounds__(256) bessel_bwd_kernel(const float* __restrict
 using namespace eqf;
 
 static int fill_geom(EdgeGeomArgs& a, const float* pos, const int64_t* src, const int64_t* dst, const float* offsets,
-                     const float* a1, const float* a2, int64_t E, int32_t lmax, const char* who) {
-  if (lmax < 0 || lmax > 3) { set_error(std::string(who) + ": lmax must be 0..3"); return EQF_ERR_UNSUPPORTED; }
-  if (!pos || !src || !dst || (lmax >= 2 && !a1) || (lmax >= 3 && !a2)) { set_error(std::string(who) + ": null pointer"); return EQF_ERR_INVALID; }
+                     const float* a1, const float* a2, const float* a3, int64_t E, int32_t lmax, const char* who) {
+  if (lmax < 0 || lmax > 4) { set_error(std::string(who) + ": lmax must be 0..4"); return EQF_ERR_UNSUPPORTED; }
+  if (!pos || !src || !dst || (lmax >= 2 && !a1) || (lmax >= 3 && !a2) || (lmax >= 4 && !a3)) {
+    set_error(std::string(who) + ": null pointer"); return EQF_ERR_INVALID;
+  }
   a.pos = pos; a.src = reinterpret_cast<const long long*>(src); a.dst = reinterpret_cast<const long long*>(dst);
-  a.offsets = offsets; a.a1 = a1; a.a2 = a2; a.E = E; a.lmax = lmax; a.n_sh = (lmax + 1) * (lmax + 1);
+  a.offsets = offsets; a.a1 = a1; a.a2 = a2; a.a3 = a3; a.E = E; a.lmax = lmax; a.n_sh = (lmax + 1) * (lmax + 1);
   return EQF_OK;
 }
 
 extern "C" int eqf_edge_geom_fwd(const float* pos, const int64_t* src, const int64_t* dst, const float* offsets,
-                                 const float* a1, const float* a2, int64_t E, int32_t lmax, float* vec, float* len, float* sh,
-                                 void* stream) {
+                                 const float* a1, const float* a2, const float* a3, int64_t E, int32_t lmax, float* vec,
+                                 float* len, float* sh, void* stream) {
   if (E <= 0) return EQF_OK;
   EdgeGeomArgs a;
-  int rc = fill_geom(a, pos, src, dst, offsets, a1, a2, E, lmax, "eqf_edge_geom_fwd");
+  int rc = fill_geom(a, pos, src, dst, offsets, a1, a2, a3, E, lmax, "eqf_edge_geom_fwd");
   if (rc != EQF_OK) return rc;
   if (!vec || !len || !sh) { set_error("eqf_edge_geom_fwd: null output"); return EQF_ERR_INVALID; }
   edge_geom_fwd_kernel<<<(unsigned)((E + 255) / 256), 256, 0, (cudaStream_t)stream>>>(a, vec, len, sh);
   return check_cuda(cudaGetLastError(), "edge_geom_fwd_kernel launch");
 }
 
-extern "C" int eqf_edge_geom_bwd(const float* vec, const float* a1, const float* a2, int64_t E, int32_t lmax,
-                                 const float* g_sh, const float* g_len, float* g_vec, void* stream) {
+extern "C" int eqf_edge_geom_bwd(const float* vec, const float* a1, const float* a2, const float* a3, int64_t E,
+                                 int32_t lmax, const float* g_sh, const float* g_len, float* g_vec, void* stream) {
   if (E <= 0) return EQF_OK;
-  if (lmax < 0 || lmax > 3 || !vec || !g_vec || (lmax >= 2 && !a1) || (lmax >= 3 && !a2)) {
+  if (lmax < 0 || lmax > 4 || !vec || !g_vec || (lmax >= 2 && !a1) || (lmax >= 3 && !a2) || (lmax >= 4 && !a3)) {
     set_error("eqf_edge_geom_bwd: bad arguments"); return EQF_ERR_INVALID;
   }
   EdgeGeomArgs a;
-  a.pos = nullptr; a.src = a.dst = nullptr; a.offsets = nullptr; a.a1 = a1; a.a2 = a2; a.E = E; a.lmax = lmax;
+  a.pos = nullptr; a.src = a.dst = nullptr; a.offsets = nullptr; a.a1 = a1; a.a2 = a2; a.a3 = a3; a.E = E; a.lmax = lmax;
   a.n_sh = (lmax + 1) * (lmax + 1);
   edge_geom_bwd_kernel<<<(unsigned)((E + 255) / 256), 256, 0, (cudaStream_t)stream>>>(a, vec, g_sh, g_len, g_vec);
   return check_cuda(cudaGetLastError(), "edge_geom_bwd_kernel launch");

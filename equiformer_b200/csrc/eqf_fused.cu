@@ -600,6 +600,12 @@ static int collect_paths(const EqfPlan* plan, int group, FArgs& a) {
   int koff = 0, m_off = 0;
   for (size_t i = 0; i < ps.size(); ++i) {
     const PathDev& s = *ps[i];
+    // the coupling row cgr[kMaxD] spans d2, the non-zero mask nz has 64 bits for d1 x d3, and the group-forward kernel has
+    // instances up to d3 = 7: a group with a degree-4 operand or output takes the unfused route (table-walk DTP + GEMM)
+    if (s.d1 > kMaxD || s.d2 > kMaxD || s.d3 > kMaxD) {
+      set_error("fused DTP: degree-4 paths are not supported (2l+1 <= 7)");
+      return EQF_ERR_UNSUPPORTED;
+    }
     if (s.koff != koff || s.mul % BKT != 0) {
       set_error("fused DTP: group channels must be covered by paths of multiplicity % 32 == 0");
       return EQF_ERR_UNSUPPORTED;

@@ -841,10 +841,10 @@ def radial_basis(basis_type: str, number_of_basis: int, max_radius: float, suppo
 
 def edge_features(irreps_edge_attr, pos, graph, edge_vec=None):
     """``(edge_vec, edge_length, edge_sh)`` of a destination-sorted graph (ref :866-870).  When the edge irreps are the plain
-    harmonics ``0 .. lmax <= 3`` and the vector is ``pos[src] - pos[dst]`` this is ONE kernel (``ops.EdgeGeometry``; its
+    harmonics ``0 .. lmax <= 4`` and the vector is ``pos[src] - pos[dst]`` this is ONE kernel (``ops.EdgeGeometry``; its
     backward scatters to ``pos``); a caller-supplied ``edge_vec`` (periodic images) or other irreps take the torch chain."""
     ls = [ir.l for mul, ir in irreps_edge_attr for _ in range(mul)]
-    if (edge_vec is None and ls == list(range(len(ls))) and 1 <= len(ls) <= 4 and pos.is_cuda and pos.dtype == torch.float32
+    if (edge_vec is None and ls == list(range(len(ls))) and 1 <= len(ls) <= 5 and pos.is_cuda and pos.dtype == torch.float32
             and graph.perm is None and graph.n_edges > 0):
         return ops.edge_geometry(pos, graph, len(ls) - 1)
     if edge_vec is None:

@@ -225,8 +225,8 @@ def dtp_forward_raw(plan: DtpPlan, xs, y, w, gather=None, w_offset=None) -> List
     outs = [torch.empty((E, 2 * l + 1, mul), device=y.device, dtype=torch.float32) for l, _p, mul in plan.out_groups]
     op = _operands(plan, xs, y, w, None, shared, gather, w_offset)
     with torch.cuda.device(y.device), _kernel("dtp_forward", _dtp_bytes(plan, E, shared, "forward")):
-        rc = _lib.load().eqf_dtp_forward(plan.handle, ctypes.byref(op), E, _ptr_array(outs), _stream())
-    _lib.check(rc, "eqf_dtp_forward")
+        rc = plan.lib.eqf_dtp_forward(plan.handle, ctypes.byref(op), E, _ptr_array(outs), _stream())
+    _lib.check(rc, "eqf_dtp_forward", plan.lib)
     return outs
 
 
@@ -236,15 +236,15 @@ def dtp_grad_x_raw(plan: DtpPlan, gs, y, w) -> List[torch.Tensor]:
     gxs = [torch.empty((E, 2 * l + 1, mul), device=y.device, dtype=torch.float32) for l, mul in plan.in1_blocks]
     op = _operands(plan, None, y, w, gs, shared)
     with torch.cuda.device(y.device), _kernel("dtp_grad_x", _dtp_bytes(plan, E, shared, "grad_x")):
-        rc = _lib.load().eqf_dtp_grad_x(plan.handle, ctypes.byref(op), E, _ptr_array(gxs), _stream())
-    _lib.check(rc, "eqf_dtp_grad_x")
+        rc = plan.lib.eqf_dtp_grad_x(plan.handle, ctypes.byref(op), E, _ptr_array(gxs), _stream())
+    _lib.check(rc, "eqf_dtp_grad_x", plan.lib)
     return gxs
 
 
 def _gw_buffer(plan: DtpPlan, E: int, shared: bool, device) -> torch.Tensor:
     if shared:
         # upper bound on the CTAs of whichever kernel runs; rows a launch does not write must read as zero
-        rows = _lib.load().eqf_plan_partial_rows(plan.handle, E)
+        rows = plan.lib.eqf_plan_partial_rows(plan.handle, E)
         return torch.zeros((max(rows, 1), plan.weight_numel), device=device, dtype=torch.float32)
     return torch.empty((E, plan.weight_numel), device=device, dtype=torch.float32)
 
@@ -258,8 +258,8 @@ def dtp_grad_w_raw(plan: DtpPlan, xs, y, gs, shared: bool) -> torch.Tensor:
     gw = _gw_buffer(plan, E, shared, y.device)
     op = _operands(plan, xs, y, None, gs, shared)
     with torch.cuda.device(y.device), _kernel("dtp_grad_w", _dtp_bytes(plan, E, shared, "grad_w")):
-        rc = _lib.load().eqf_dtp_grad_w(plan.handle, ctypes.byref(op), E, ctypes.c_void_p(gw.data_ptr()), _stream())
-    _lib.check(rc, "eqf_dtp_grad_w")
+        rc = plan.lib.eqf_dtp_grad_w(plan.handle, ctypes.byref(op), E, ctypes.c_void_p(gw.data_ptr()), _stream())
+    _lib.check(rc, "eqf_dtp_grad_w", plan.lib)
     return _colsum(gw) if shared else gw
 
 
@@ -270,8 +270,8 @@ def dtp_grad_y_raw(plan: DtpPlan, xs, w, gs, y_like) -> torch.Tensor:
     gy = torch.empty((E, plan.d_y), device=y.device, dtype=torch.float32)
     op = _operands(plan, xs, y, w, gs, shared)
     with torch.cuda.device(y.device), _kernel("dtp_grad_y", _dtp_bytes(plan, E, shared, "grad_y")):
-        rc = _lib.load().eqf_dtp_grad_y(plan.handle, ctypes.byref(op), E, ctypes.c_void_p(gy.data_ptr()), _stream())
-    _lib.check(rc, "eqf_dtp_grad_y")
+        rc = plan.lib.eqf_dtp_grad_y(plan.handle, ctypes.byref(op), E, ctypes.c_void_p(gy.data_ptr()), _stream())
+    _lib.check(rc, "eqf_dtp_grad_y", plan.lib)
     return gy
 
 
@@ -285,9 +285,9 @@ def dtp_grad_xw_raw(plan: DtpPlan, xs, y, w, gs, gather=None, w_offset=None) -> 
     gw = _gw_buffer(plan, E, shared, y.device)
     op = _operands(plan, xs, y, w, gs, shared, gather, w_offset)
     with torch.cuda.device(y.device), _kernel("dtp_grad_xw", _dtp_bytes(plan, E, shared, "grad_xw")):
-        rc = _lib.load().eqf_dtp_grad_xw(plan.handle, ctypes.byref(op), E, _ptr_array(gxs),
+        rc = plan.lib.eqf_dtp_grad_xw(plan.handle, ctypes.byref(op), E, _ptr_array(gxs),
                                          ctypes.c_void_p(gw.data_ptr()), _stream())
-    _lib.check(rc, "eqf_dtp_grad_xw")
+    _lib.check(rc, "eqf_dtp_grad_xw", plan.lib)
     return gxs, (_colsum(gw) if shared else gw)
 
 
@@ -576,7 +576,8 @@ def dtp_linear_supported(plan: DtpPlan) -> bool:
     ok = getattr(plan, "_fused_ok", None)
     if ok is None:
         lib = _lib.load()
-        ok = all(lib.eqf_dtp_linear_supported(plan.handle, g) == 1 for g in range(len(plan.out_groups)))
+        # the fused kernel is built for degrees <= 3 only; a degree-4 plan (libeqf_b200_l4.so) takes the unfused route
+        ok = plan.max_degree <= 3 and all(lib.eqf_dtp_linear_supported(plan.handle, g) == 1 for g in range(len(plan.out_groups)))
         plan._fused_ok = ok
     return ok
 
@@ -2113,22 +2114,23 @@ def edge_geometry_torch(pos, src, dst, lmax: int, offsets=None):
 
 
 def _sh_couplings(device):
+    """A_1, A_2, A_3 of the harmonics recurrence (``o3/sh.py``), as the edge-geometry kernel reads them."""
     from .o3.sh import _coupling_tensor
-    return _coupling_tensor(1, torch.float32, device).contiguous(), _coupling_tensor(2, torch.float32, device).contiguous()
+    return tuple(_coupling_tensor(deg, torch.float32, device).contiguous() for deg in (1, 2, 3))
 
 
 def edge_geom_fwd_raw(pos, graph: "Graph", lmax: int, offsets):
     """(edge_vec [E, 3], length [E], sh [E, (lmax + 1)^2]) of ``pos[src] - pos[dst] (+ offsets)`` (``eqf_edge_geom_fwd``)."""
     pos = _require_cuda(pos, "pos")
     E = graph.n_edges
-    a1, a2 = _sh_couplings(pos.device)
+    a1, a2, a3 = _sh_couplings(pos.device)
     vec = torch.empty((E, 3), device=pos.device, dtype=torch.float32)
     length = torch.empty(E, device=pos.device, dtype=torch.float32)
     sh = torch.empty((E, (lmax + 1) ** 2), device=pos.device, dtype=torch.float32)
     with torch.cuda.device(pos.device), _kernel("edge_geom_fwd", 4 * E * (6 + 4 + (lmax + 1) ** 2)):
         rc = _lib.load().eqf_edge_geom_fwd(pos.data_ptr(), graph.src.data_ptr(), graph.dst.data_ptr(),
                                            offsets.data_ptr() if offsets is not None else None, a1.data_ptr(), a2.data_ptr(),
-                                           E, lmax, vec.data_ptr(), length.data_ptr(), sh.data_ptr(), _stream())
+                                           a3.data_ptr(), E, lmax, vec.data_ptr(), length.data_ptr(), sh.data_ptr(), _stream())
     _lib.check(rc, "eqf_edge_geom_fwd")
     return vec, length, sh
 
@@ -2137,12 +2139,12 @@ def edge_geom_bwd_raw(vec, lmax: int, g_sh, g_len):
     """``[E, 3]`` gradient of the edge vectors from the cotangents of the harmonics and of the length (either may be
     None; ``eqf_edge_geom_bwd``)."""
     E = vec.shape[0]
-    a1, a2 = _sh_couplings(vec.device)
+    a1, a2, a3 = _sh_couplings(vec.device)
     gv = torch.empty((E, 3), device=vec.device, dtype=torch.float32)
     gs = g_sh.contiguous() if g_sh is not None else None
     gl = g_len.contiguous() if g_len is not None else None
     with torch.cuda.device(vec.device), _kernel("edge_geom_bwd", 4 * E * (6 + (lmax + 1) ** 2)):
-        rc = _lib.load().eqf_edge_geom_bwd(vec.data_ptr(), a1.data_ptr(), a2.data_ptr(), E, lmax,
+        rc = _lib.load().eqf_edge_geom_bwd(vec.data_ptr(), a1.data_ptr(), a2.data_ptr(), a3.data_ptr(), E, lmax,
                                            gs.data_ptr() if gs is not None else None,
                                            gl.data_ptr() if gl is not None else None, gv.data_ptr(), _stream())
     _lib.check(rc, "eqf_edge_geom_bwd")
@@ -2182,7 +2184,7 @@ class EdgeGeometry(torch.autograd.Function):
 
 def edge_geometry(pos, graph: "Graph", lmax: int, offsets=None):
     """(edge_vec [E, 3], length [E], sh [E, (lmax + 1)^2]) - fused kernel on CUDA fp32, torch statement otherwise."""
-    if pos.is_cuda and pos.dtype == torch.float32 and lmax <= 3 and graph.n_edges > 0:
+    if pos.is_cuda and pos.dtype == torch.float32 and lmax <= 4 and graph.n_edges > 0:
         return EdgeGeometry.apply(pos, graph, lmax, offsets)
     return edge_geometry_torch(pos, graph.src, graph.dst, lmax, offsets)
 

@@ -108,13 +108,20 @@ class DtpPlan:
         self.cg = np.concatenate(cg_chunks).astype(np.float32)
         self.cg64 = np.concatenate(cg_chunks)
         self.d_y = self.irreps_in2.dim
+        # in1 / output degree 4 runs on libeqf_b200_l4.so (the table-walk kernels built with the degree-4 branches)
+        self.max_degree = max([l for l, _ in self.in1_blocks] + [l for l, _, _ in self.out_groups])
         self._handle = None
 
     # ------------------------------------------------------------------ native handle
     @property
+    def lib(self):
+        """The library whose kernels run this plan (its handle belongs to that library)."""
+        return _lib.load_l4() if self.max_degree > 3 else _lib.load()
+
+    @property
     def handle(self):
         if self._handle is None:
-            lib = _lib.load()
+            lib = self.lib
             n = len(self.paths)
             arr = (_lib.EqfPathDesc * n)()
             for i, p in enumerate(self.paths):
@@ -129,13 +136,13 @@ class DtpPlan:
             rc = lib.eqf_plan_create(arr, n, in1_l, in1_mul, len(self.in1_blocks), out_l, out_mul,
                                      len(self.out_groups), self.d_y, self.weight_numel,
                                      cg.ctypes.data_as(ctypes.POINTER(ctypes.c_float)), cg.size, ctypes.byref(h))
-            _lib.check(rc, "eqf_plan_create")
+            _lib.check(rc, "eqf_plan_create", lib)
             self._handle = h
         return self._handle
 
     def info(self) -> dict:
         out = (ctypes.c_int32 * 13)()
-        _lib.check(_lib.load().eqf_plan_info(self.handle, out, 13), "eqf_plan_info")
+        _lib.check(self.lib.eqf_plan_info(self.handle, out, 13), "eqf_plan_info", self.lib)
         keys = ("n_paths", "m_size", "n_wtasks", "n_xtasks", "tile_edges", "smem_bytes", "blob_words", "weight_numel",
                 "vec_ok", "n_vwtasks", "n_vxtasks", "smem_bytes_vec_fwd", "generated")
         return dict(zip(keys, list(out)))
@@ -153,7 +160,7 @@ class DtpPlan:
         h, self._handle = getattr(self, "_handle", None), None
         if h is not None:
             try:
-                _lib.load().eqf_plan_destroy(h)
+                self.lib.eqf_plan_destroy(h)
             except Exception:
                 pass
 

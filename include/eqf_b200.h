@@ -242,14 +242,16 @@ int eqf_dtp_linear_fwd(const EqfPlan* plan, const EqfEdgeOperands* op, int64_t n
                        const float* Wt, int64_t N, int64_t ldw, float* C, int64_t ldc, float* split, void* stream);
 
 /* Edge geometry in one kernel (nets/graph_attention_transformer.py:866-870; ..._oc20.py:283-296 with `offsets`):
- * vec = pos[src] - pos[dst] (+ offsets), len = |vec|, sh = real spherical harmonics of vec / |vec| up to lmax <= 3 in e3nn's
- * convention ('component' normalisation, y polar), [E][(lmax + 1)^2].  a1 [5][3][3], a2 [7][3][5]: coupling tensors of
- * the recurrence Y_{l+1} = A_l . (x (x) Y_l) (host: equiformer_b200/o3/sh.py).  _bwd: g_vec [E][3] from g_sh / g_len
- * (either may be NULL); the scatter of g_vec to the positions is two segment sums (eqf_attn_aggregate). */
+ * vec = pos[src] - pos[dst] (+ offsets), len = |vec|, sh = real spherical harmonics of vec / |vec| up to lmax <= 4 in e3nn's
+ * convention ('component' normalisation, y polar), [E][(lmax + 1)^2].  a1 [5][3][3], a2 [7][3][5], a3 [9][3][7]: coupling
+ * tensors of the recurrence Y_{l+1} = A_l . (x (x) Y_l) (host: equiformer_b200/o3/sh.py; A_l may be NULL when l >= lmax).
+ * _bwd: g_vec [E][3] from g_sh / g_len (either may be NULL); the scatter of g_vec to the positions is two segment sums
+ * (eqf_attn_aggregate). */
 int eqf_edge_geom_fwd(const float* pos, const int64_t* src, const int64_t* dst, const float* offsets, const float* a1,
-                      const float* a2, int64_t E, int32_t lmax, float* vec, float* len, float* sh, void* stream);
-int eqf_edge_geom_bwd(const float* vec, const float* a1, const float* a2, int64_t E, int32_t lmax, const float* g_sh,
-                      const float* g_len, float* g_vec, void* stream);
+                      const float* a2, const float* a3, int64_t E, int32_t lmax, float* vec, float* len, float* sh,
+                      void* stream);
+int eqf_edge_geom_bwd(const float* vec, const float* a1, const float* a2, const float* a3, int64_t E, int32_t lmax,
+                      const float* g_sh, const float* g_len, float* g_vec, void* stream);
 /* ExpNormalSmearing of the MD17 models (nets/expnorm_rbf.py:73-78 with CosineCutoff(0, cutoff_upper) :11-33):
  * out[e][b] = cutoff(d_e) exp(-betas[b] (exp(-alpha d_e) - means[b])^2); _bwd returns d/d d_e of <g, out>. */
 int eqf_expnorm_fwd(const float* dist, const float* means, const float* betas, float alpha, float cutoff_upper, int64_t E,
