@@ -23,6 +23,11 @@ LIB_PATH = PKG_DIR / "libeqf_b200.so"
 # -DEQF_MAX_DEGREE=4, so that the degree-4 branches stay out of the kernels of the main library
 L4_LIB_PATH = PKG_DIR / "libeqf_b200_l4.so"
 L4_SOURCES = ("eqf_abi.cu", "eqf_dtp.cu", "eqf_dtp_vec.cu")
+# the per-graph equivariant norms (EquivariantGraphNorm / EquivariantInstanceNorm): their own library and header
+# (include/eqf_b200_norm.h), bound by load_norm()
+NORM_LIB_PATH = PKG_DIR / "libeqf_b200_norm.so"
+NORM_SOURCES = ("eqf_norm.cu",)
+EQF_NORM_MAX_ENTRIES = 8      # include/eqf_b200_norm.h: irreps entries per norm layout
 SOURCES = ("eqf_abi.cu", "eqf_dtp.cu", "eqf_dtp_vec.cu", "eqf_attn.cu", "eqf_pointwise.cu", "eqf_gemm_tf32x3.cu", "eqf_graph.cu",
            "eqf_fused.cu", "eqf_edge.cu", "eqf_gemm_small.cu")
 
@@ -74,6 +79,19 @@ class EqfNormLayout(ctypes.Structure):
         ("mul", c_int32 * EQF_MAX_BLOCKS),
         ("d", c_int32 * EQF_MAX_BLOCKS),
         ("is_scalar", c_int32 * EQF_MAX_BLOCKS),
+        ("eps", c_float),
+    ]
+
+
+class EqfSegNormLayout(ctypes.Structure):
+    _fields_ = [
+        ("n_entries", c_int32),
+        ("mul", c_int32 * EQF_NORM_MAX_ENTRIES),
+        ("d", c_int32 * EQF_NORM_MAX_ENTRIES),
+        ("is_scalar", c_int32 * EQF_NORM_MAX_ENTRIES),
+        ("w_off", c_int32 * EQF_NORM_MAX_ENTRIES),
+        ("s_off", c_int32 * EQF_NORM_MAX_ENTRIES),
+        ("n_w", c_int32), ("n_s", c_int32), ("component", c_int32),
         ("eps", c_float),
     ]
 
@@ -189,6 +207,17 @@ SIGNATURES = {
                                       c_void_p]),
 }
 
+# every symbol include/eqf_b200_norm.h declares
+NORM_SIGNATURES = {
+    "eqf_last_error": (c_char_p, []),
+    "eqf_norm_graph_ptr": (c_int32, [c_void_p, c_int64, c_int64, c_void_p, c_void_p]),
+    "eqf_norm_fwd": (c_int32, [POINTER(EqfSegNormLayout), POINTER(c_void_p), c_void_p, c_int64, c_void_p, c_void_p,
+                               c_void_p, POINTER(c_void_p), c_void_p, c_void_p, c_void_p]),
+    "eqf_norm_bwd": (c_int32, [POINTER(EqfSegNormLayout), POINTER(c_void_p), POINTER(c_void_p), c_void_p, c_int64,
+                               c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_void_p), c_void_p, c_void_p]),
+    "eqf_norm_param_reduce": (c_int32, [c_void_p, c_int64, c_int32, c_void_p, c_void_p]),
+}
+
 
 class EqfError(RuntimeError):
     pass
@@ -210,16 +239,19 @@ def generate_sources():
 
 
 def needs_build() -> bool:
-    if not LIB_PATH.exists() or not L4_LIB_PATH.exists():
+    libs = (LIB_PATH, L4_LIB_PATH, NORM_LIB_PATH)
+    if not all(p.exists() for p in libs):
         return True
-    mtime = min(LIB_PATH.stat().st_mtime, L4_LIB_PATH.stat().st_mtime)
-    deps = sources() + list(CSRC_DIR.glob("*.cuh")) + [INCLUDE_DIR / "eqf_b200.h"]
+    mtime = min(p.stat().st_mtime for p in libs)
+    deps = (sources() + [CSRC_DIR / s for s in NORM_SOURCES] + list(CSRC_DIR.glob("*.cuh"))
+            + [INCLUDE_DIR / "eqf_b200.h", INCLUDE_DIR / "eqf_b200_norm.h"])
     return any(p.stat().st_mtime > mtime for p in deps)
 
 
 def build(force: bool = False, verbose: bool = False) -> Path:
-    """Compile ``csrc/*.cu`` for sm_90a into ``equiformer_b200/libeqf_b200.so`` and ``L4_SOURCES`` with
-    ``-DEQF_MAX_DEGREE=4`` into ``equiformer_b200/libeqf_b200_l4.so`` (in-tree)."""
+    """Compile ``csrc/*.cu`` for sm_90a into ``equiformer_b200/libeqf_b200.so``, ``L4_SOURCES`` with
+    ``-DEQF_MAX_DEGREE=4`` into ``equiformer_b200/libeqf_b200_l4.so`` and ``NORM_SOURCES`` into
+    ``equiformer_b200/libeqf_b200_norm.so`` (in-tree)."""
     generate_sources()
     if not force and not needs_build():
         return LIB_PATH
@@ -232,7 +264,8 @@ def build(force: bool = False, verbose: bool = False) -> Path:
     obj_dir = PKG_DIR / "build" / ("obj%d" % os.getpid())
     obj_dir.mkdir(parents=True, exist_ok=True)
     compile_flags = [f for f in NVCC_FLAGS if f != "--shared"]
-    jobs = [(src, "", []) for src in sources()] + [(CSRC_DIR / s, "_l4", ["-DEQF_MAX_DEGREE=4"]) for s in L4_SOURCES]
+    jobs = ([(src, "", []) for src in sources()] + [(CSRC_DIR / s, "_l4", ["-DEQF_MAX_DEGREE=4"]) for s in L4_SOURCES]
+            + [(CSRC_DIR / s, "_norm", []) for s in NORM_SOURCES])
 
     def compile_one(job):
         src, suffix, defines = job
@@ -260,6 +293,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
                 print(proc.stderr)
         link(LIB_PATH, [o for o, suffix, _ in results if suffix == ""])
         link(L4_LIB_PATH, [o for o, suffix, _ in results if suffix == "_l4"])
+        link(NORM_LIB_PATH, [o for o, suffix, _ in results if suffix == "_norm"])
     finally:
         shutil.rmtree(obj_dir, ignore_errors=True)
     return LIB_PATH
@@ -296,6 +330,27 @@ def load_l4():
                 raise EqfError(f"{L4_LIB_PATH.name} does not export eqf_dtp_forward; rebuild it")
             _lib_l4 = lib
     return _lib_l4
+
+
+_lib_norm = None
+
+
+def load_norm():
+    """Return the loaded norm library (``include/eqf_b200_norm.h``)."""
+    global _lib_norm
+    with _lock:
+        if _lib_norm is None:
+            if not NORM_LIB_PATH.exists():
+                raise EqfError(f"{NORM_LIB_PATH} is missing: run `python -c 'import __graft_entry__ as g; g.build()'`")
+            lib = ctypes.CDLL(str(NORM_LIB_PATH))
+            for name, (restype, argtypes) in NORM_SIGNATURES.items():
+                try:
+                    fn = getattr(lib, name)
+                except AttributeError as exc:
+                    raise EqfError(f"{NORM_LIB_PATH.name} does not export {name}; rebuild it") from exc
+                fn.restype, fn.argtypes = restype, argtypes
+            _lib_norm = lib
+    return _lib_norm
 
 
 def load():

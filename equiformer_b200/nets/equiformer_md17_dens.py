@@ -21,7 +21,9 @@ from .drop import EquivariantDropout
 from .fast_activation import Activation
 from .gaussian_rbf import GaussianRadialBasisLayer
 from .graph_attention_transformer import (_run_blocks, edge_features, EdgeDegreeEmbeddingNetwork, GraphAttention,
-                                          NodeEmbeddingNetwork, ScaledScatter, TransBlock, get_norm_layer, radial_basis)
+                                          NodeEmbeddingNetwork, ScaledScatter, TransBlock, get_norm_layer, norm_segments,
+                                          radial_basis)
+from .graph_norm import EquivariantGraphNorm
 from .layer_norm import EquivariantLayerNormV2
 from .registry import register_model
 from .tensor_product_rescale import LinearRS
@@ -106,8 +108,8 @@ class Equiformer_MD17_DeNS(torch.nn.Module):
     def no_weight_decay(self):
         skip = set()
         for mod_name, mod in self.named_modules():
-            if isinstance(mod, (torch.nn.Linear, torch.nn.LayerNorm, EquivariantLayerNormV2, GaussianRadialBasisLayer,
-                                RadialBasis)):
+            if isinstance(mod, (torch.nn.Linear, torch.nn.LayerNorm, EquivariantLayerNormV2, EquivariantGraphNorm,
+                                GaussianRadialBasisLayer, RadialBasis)):
                 for p_name, _ in mod.named_parameters():
                     if isinstance(mod, torch.nn.Linear) and "weight" in p_name:
                         continue
@@ -174,9 +176,10 @@ class Equiformer_MD17_DeNS(torch.nn.Module):
                                    device=node_features.device, dtype=node_features.dtype)
         node_features = node_features + self.force_embed(force_sh)
 
+        seg = norm_segments(self, batch, n_graphs)
         node_features = _run_blocks(self.blocks, node_features, self.irreps_node_embedding, node_attr, edge_src, edge_dst,
-                                    edge_sh, edge_length_embedding, batch, graph, n_graphs)
-        node_features = self.norm(node_features, batch=batch)
+                                    edge_sh, edge_length_embedding, batch, graph, **seg)
+        node_features = self.norm(node_features, batch=batch, **seg)
         if self.out_dropout is not None:
             node_features = self.out_dropout(node_features)
 

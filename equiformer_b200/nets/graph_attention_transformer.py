@@ -28,7 +28,10 @@ from .bessel_rbf import RadialBasis
 from .drop import EquivariantDropout, GraphDropPath
 from .expnorm_rbf import ExpNormalSmearing
 from .fast_activation import Activation, Gate
+from .fast_layer_norm import EquivariantLayerNormFast
 from .gaussian_rbf import GaussianRadialBasisLayer
+from .graph_norm import EquivariantGraphNorm
+from .instance_norm import EquivariantInstanceNorm
 from .layer_norm import EquivariantLayerNormV2
 from .radial_func import RadialProfile, clear_hoisted, hoist_first_layers
 from .registry import register_model
@@ -46,12 +49,16 @@ _AVG_DEGREE = 15.57930850982666
 
 
 def get_norm_layer(norm_type):
+    if norm_type == "graph":
+        return EquivariantGraphNorm
+    if norm_type == "instance":
+        return EquivariantInstanceNorm
     if norm_type == "layer":
         return EquivariantLayerNormV2
+    if norm_type == "fast_layer":
+        return EquivariantLayerNormFast
     if norm_type is None:
         return None
-    if norm_type in ("graph", "instance", "fast_layer"):
-        raise NotImplementedError(f"norm '{norm_type}' is not used by any shipped Equiformer config (out of scope)")
     raise ValueError(f"Norm type {norm_type} not supported.")
 
 
@@ -578,15 +585,16 @@ class TransBlock(torch.nn.Module):
         return getattr(self, self._attn_name)
 
     def forward(self, node_input, node_attr, edge_src, edge_dst, edge_attr, edge_scalars, batch, **kwargs):
-        features = self.norm_1(node_input, batch=batch)
+        n_graphs = kwargs.get("n_graphs")
+        seg = _norm_segments(kwargs)
+        features = self.norm_1(node_input, batch=batch, **seg)
         features = self.attention(node_input=features, node_attr=node_attr, edge_src=edge_src, edge_dst=edge_dst,
                                   edge_attr=edge_attr, edge_scalars=edge_scalars, batch=batch, **kwargs)
-        n_graphs = kwargs.get("n_graphs")
         if self.drop_path is not None:
             features = self._drop_path(features, batch, n_graphs)
         node_output = node_input + features
 
-        features = self.ffn(self.norm_2(node_output, batch=batch), node_attr)
+        features = self.ffn(self.norm_2(node_output, batch=batch, **seg), node_attr)
         if self.ffn_shortcut is not None:
             node_output = self.ffn_shortcut(node_output, node_attr)
         if self.drop_path is not None:
@@ -611,10 +619,11 @@ class TransBlock(torch.nn.Module):
     def forward_planar(self, xs, node_attr, edge_src, edge_dst, edge_attr, edge_scalars, batch, **kwargs):
         """``forward`` on planar node blocks -> planar node blocks: the features never pass through the e3nn layout
         (saves the layout copies at every sub-layer boundary, ~24 small launches per block and step)."""
-        f = self.attention.forward_planar(self.norm_1.planar(xs), node_attr, edge_src, edge_dst, edge_attr, edge_scalars,
-                                          batch, **kwargs)
+        seg = _norm_segments(kwargs)
+        f = self.attention.forward_planar(self.norm_1.planar(xs, batch=batch, **seg), node_attr, edge_src, edge_dst,
+                                          edge_attr, edge_scalars, batch, **kwargs)
         xs = self._residual(xs, f, batch, kwargs.get("n_graphs"))
-        f = self.ffn.forward_planar(self.norm_2.planar(xs), node_attr)
+        f = self.ffn.forward_planar(self.norm_2.planar(xs, batch=batch, **seg), node_attr)
         return self._residual(xs, f, batch, kwargs.get("n_graphs"))
 
     def _residual(self, xs, f, batch, n_graphs):
@@ -624,6 +633,12 @@ class TransBlock(torch.nn.Module):
             return [a + b for a, b in zip(xs, f)]
         s = self.drop_path.node_scale(f[0], batch, n_graphs)
         return [torch.addcmul(a, b, s) for a, b in zip(xs, f)]
+
+
+def _norm_segments(kwargs) -> dict:
+    """The batch's graph count and, when the blocks were handed them, the graphs' first nodes (the per-graph norms read
+    them; the layer norms ignore them)."""
+    return {k: kwargs[k] for k in ("n_graphs", "graph_ptr") if kwargs.get(k) is not None}
 
 
 class NodeEmbeddingNetwork(torch.nn.Module):
@@ -770,8 +785,8 @@ class GraphAttentionTransformer(torch.nn.Module):
         skip = set()
         names = {n for n, _ in self.named_parameters()}
         for mod_name, mod in self.named_modules():
-            if isinstance(mod, (torch.nn.Linear, torch.nn.LayerNorm, EquivariantLayerNormV2, GaussianRadialBasisLayer,
-                                RadialBasis)):
+            if isinstance(mod, (torch.nn.Linear, torch.nn.LayerNorm, EquivariantLayerNormV2, EquivariantGraphNorm,
+                                GaussianRadialBasisLayer, RadialBasis)):
                 for p_name, _ in mod.named_parameters():
                     if isinstance(mod, torch.nn.Linear) and "weight" in p_name:
                         continue
@@ -811,11 +826,12 @@ class GraphAttentionTransformer(torch.nn.Module):
             node_features = atom_embedding + edge_degree_embedding
             node_attr = torch.ones_like(node_features.narrow(1, 0, 1))
             node_attr._eqf_all_ones = True          # lets the node-level FCTPs skip the multiply by the constant 1
+            seg = norm_segments(self, batch, n_graphs)
             node_features = _run_blocks(self.blocks, node_features, self.irreps_node_embedding, node_attr, edge_src, edge_dst,
-                                        edge_sh, edge_length_embedding, batch, graph, n_graphs)
+                                        edge_sh, edge_length_embedding, batch, graph, **seg)
         finally:
             clear_hoisted(served)
-        node_features = self.norm(node_features, batch=batch)
+        node_features = self.norm(node_features, batch=batch, **seg)
         if self.out_dropout is not None:
             node_features = self.out_dropout(node_features)
         outputs = self.head(node_features)
@@ -862,14 +878,30 @@ def hoist_radial(model, edge_scalars):
     return hoist_first_layers(mods, edge_scalars)
 
 
+def norm_segments(model, batch, n_graphs=None) -> dict:
+    """The keyword arguments the norms of ``model`` take besides ``batch``: ``n_graphs`` (when known) and, when the
+    model has a per-graph norm and ``batch`` lives on the GPU, the graphs' first nodes ``graph_ptr``.  These are built
+    once per forward, on the device (no host read when ``n_graphs`` is given), and shared by every norm of the model."""
+    per_graph = model.__dict__.get("_per_graph_norm")
+    if per_graph is None:
+        per_graph = any(isinstance(m, EquivariantGraphNorm) for m in model.modules())
+        model.__dict__["_per_graph_norm"] = per_graph
+    if not (per_graph and batch is not None and batch.is_cuda):
+        return {} if n_graphs is None else {"n_graphs": n_graphs}
+    segments = ops.GraphSegments(batch, n_graphs)
+    return {"n_graphs": segments.n_graphs, "graph_ptr": segments.ptr}
+
+
 def _run_blocks(blocks, node_features, irreps, node_attr, edge_src, edge_dst, edge_sh, edge_scalars, batch, graph,
-                n_graphs=None):
+                n_graphs=None, graph_ptr=None):
     """The transformer blocks; consecutive blocks that support it keep the node features in planar blocks.  ``n_graphs``
-    lets stochastic depth draw its per-graph factors without reading the batch vector on the host."""
+    lets stochastic depth draw its per-graph factors without reading the batch vector on the host; ``graph_ptr``
+    (``norm_segments``) is handed to every block's norms."""
     planar = None
+    seg = {} if graph_ptr is None else {"graph_ptr": graph_ptr}
     for blk in blocks:
         kw = dict(node_attr=node_attr, edge_src=edge_src, edge_dst=edge_dst, edge_attr=edge_sh, edge_scalars=edge_scalars,
-                  batch=batch, graph=graph, n_graphs=n_graphs)
+                  batch=batch, graph=graph, n_graphs=n_graphs, **seg)
         if getattr(blk, "supports_planar", False) and ops.fused_ok(node_features if planar is None else planar[0]):
             if planar is None:
                 planar = ops.to_planar(node_features, Irreps(irreps))

@@ -15,7 +15,8 @@ from .drop import EquivariantDropout
 from .fast_activation import Activation
 from .gaussian_rbf import GaussianRadialBasisLayer
 from .graph_attention_transformer import (_run_blocks, edge_features, EdgeDegreeEmbeddingNetwork, GraphAttention, NodeEmbeddingNetwork,
-                                          ScaledScatter, TransBlock, get_norm_layer, radial_basis)
+                                          ScaledScatter, TransBlock, get_norm_layer, norm_segments, radial_basis)
+from .graph_norm import EquivariantGraphNorm
 from .layer_norm import EquivariantLayerNormV2
 from .registry import register_model
 from .tensor_product_rescale import LinearRS
@@ -102,8 +103,8 @@ class GraphAttentionTransformerMD17(torch.nn.Module):
     def no_weight_decay(self):
         skip = set()
         for mod_name, mod in self.named_modules():
-            if isinstance(mod, (torch.nn.Linear, torch.nn.LayerNorm, EquivariantLayerNormV2, GaussianRadialBasisLayer,
-                                RadialBasis)):
+            if isinstance(mod, (torch.nn.Linear, torch.nn.LayerNorm, EquivariantLayerNormV2, EquivariantGraphNorm,
+                                GaussianRadialBasisLayer, RadialBasis)):
                 for p_name, _ in mod.named_parameters():
                     if isinstance(mod, torch.nn.Linear) and "weight" in p_name:
                         continue
@@ -131,9 +132,10 @@ class GraphAttentionTransformerMD17(torch.nn.Module):
         node_features = atom_embedding + edge_degree_embedding
         node_attr = torch.ones_like(node_features.narrow(1, 0, 1))
         node_attr._eqf_all_ones = True
+        seg = norm_segments(self, batch, n_graphs)
         node_features = _run_blocks(self.blocks, node_features, self.irreps_node_embedding, node_attr, edge_src, edge_dst,
-                                    edge_sh, edge_length_embedding, batch, graph, n_graphs)
-        node_features = self.norm(node_features, batch=batch)
+                                    edge_sh, edge_length_embedding, batch, graph, **seg)
+        node_features = self.norm(node_features, batch=batch, **seg)
         if self.out_dropout is not None:
             node_features = self.out_dropout(node_features)
         if self.use_attn_head:

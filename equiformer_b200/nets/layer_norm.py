@@ -42,8 +42,9 @@ class EquivariantLayerNormV2(nn.Module):
     def supports_planar(self) -> bool:
         return self._layout is not None
 
-    def planar(self, xs):
-        """The same normalisation on planar blocks (one ``[N, 2l+1, mul]`` tensor per irreps entry)."""
+    def planar(self, xs, **kwargs):
+        """The same normalisation on planar blocks (one ``[N, 2l+1, mul]`` tensor per irreps entry); the per-graph
+        arguments the transformer blocks hand every norm (``batch``, ``n_graphs``, ``graph_ptr``) are not used."""
         if self._layout is None:
             raise NotImplementedError("planar LayerNorm needs the affine 'component' configuration")
         return ops.equivariant_layer_norm_planar(self._layout, xs, self.affine_weight, self.affine_bias)

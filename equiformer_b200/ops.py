@@ -2042,6 +2042,104 @@ def equivariant_layer_norm_planar(lay: NormLayout, xs, w, b):
     return eln_planar_torch(lay, list(xs), w, b)
 
 
+# ----------------------------------------------------------------------------- per-graph equivariant norms
+
+
+def segment_norm_torch(lay, fields, batch, n_graphs: int, w, b, shift, reduce: str = "mean"):
+    """Torch statement of EquivariantGraphNorm / EquivariantInstanceNorm (ref nets/graph_norm.py:57-134,
+    nets/instance_norm.py:56-134) on ``fields``, one ``[N, mul, 2l+1]`` tensor per entry of ``lay``
+    (``norm_kernels.SegNormLayout``).  ``w`` / ``b`` None: no affine; ``shift`` None: the instance norm (no mean shift).
+    Graphs are ``batch`` values ``0 .. n_graphs-1``; a graph without nodes has mean and square mean 0."""
+    G = int(n_graphs)
+    like = fields[0]
+    count = torch.zeros(G, dtype=like.dtype, device=like.device).index_add_(
+        0, batch, torch.ones(batch.shape[0], dtype=like.dtype, device=like.device)).clamp_(min=1)
+    out, iw, ib = [], 0, 0
+    for (mul, d, scalar), f in zip(lay.entries, fields):
+        if scalar:
+            mean = f.new_zeros((G, mul, d)).index_add(0, batch, f) / count.view(-1, 1, 1)
+            if shift is not None:
+                mean = mean * shift[:mul].reshape(1, mul, 1)
+            f = f - mean[batch]
+        sq = f.pow(2)
+        per_node = sq.mean(-1) if lay.component else sq.sum(-1)
+        if reduce == "mean":
+            v = f.new_zeros((G, mul)).index_add(0, batch, per_node) / count.view(-1, 1)
+        else:
+            v = f.new_zeros((G, mul)).scatter_reduce(0, batch.view(-1, 1).expand_as(per_node), per_node, "amax",
+                                                      include_self=False)
+        scale = (v + lay.eps).pow(-0.5)
+        if w is not None:
+            scale = scale * w[None, iw:iw + mul]
+            iw += mul
+        f = f * scale[batch].unsqueeze(-1)
+        if w is not None and scalar:
+            f = f + b[ib:ib + mul].reshape(mul, 1)
+            ib += mul
+        out.append(f)
+    return out
+
+
+def segment_norm_planar_torch(lay, xs, batch, n_graphs: int, w, b, shift, reduce: str = "mean"):
+    """:func:`segment_norm_torch` on planar blocks ``[N, 2l+1, mul]``."""
+    ys = segment_norm_torch(lay, [x.transpose(1, 2) for x in xs], batch, n_graphs, w, b, shift, reduce)
+    return [y.transpose(1, 2).contiguous() for y in ys]
+
+
+class GraphSegments:
+    """The graphs of a batch: ``batch`` (ascending node -> graph), ``n_graphs`` and ``ptr[n_graphs + 1]`` (first node of
+    each graph), built on the device without a host read when ``n_graphs`` is given."""
+
+    def __init__(self, batch: torch.Tensor, n_graphs: Optional[int] = None, ptr: Optional[torch.Tensor] = None):
+        if n_graphs is None:
+            n_graphs = int(batch.max()) + 1 if batch.numel() else 0
+        self.batch, self.n_graphs = batch, int(n_graphs)
+        if ptr is None and batch.is_cuda:
+            from . import norm_kernels
+            ptr = norm_kernels.graph_ptr_raw(batch, self.n_graphs)
+        elif ptr is None:
+            ptr = torch.searchsorted(batch, torch.arange(self.n_graphs + 1, device=batch.device, dtype=batch.dtype))
+        self.ptr = ptr
+
+
+class SegmentNorm(torch.autograd.Function):
+    """Per-graph norm on planar blocks: apply(lay, segments, w, b, shift, *xs) with ``shift`` None for the instance norm.
+    First order: the norm library's forward and backward kernels; under ``create_graph`` the backward is rebuilt from
+    :func:`segment_norm_planar_torch` on the saved inputs."""
+
+    @staticmethod
+    def forward(ctx, lay, seg: GraphSegments, w, b, shift, *xs):
+        from . import norm_kernels
+        xs = [x.contiguous() for x in xs]
+        ys, mean, rstd = norm_kernels.norm_fwd_raw(lay, xs, seg.ptr, seg.n_graphs, shift, w, b)
+        ctx.lay, ctx.seg = lay, seg
+        ctx.save_for_backward(w, b, shift, mean, rstd, *xs)
+        return tuple(ys)
+
+    @staticmethod
+    def backward(ctx, *gys):
+        from . import norm_kernels
+        w, b, shift, mean, rstd, *xs = ctx.saved_tensors
+        seg = ctx.seg
+        gys = [g if g is not None else torch.zeros_like(x) for g, x in zip(gys, xs)]
+        if torch.is_grad_enabled():
+            fn = lambda ww, bb, ss, *blocks: tuple(segment_norm_planar_torch(ctx.lay, list(blocks), seg.batch,
+                                                                             seg.n_graphs, ww, bb, ss))
+            grads = _higher_order_grads(fn, (w, b, shift, *xs), gys)
+            return (None, None, *grads)
+        gxs, gw, gb, gs = norm_kernels.norm_bwd_raw(ctx.lay, xs, [g.contiguous() for g in gys], seg.ptr, seg.n_graphs,
+                                                    shift, w, mean, rstd)
+        return (None, None, gw, gb, gs, *gxs)
+
+
+def segment_norm_planar(lay, xs, seg: GraphSegments, w, b, shift, reduce: str = "mean"):
+    """EquivariantGraphNorm / EquivariantInstanceNorm on planar blocks: the kernels for the affine 'mean' norms of at most
+    8 entries, the torch statement for the rest (``reduce='max'``, no affine) and for other devices and dtypes."""
+    if w is not None and reduce == "mean" and lay.c is not None and fused_ok(xs[0]):
+        return list(SegmentNorm.apply(lay, seg, w, b, shift, *xs))
+    return segment_norm_planar_torch(lay, list(xs), seg.batch, seg.n_graphs, w, b, shift, reduce)
+
+
 def gaussian_rbf_torch(dist, mean, std, weight, bias, cutoff: float):
     """Torch statement of GaussianRadialBasisLayer.forward (ref nets/gaussian_rbf.py:5-40, truncated pi included)."""
     x = weight * (dist / cutoff).unsqueeze(-1) + bias
