@@ -25,58 +25,19 @@ import torch
 from oracle import equiformer_ref as R
 from tests import oracle_bessel as OB
 from tests.helpers import rel_err
+from tests.reference_fixtures import GOLDEN, load, mirror, oracle_config, run_mirror, worst_grad
 
-GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
-FIXTURE = os.path.join(GOLDEN, "reference_model_bessel_small.npz")
+FIXTURE = "reference_model_bessel_small.npz"
 SHAPES = os.path.join(GOLDEN, "reference_state_shapes_bessel.json")
 TOL = 2e-5          # kernel vs fp64
 TOL_FREQ = 5e-5     # frequency gradient: a sum over all edges
 _POINTWISE_CTAS = 132 * 8   # eqf_pointwise.cu pointwise_grid: min(ceil(E / 8), 132 * 8) CTAs of 8 warps, one edge per warp
 
 
-@pytest.fixture(scope="module")
-def gold():
-    return np.load(FIXTURE)
-
-
-def _part(g, prefix):
-    head = f"{prefix}/"
-    return {k[len(head):]: g[k] for k in g.files if k.startswith(head)}
-
-
-def _cfg(p, basis_md17: bool):
-    return R.Config(irreps_node_embedding=str(p["cfg/irreps_node_embedding"]), irreps_sh=str(p["cfg/irreps_sh"]),
-                    irreps_head=str(p["cfg/irreps_head"]), irreps_mlp_mid=str(p["cfg/irreps_mlp_mid"]),
-                    irreps_feature=str(p["cfg/irreps_feature"]), num_heads=int(p["cfg/num_heads"]),
-                    num_layers=int(p["cfg/num_layers"]), max_radius=float(p["cfg/max_radius"]),
-                    number_of_basis=int(p["cfg/number_of_basis"]), basis_type="bessel",
-                    nonlinear_message=bool(p["cfg/nonlinear_message"]),
-                    **(dict(max_atom_type=64, qm9_atom_remap=False) if basis_md17 else {}))
-
-
-def _state(p):
-    return {k[len("state/"):]: torch.from_numpy(v) for k, v in p.items() if k.startswith("state/")}
-
-
-def _mirror(p, cls):
-    cfg = {k[len("cfg/"):]: v for k, v in p.items() if k.startswith("cfg/")}
-    kw = {k: (str(v) if v.dtype.kind in "US" else bool(v) if v.dtype.kind == "b" else
-              [int(c) for c in v] if v.ndim == 1 else int(v) if v.dtype.kind == "i" else float(v)) for k, v in cfg.items()}
-    model = cls(**kw)
-    res = model.load_state_dict(_state(p), strict=False)
-    assert not res.unexpected_keys and all(k.endswith("tp.output_mask") for k in res.missing_keys), res
-    return model.eval()
-
-
-def _worst_grad(got: dict, p, n_min: int):
-    keys = [k[len("grad/"):] for k in p if k.startswith("grad/")]
-    assert len(keys) >= n_min and "rbf.rbf.frequencies" in keys
-    worst = 0.0
-    for k in keys:
-        ref = torch.from_numpy(p[f"grad/{k}"])
-        assert got[k] is not None, k
-        worst = max(worst, float((got[k].detach().double().cpu() - ref).abs().max() / ref.abs().max().clamp_min(1e-12)))
-    return worst
+def _part(prefix):
+    case = load(FIXTURE, prefix)
+    assert "rbf.rbf.frequencies" in case.grads
+    return case
 
 
 def _envelope(x):
@@ -120,37 +81,40 @@ def test_zero_distance_gives_nan_as_the_reference():
 
 # ------------------------------------------------------------------------------------------------ fixture (CPU)
 
-def test_module_matches_reference_restatement(gold):
+def test_module_matches_reference_restatement():
     from equiformer_b200.nets.bessel_rbf import RadialBasis
+    case = load(FIXTURE, "module")
     m = RadialBasis(128, 5.0, rbf={"name": "spherical_bessel"})
     assert [k for k, _ in m.named_parameters()] == ["rbf.frequencies"]
     assert torch.equal(m.rbf.frequencies.detach(), torch.tensor(np.pi * np.arange(1, 129, dtype=np.float32)))
-    m.load_state_dict({"rbf.frequencies": torch.from_numpy(gold["module/state/rbf.frequencies"])})
-    out = m.double()(torch.from_numpy(gold["module/dist"]).double())
-    assert rel_err(out, torch.from_numpy(gold["module/y"])) < 1e-12
-    p = {"m.rbf.frequencies": torch.from_numpy(gold["module/state/rbf.frequencies"]).double()}
-    assert rel_err(OB.bessel_rbf(p, "m", torch.from_numpy(gold["module/dist"]).double(), 5.0), torch.from_numpy(gold["module/y"])) < 1e-12
+    m.load_state_dict(case.state)
+    out = m.double()(case.t("dist", dtype=torch.float64))
+    assert rel_err(out, case.t("y")) < 1e-12
+    p = {"m.rbf.frequencies": case.state["rbf.frequencies"].double()}
+    assert rel_err(OB.bessel_rbf(p, "m", case.t("dist", dtype=torch.float64), 5.0), case.t("y")) < 1e-12
 
 
-def test_oracle_qm9_bessel_model_matches_reference(gold):
-    p = _part(gold, "qm9")
-    params = {k: v.double().requires_grad_(True) if v.is_floating_point() else v for k, v in _state(p).items()}
-    pos, batch, z = torch.from_numpy(p["pos"]).double(), torch.from_numpy(p["batch"]), torch.from_numpy(p["z"])
-    energy = OB.model_forward_bessel(params, _cfg(p, False), pos, batch, z, n_graphs=2)
-    assert rel_err(energy.detach(), torch.from_numpy(p["energy"])) < 1e-11
+def test_oracle_qm9_bessel_model_matches_reference():
+    p = _part("qm9")
+    params = {k: v.double().requires_grad_(True) if v.is_floating_point() else v for k, v in p.state.items()}
+    pos, batch, z = p.t("pos", dtype=torch.float64), p.t("batch"), p.t("z")
+    ocfg = oracle_config("qm9", p.cfg, basis_type="bessel")
+    energy = OB.model_forward_bessel(params, ocfg, pos, batch, z, n_graphs=2)
+    assert rel_err(energy.detach(), p.t("energy")) < 1e-11
     (energy ** 2).sum().backward()
-    assert _worst_grad({k: v.grad for k, v in params.items()}, p, 80) < 1e-8
+    assert worst_grad({k: v.grad for k, v in params.items()}, p.grads, 80) < 1e-8
 
 
-def test_oracle_md17_bessel_model_matches_reference(gold):
-    p = _part(gold, "md17")
-    params = {k: v.double().requires_grad_(True) if v.is_floating_point() else v for k, v in _state(p).items()}
-    pos, batch, z = torch.from_numpy(p["pos"]).double(), torch.from_numpy(p["batch"]), torch.from_numpy(p["z"])
-    e, f = OB.energy_and_forces_bessel(params, _cfg(p, True), pos, batch, z, 1, create_graph=True)
-    assert rel_err(e.detach(), torch.from_numpy(p["energy"])) < 1e-11
-    assert rel_err(f.detach(), torch.from_numpy(p["forces"])) < 1e-10
+def test_oracle_md17_bessel_model_matches_reference():
+    p = _part("md17")
+    params = {k: v.double().requires_grad_(True) if v.is_floating_point() else v for k, v in p.state.items()}
+    pos, batch, z = p.t("pos", dtype=torch.float64), p.t("batch"), p.t("z")
+    ocfg = oracle_config("md17", p.cfg, basis_type="bessel")
+    e, f = OB.energy_and_forces_bessel(params, ocfg, pos, batch, z, 1, create_graph=True)
+    assert rel_err(e.detach(), p.t("energy")) < 1e-11
+    assert rel_err(f.detach(), p.t("forces")) < 1e-10
     (e.sum() + (f ** 2).sum()).backward()
-    assert _worst_grad({k: v.grad for k, v in params.items()}, p, 80) < 1e-8
+    assert worst_grad({k: v.grad for k, v in params.items()}, p.grads, 80) < 1e-8
 
 
 def _bessel_fwd_emulated(dist, freq, cutoff):
@@ -195,28 +159,25 @@ def test_bessel_rbf_gradcheck_through_emulated_launch():
         assert out.grad_fn is not None and "BesselRbf" in type(out.grad_fn).__name__
 
 
-def test_mirror_models_match_reference_on_host(gold):
+def test_mirror_models_match_reference_on_host():
     """The mirrors' own wiring with the kernel launches emulated in float64: QM9 energies + gradients of sum(E^2); MD17
     energy, forces and gradients of the energy + force loss."""
     from equiformer_b200.nets.graph_attention_transformer import GraphAttentionTransformer
     from equiformer_b200.nets.graph_attention_transformer_md17 import GraphAttentionTransformerMD17
-    p = _part(gold, "qm9")
-    model = _mirror(p, GraphAttentionTransformer).double()
+    p = _part("qm9")
+    model = mirror(GraphAttentionTransformer, p.cfg, p.state).double()
     with _emulated():
-        energy = model(f_in=None, pos=torch.from_numpy(p["pos"]).double(), batch=torch.from_numpy(p["batch"]),
-                       node_atom=torch.from_numpy(p["z"]))
-        (energy ** 2).sum().backward()
-    assert rel_err(energy.detach(), torch.from_numpy(p["energy"])) < 1e-10
-    assert _worst_grad({k: q.grad for k, q in model.named_parameters()}, p, 80) < 1e-7
+        energy, _forces = run_mirror("qm9", model, p)
+    assert rel_err(energy.detach(), p.t("energy")) < 1e-10
+    assert worst_grad({k: q.grad for k, q in model.named_parameters()}, p.grads, 80) < 1e-7
 
-    p = _part(gold, "md17")
-    model = _mirror(p, GraphAttentionTransformerMD17).double()
+    p = _part("md17")
+    model = mirror(GraphAttentionTransformerMD17, p.cfg, p.state).double()
     with _emulated():
-        e, f = model(node_atom=torch.from_numpy(p["z"]), pos=torch.from_numpy(p["pos"]).double(), batch=torch.from_numpy(p["batch"]))
-        (e.sum() + (f ** 2).sum()).backward()
-    assert rel_err(e.detach(), torch.from_numpy(p["energy"])) < 1e-10
-    assert rel_err(f.detach(), torch.from_numpy(p["forces"])) < 1e-9
-    assert _worst_grad({k: q.grad for k, q in model.named_parameters()}, p, 80) < 1e-6
+        e, f = run_mirror("md17", model, p)
+    assert rel_err(e.detach(), p.t("energy")) < 1e-10
+    assert rel_err(f.detach(), p.t("forces")) < 1e-9
+    assert worst_grad({k: q.grad for k, q in model.named_parameters()}, p.grads, 80) < 1e-6
 
 
 def _shape_table():
@@ -329,21 +290,17 @@ def test_k8_first_layer_gemms(cuda_device, monkeypatch, deterministic):
     assert rel_err(ops.gemm_raw(2, d(X), d(G)).cpu(), X.double().t() @ G.double()) < 4e-5
 
 
-def _cuda_qm9(gold, dev):
-    from equiformer_b200.nets.graph_attention_transformer import GraphAttentionTransformer
-    p = _part(gold, "qm9")
-    model = _mirror(p, GraphAttentionTransformer).to(dev)
-    return p, model, tuple(torch.from_numpy(p[k]).to(dev) for k in ("pos", "batch", "z"))
-
-
 @pytest.mark.gpu
-def test_cuda_qm9_bessel_model_matches_reference(cuda_device, gold):
+def test_cuda_qm9_bessel_model_matches_reference(cuda_device):
     """Energies and gradients of sum(E^2) through GraphedStep (capture + replay), then eager.  The captured step runs
     first, as in the other capture tests: its warm-up runs on a side stream, never on the default one."""
     from equiformer_b200 import ops
     from equiformer_b200.graphs import GraphedStep
+    from equiformer_b200.nets.graph_attention_transformer import GraphAttentionTransformer
     from equiformer_b200.parallel import FlatGradAllReduce
-    p, model, (pos, batch, z) = _cuda_qm9(gold, cuda_device)
+    p = _part("qm9")
+    model = mirror(GraphAttentionTransformer, p.cfg, p.state).to(cuda_device)
+    pos, batch, z = (p.t(k, cuda_device) for k in ("pos", "batch", "z"))
     graph = ops.Graph(*R.radius_graph(pos, 5.0, batch), pos.shape[0])
     src, dst = graph.src, graph.dst
     bucket = FlatGradAllReduce(model.parameters())
@@ -360,27 +317,26 @@ def test_cuda_qm9_bessel_model_matches_reference(cuda_device, gold):
     for _ in range(2):
         loss = step((int(pos.shape[0]), int(src.numel())), [pos, batch, z, src, dst, graph.row_ptr]).clone()
     assert step.captures == 1
-    assert rel_err(loss.cpu(), (torch.from_numpy(p["energy"]) ** 2).sum()) < 1e-4
-    assert _worst_grad({k: q.grad for k, q in model.named_parameters()}, p, 80) < 1e-3
+    assert rel_err(loss.cpu(), (p.t("energy") ** 2).sum()) < 1e-4
+    assert worst_grad({k: q.grad for k, q in model.named_parameters()}, p.grads, 80) < 1e-3
 
     bucket.zero_grad()
-    energy = model(f_in=None, pos=pos, batch=batch, node_atom=z)
-    assert rel_err(energy.detach().cpu(), torch.from_numpy(p["energy"])) < 5e-5
-    (energy ** 2).sum().backward()
-    assert _worst_grad({k: q.grad for k, q in model.named_parameters()}, p, 80) < 1e-3
+    energy, _forces = run_mirror("qm9", model, p, cuda_device, torch.float32)
+    assert rel_err(energy.detach().cpu(), p.t("energy")) < 5e-5
+    assert worst_grad({k: q.grad for k, q in model.named_parameters()}, p.grads, 80) < 1e-3
 
 
 @pytest.mark.gpu
-def test_cuda_md17_bessel_model_matches_reference(cuda_device, gold):
+def test_cuda_md17_bessel_model_matches_reference(cuda_device):
     """Energy, forces and gradients of the energy + force loss (double backward through the basis), captured, then
     eager."""
     from equiformer_b200 import ops
     from equiformer_b200.graphs import GraphedStep
     from equiformer_b200.nets.graph_attention_transformer_md17 import GraphAttentionTransformerMD17
     from equiformer_b200.parallel import FlatGradAllReduce
-    p = _part(gold, "md17")
-    model = _mirror(p, GraphAttentionTransformerMD17).to(cuda_device)
-    pos, batch, z = (torch.from_numpy(p[k]).to(cuda_device) for k in ("pos", "batch", "z"))
+    p = _part("md17")
+    model = mirror(GraphAttentionTransformerMD17, p.cfg, p.state).to(cuda_device)
+    pos, batch, z = (p.t(k, cuda_device) for k in ("pos", "batch", "z"))
     graph = ops.Graph(*R.radius_graph(pos, 5.0, batch), pos.shape[0])
     bucket = FlatGradAllReduce(model.parameters())
 
@@ -396,16 +352,15 @@ def test_cuda_md17_bessel_model_matches_reference(cuda_device, gold):
     for _ in range(2):
         loss = step((int(pos.shape[0]), graph.n_edges), [pos, batch, z, graph.src, graph.dst, graph.row_ptr]).clone()
     assert step.captures == 1
-    ref_loss = float(p["energy"].sum() + (p["forces"] ** 2).sum())
+    ref_loss = float(p.t("energy").sum() + (p.t("forces") ** 2).sum())
     assert abs(float(loss) - ref_loss) / abs(ref_loss) < 1e-4
-    assert _worst_grad({k: q.grad for k, q in model.named_parameters()}, p, 80) < 1e-3
+    assert worst_grad({k: q.grad for k, q in model.named_parameters()}, p.grads, 80) < 1e-3
 
     bucket.zero_grad()
-    e, f = model(node_atom=z, pos=pos.clone(), batch=batch)
-    assert rel_err(e.detach().cpu(), torch.from_numpy(p["energy"])) < 5e-5
-    assert rel_err(f.detach().cpu(), torch.from_numpy(p["forces"])) < 2e-4
-    (e.sum() + (f ** 2).sum()).backward()
-    assert _worst_grad({k: q.grad for k, q in model.named_parameters()}, p, 80) < 1e-3
+    e, f = run_mirror("md17", model, p, cuda_device, torch.float32)
+    assert rel_err(e.detach().cpu(), p.t("energy")) < 5e-5
+    assert rel_err(f.detach().cpu(), p.t("forces")) < 2e-4
+    assert worst_grad({k: q.grad for k, q in model.named_parameters()}, p.grads, 80) < 1e-3
 
 
 @pytest.mark.gpu

@@ -23,12 +23,11 @@ import numpy as np
 import pytest
 import torch
 
-from oracle import equiformer_ref as R
 from tests import _emulation as emu
 from tests.helpers import rel_err
+from tests.reference_fixtures import GOLDEN, load, mirror, oracle_config, run_mirror, run_oracle, worst_grad
 
-FIXTURE = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_model_linear_small.npz")
-OC20_STATS = dict(max_atom_type=84, qm9_atom_remap=False, avg_degree=23.395238876342773, avg_num_nodes=77.81317)
+FIXTURE = "reference_model_linear_small.npz"
 TOL = 2e-5                      # kernel vs the float32 chain
 
 # head layouts: (H, A, value ds, value Cs) - the value scalars (R = A channels per head) lead
@@ -52,7 +51,7 @@ def test_oc20_l1_256_configuration_matches_the_yml():
 def test_full_size_state_dict_and_no_weight_decay_match_the_reference():
     from equiformer_b200.nets import model_entrypoint
     from equiformer_b200.nets.graph_attention_transformer_oc20 import OC20_L1_256
-    g = np.load(FIXTURE)
+    g = np.load(os.path.join(GOLDEN, FIXTURE))
     model = model_entrypoint("graph_attention_transformer_oc20")(**OC20_L1_256)
     assert len(model.blocks) == 8 and all(not b.ga.nonlinear_message for b in model.blocks)
     assert all(b.ga._mlp_layout is not None for b in model.blocks)
@@ -62,105 +61,37 @@ def test_full_size_state_dict_and_no_weight_decay_match_the_reference():
 
 
 # ------------------------------------------------------------------------------------------------ reference fixture
-def _case(kind):
-    g = np.load(FIXTURE)
-    p = f"{kind}/"
-    sub = {k[len(p):]: g[k] for k in g.files if k.startswith(p)}
-    cfg = {k[4:]: v for k, v in sub.items() if k.startswith("cfg/")}
-    cfg = {k: (str(v) if v.dtype.kind in "US" else bool(v) if v.dtype.kind == "b" else
-               [int(c) for c in v] if v.ndim == 1 else int(v) if v.dtype.kind == "i" else float(v)) for k, v in cfg.items()}
-    state = {k[6:]: torch.from_numpy(v) for k, v in sub.items() if k.startswith("state/")}
-    grads = {k[5:]: torch.from_numpy(v) for k, v in sub.items() if k.startswith("grad/")}
-    return sub, cfg, state, grads
-
-
-def _worst_grad(named: dict, ref: dict) -> float:
-    assert len(ref) > 50
-    worst = 0.0
-    for k, r in ref.items():
-        got = named[k]
-        assert got is not None, k
-        worst = max(worst, float((got.detach().double().cpu() - r.double()).abs().max() / r.abs().max().clamp_min(1e-12)))
-    return worst
-
-
-def _oracle_cfg(kind, cfg):
-    extra = {"qm9": dict(basis_type="gaussian"), "md17": dict(basis_type="exp", max_atom_type=64, qm9_atom_remap=False),
-             "oc20": OC20_STATS}[kind]
-    return R.Config(irreps_node_embedding=cfg["irreps_node_embedding"], irreps_sh=cfg["irreps_sh"],
-                    irreps_head=cfg["irreps_head"], irreps_mlp_mid=cfg["irreps_mlp_mid"],
-                    irreps_feature=cfg["irreps_feature"], num_heads=cfg["num_heads"], num_layers=cfg["num_layers"],
-                    max_radius=cfg["max_radius"], number_of_basis=cfg["number_of_basis"], nonlinear_message=False,
-                    **extra)
-
-
-@pytest.mark.parametrize("kind", ["qm9", "md17", "oc20"])
-def test_oracle_matches_reference_linear_message_model_files(kind):
-    sub, cfg, state, grads = _case(kind)
-    ocfg = _oracle_cfg(kind, cfg)
-    params = {k: v.requires_grad_(v.is_floating_point() and v.numel() > 0) for k, v in R.cast_params(state, torch.float64).items()}
-    t = lambda k: torch.from_numpy(sub[k])
-    pos = t("pos").double()
-    if kind == "qm9":
-        energy = R.model_forward(params, ocfg, pos, t("batch"), t("z"), n_graphs=2)
-        (energy ** 2).sum().backward()
-    elif kind == "md17":
-        energy, forces = R.energy_and_forces(params, ocfg, pos, t("batch"), t("z"), 1, create_graph=True)
-        assert rel_err(forces.detach(), t("forces")) < 1e-10
-        (energy.sum() + (forces ** 2).sum()).backward()
-    else:
-        edge = t("edge_index")
-        energy = R.model_forward_oc20(params, ocfg, pos, t("cell").double(), t("batch"), t("z"), t("tags"), 2, edge[0],
-                                      edge[1], t("cell_offsets"))
-        (energy ** 2).sum().backward()
-    assert rel_err(energy.detach(), t("energy")) < 1e-10
-    assert _worst_grad({k: v.grad for k, v in params.items()}, grads) < 1e-8
-
-
-def _mirror(kind, cfg, state):
+def _mirror(kind, case):
     from equiformer_b200.nets.graph_attention_transformer import GraphAttentionTransformer
     from equiformer_b200.nets.graph_attention_transformer_md17 import GraphAttentionTransformerMD17
     from equiformer_b200.nets.graph_attention_transformer_oc20 import GraphAttentionTransformerOC20
     if kind == "oc20":
-        model = GraphAttentionTransformerOC20(None, None, 1, **cfg)
-    else:
-        model = {"qm9": GraphAttentionTransformer, "md17": GraphAttentionTransformerMD17}[kind](**cfg)
-    res = model.load_state_dict(state, strict=False)
-    assert not res.unexpected_keys and all(k.endswith("tp.output_mask") for k in res.missing_keys), res
-    return model.eval()
+        return mirror(GraphAttentionTransformerOC20, case.cfg, case.state, None, None, 1)
+    return mirror({"qm9": GraphAttentionTransformer, "md17": GraphAttentionTransformerMD17}[kind], case.cfg, case.state)
 
 
-def _run_mirror(kind, model, sub, dev=None, dtype=torch.float64):
-    """energy (and forces) of the mirror; the training loss of the fixture backpropagated into the parameters"""
-    t = lambda k: torch.from_numpy(sub[k]).to(dev) if dev is not None else torch.from_numpy(sub[k])
-    pos = t("pos").to(dtype)
-    if kind == "qm9":
-        energy = model(f_in=None, pos=pos, batch=t("batch"), node_atom=t("z"))
-        (energy ** 2).sum().backward()
-        return energy, None
-    if kind == "md17":
-        energy, forces = model(node_atom=t("z"), pos=pos.clone(), batch=t("batch"))
-        (energy.sum() + (forces ** 2).sum()).backward()
-        return energy, forces
-    data = types.SimpleNamespace(pos=pos, cell=t("cell").to(dtype), batch=t("batch"), atomic_numbers=t("z"),
-                                 tags=t("tags"), n_graphs=2)
-    energy = model(data)
-    (energy ** 2).sum().backward()
-    return energy, None
+@pytest.mark.parametrize("kind", ["qm9", "md17", "oc20"])
+def test_oracle_matches_reference_linear_message_model_files(kind):
+    case = load(FIXTURE, kind)
+    energy, forces, params = run_oracle(kind, case, oracle_config(kind, case.cfg))
+    if forces is not None:
+        assert rel_err(forces.detach(), case.t("forces")) < 1e-10
+    assert rel_err(energy.detach(), case.t("energy")) < 1e-10
+    assert worst_grad({k: v.grad for k, v in params.items()}, case.grads, 51) < 1e-8
 
 
 @pytest.mark.parametrize("kind", ["qm9", "md17", "oc20"])
 def test_mirror_with_emulated_kernels_matches_reference_linear_message_model_files(kind):
     """float64 CPU stand-ins: the predicate of the fused kernel is false, so the existing chain runs."""
     from tests._emulation import emulated_kernels
-    sub, cfg, state, grads = _case(kind)
-    model = _mirror(kind, cfg, state).double()
+    case = load(FIXTURE, kind)
+    model = _mirror(kind, case).double()
     with emulated_kernels():
-        energy, forces = _run_mirror(kind, model, sub)
-    assert rel_err(energy.detach(), torch.from_numpy(sub["energy"])) < 1e-10
+        energy, forces = run_mirror(kind, model, case)
+    assert rel_err(energy.detach(), case.t("energy")) < 1e-10
     if forces is not None:
-        assert rel_err(forces.detach(), torch.from_numpy(sub["forces"])) < 1e-10
-    assert _worst_grad({k: p.grad for k, p in model.named_parameters()}, grads) < 1e-7
+        assert rel_err(forces.detach(), case.t("forces")) < 1e-10
+    assert worst_grad({k: p.grad for k, p in model.named_parameters()}, case.grads, 51) < 1e-7
 
 
 # ------------------------------------------------------------------------------------------------ host logic (float64)
@@ -391,8 +322,8 @@ def test_md17_l2_forces_and_their_training_gradients_match_the_chain(cuda_device
 @pytest.mark.parametrize("kind", ["qm9", "md17", "oc20"])
 def test_cuda_linear_message_models_match_reference_model_files(cuda_device, kind):
     from equiformer_b200 import ops
-    sub, cfg, state, grads = _case(kind)
-    model = _mirror(kind, cfg, state).to(cuda_device)
+    case = load(FIXTURE, kind)
+    model = _mirror(kind, case).to(cuda_device)
     calls = []
     orig = ops.mlp_softmax_aggregate_raw
 
@@ -402,14 +333,14 @@ def test_cuda_linear_message_models_match_reference_model_files(cuda_device, kin
 
     ops.mlp_softmax_aggregate_raw = counting
     try:
-        energy, forces = _run_mirror(kind, model, sub, cuda_device, torch.float32)
+        energy, forces = run_mirror(kind, model, case, cuda_device, torch.float32)
     finally:
         ops.mlp_softmax_aggregate_raw = orig
-    assert len(calls) >= cfg["num_layers"]
-    assert rel_err(energy, torch.from_numpy(sub["energy"])) < 5e-5
+    assert len(calls) >= case.cfg["num_layers"]
+    assert rel_err(energy, case.t("energy")) < 5e-5
     if forces is not None:
-        assert rel_err(forces, torch.from_numpy(sub["forces"])) < 2e-4
-    assert _worst_grad({k: p.grad for k, p in model.named_parameters()}, grads) < 1e-3
+        assert rel_err(forces, case.t("forces")) < 2e-4
+    assert worst_grad({k: p.grad for k, p in model.named_parameters()}, case.grads, 51) < 1e-3
 
 
 @pytest.mark.gpu

@@ -13,8 +13,6 @@ models against the fixture, eager and captured.
 """
 from __future__ import annotations
 
-import os
-
 import numpy as np
 import pytest
 import scipy.linalg
@@ -24,8 +22,9 @@ from oracle import e3nn_ref as e3
 from oracle import equiformer_ref as R
 from tests import oracle_l4
 from tests.helpers import rel_err
+from tests.reference_fixtures import load, mirror, oracle_config, run_mirror, run_oracle, worst_grad
 
-FIXTURE = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_model_l4_small.npz")
+FIXTURE = "reference_model_l4_small.npz"
 SH4 = "1x0e+1x1e+1x2e+1x3e+1x4e"
 FULL_IN1 = "32x0e+16x1e+16x2e+16x3e+16x4e"
 
@@ -105,83 +104,34 @@ def test_oracle_degree4_harmonics_equal_the_package_recurrence():
 
 
 # ------------------------------------------------------------------------------------------------ reference fixture
-def _case(kind):
-    g = np.load(FIXTURE)
-    p = f"{kind}/"
-    sub = {k[len(p):]: g[k] for k in g.files if k.startswith(p)}
-    cfg = {k[4:]: v for k, v in sub.items() if k.startswith("cfg/")}
-    cfg = {k: (str(v) if v.dtype.kind in "US" else bool(v) if v.dtype.kind == "b" else
-               [int(c) for c in v] if v.ndim == 1 else int(v) if v.dtype.kind == "i" else float(v)) for k, v in cfg.items()}
-    state = {k[6:]: torch.from_numpy(v) for k, v in sub.items() if k.startswith("state/")}
-    grads = {k[5:]: torch.from_numpy(v) for k, v in sub.items() if k.startswith("grad/")}
-    return sub, cfg, state, grads
-
-
-def _worst_grad(named: dict, ref: dict) -> float:
-    assert len(ref) > 50
-    worst = 0.0
-    for k, r in ref.items():
-        got = named[k]
-        assert got is not None, k
-        worst = max(worst, float((got.detach().double().cpu() - r.double()).abs().max() / r.abs().max().clamp_min(1e-12)))
-    return worst
-
-
 @pytest.mark.parametrize("kind", ["qm9", "md17"])
 def test_oracle_matches_reference_l4_model_files(kind, oracle_at_l4):
-    sub, cfg, state, grads = _case(kind)
-    assert cfg["irreps_sh"] == SH4 and cfg["irreps_node_embedding"].endswith("4e")
-    extra = dict(basis_type="gaussian") if kind == "qm9" else dict(basis_type="exp", max_atom_type=64, qm9_atom_remap=False)
-    ocfg = R.Config(irreps_node_embedding=cfg["irreps_node_embedding"], irreps_sh=cfg["irreps_sh"],
-                    irreps_head=cfg["irreps_head"], irreps_mlp_mid=cfg["irreps_mlp_mid"],
-                    irreps_feature=cfg["irreps_feature"], num_heads=cfg["num_heads"], num_layers=cfg["num_layers"],
-                    max_radius=cfg["max_radius"], number_of_basis=cfg["number_of_basis"], nonlinear_message=True, **extra)
-    params = {k: v.requires_grad_(v.is_floating_point() and v.numel() > 0) for k, v in R.cast_params(state, torch.float64).items()}
-    t = lambda k: torch.from_numpy(sub[k])
-    pos = t("pos").double()
-    if kind == "qm9":
-        energy = R.model_forward(params, ocfg, pos, t("batch"), t("z"), n_graphs=2)
-        (energy ** 2).sum().backward()
-    else:
-        energy, forces = R.energy_and_forces(params, ocfg, pos, t("batch"), t("z"), 1, create_graph=True)
-        assert rel_err(forces.detach(), t("forces")) < 1e-10
-        (energy.sum() + (forces ** 2).sum()).backward()
-    assert rel_err(energy.detach(), t("energy")) < 1e-10
-    assert _worst_grad({k: v.grad for k, v in params.items()}, grads) < 1e-10
+    case = load(FIXTURE, kind)
+    assert case.cfg["irreps_sh"] == SH4 and case.cfg["irreps_node_embedding"].endswith("4e")
+    energy, forces, params = run_oracle(kind, case, oracle_config(kind, case.cfg))
+    if forces is not None:
+        assert rel_err(forces.detach(), case.t("forces")) < 1e-10
+    assert rel_err(energy.detach(), case.t("energy")) < 1e-10
+    assert worst_grad({k: v.grad for k, v in params.items()}, case.grads, 51) < 1e-10
 
 
-def _mirror(kind, cfg, state):
+def _mirror(kind, case):
     from equiformer_b200.nets.graph_attention_transformer import GraphAttentionTransformer
     from equiformer_b200.nets.graph_attention_transformer_md17 import GraphAttentionTransformerMD17
-    model = {"qm9": GraphAttentionTransformer, "md17": GraphAttentionTransformerMD17}[kind](**cfg)
-    res = model.load_state_dict(state, strict=False)
-    assert not res.unexpected_keys and all(k.endswith("tp.output_mask") for k in res.missing_keys), res
-    return model.eval()
-
-
-def _run_mirror(kind, model, sub, dev=None, dtype=torch.float64):
-    t = lambda k: torch.from_numpy(sub[k]).to(dev) if dev is not None else torch.from_numpy(sub[k])
-    pos = t("pos").to(dtype)
-    if kind == "qm9":
-        energy = model(f_in=None, pos=pos, batch=t("batch"), node_atom=t("z"))
-        (energy ** 2).sum().backward()
-        return energy, None
-    energy, forces = model(node_atom=t("z"), pos=pos.clone(), batch=t("batch"))
-    (energy.sum() + (forces ** 2).sum()).backward()
-    return energy, forces
+    return mirror({"qm9": GraphAttentionTransformer, "md17": GraphAttentionTransformerMD17}[kind], case.cfg, case.state)
 
 
 @pytest.mark.parametrize("kind", ["qm9", "md17"])
 def test_mirror_with_emulated_kernels_matches_reference_l4_model_files(kind):
     from tests._emulation import emulated_kernels
-    sub, cfg, state, grads = _case(kind)
-    model = _mirror(kind, cfg, state).double()
+    case = load(FIXTURE, kind)
+    model = _mirror(kind, case).double()
     with emulated_kernels():
-        energy, forces = _run_mirror(kind, model, sub)
-    assert rel_err(energy.detach(), torch.from_numpy(sub["energy"])) < 1e-10
+        energy, forces = run_mirror(kind, model, case)
+    assert rel_err(energy.detach(), case.t("energy")) < 1e-10
     if forces is not None:
-        assert rel_err(forces.detach(), torch.from_numpy(sub["forces"])) < 1e-10
-    assert _worst_grad({k: p.grad for k, p in model.named_parameters()}, grads) < 1e-7
+        assert rel_err(forces.detach(), case.t("forces")) < 1e-10
+    assert worst_grad({k: p.grad for k, p in model.named_parameters()}, case.grads, 51) < 1e-7
 
 
 # ------------------------------------------------------------------------------------------------ plans and routes
@@ -357,11 +307,11 @@ def test_cuda_l4_models_match_reference_model_files(cuda_device, kind):
     from equiformer_b200 import ops
     from equiformer_b200.graphs import GraphedForwardBackward, GraphedStep
     from equiformer_b200.parallel import FlatGradAllReduce
-    sub, cfg, state, grads = _case(kind)
-    model = _mirror(kind, cfg, state).to(cuda_device)
+    case = load(FIXTURE, kind)
+    cfg = case.cfg
+    model = _mirror(kind, case).to(cuda_device)
     assert not ops.dtp_linear_supported(model.blocks[0].ga.sep_act.dtp.tp.plan)
-    t = lambda k: torch.from_numpy(sub[k]).to(cuda_device)
-    pos, batch, z = t("pos"), t("batch"), t("z")
+    pos, batch, z = case.t("pos", cuda_device), case.t("batch", cuda_device), case.t("z", cuda_device)
     bucket = FlatGradAllReduce(model.parameters())
     if kind == "qm9":
         gfb = GraphedForwardBackward(model, lambda out, tgt: ((out - tgt) ** 2).sum(), bucket, max_radius=cfg["max_radius"])
@@ -385,17 +335,16 @@ def test_cuda_l4_models_match_reference_model_files(cuda_device, kind):
             loss = step((int(pos.shape[0]), graph.n_edges), [pos, batch, z, graph.src, graph.dst, graph.row_ptr]).clone()
         assert step.captures == 1
     captured_grads = {k: p.grad.clone() for k, p in model.named_parameters() if p.grad is not None}
-    energy_ref = torch.from_numpy(sub["energy"]).double()
-    ref_loss = ((energy_ref ** 2).sum() if kind == "qm9"
-                else energy_ref.sum() + (torch.from_numpy(sub["forces"]).double() ** 2).sum())
+    energy_ref = case.t("energy")
+    ref_loss = ((energy_ref ** 2).sum() if kind == "qm9" else energy_ref.sum() + (case.t("forces") ** 2).sum())
     assert abs(float(loss) - float(ref_loss)) <= 1e-4 * abs(float(ref_loss))
-    assert _worst_grad(captured_grads, grads) < 1e-3
+    assert worst_grad(captured_grads, case.grads, 51) < 1e-3
 
     bucket.zero_grad()
-    energy, forces = _run_mirror(kind, model, sub, cuda_device, torch.float32)
-    assert rel_err(energy, torch.from_numpy(sub["energy"])) < 1e-4
+    energy, forces = run_mirror(kind, model, case, cuda_device, torch.float32)
+    assert rel_err(energy, case.t("energy")) < 1e-4
     if forces is not None:
-        assert rel_err(forces, torch.from_numpy(sub["forces"])) < 1e-4
-    assert _worst_grad({k: p.grad for k, p in model.named_parameters()}, grads) < 1e-3
+        assert rel_err(forces, case.t("forces")) < 1e-4
+    assert worst_grad({k: p.grad for k, p in model.named_parameters()}, case.grads, 51) < 1e-3
     worst = max((rel_err(p.grad, captured_grads[k]), k) for k, p in model.named_parameters() if k in captured_grads)
     assert worst[0] < 1e-4, worst

@@ -17,11 +17,10 @@ import pytest
 import torch
 
 from tests.helpers import rel_err
+from tests.reference_fixtures import GOLDEN, dens_setup
 
-GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 NOISE = os.path.join(GOLDEN, "reference_dens_noise.npz")
-FIXTURES = {"l2_small": os.path.join(GOLDEN, "reference_model_dens_small.npz"),
-            "l3_small": os.path.join(GOLDEN, "reference_model_dens_l3_small.npz")}
+FIXTURES = {"l2_small": "reference_model_dens_small.npz", "l3_small": "reference_model_dens_l3_small.npz"}
 NOISE_CASES = [(None, 0.0), (None, 0.25), (None, 1.0), (0.25, 0.0), (0.25, 0.25), (0.25, 1.0)]
 TASK_MEAN, TASK_STD, STD = -0.37, 1.9, 0.05
 
@@ -118,26 +117,6 @@ def test_dens_configuration_dicts():
 
 # ----------------------------------------------------------------------------------------------------- the model (CPU)
 
-def _setup(which, dev=None, dtype=torch.float64):
-    from equiformer_b200.nets.equiformer_md17_dens import Equiformer_MD17_DeNS
-    g = np.load(FIXTURES[which])
-    cfg = {k[4:]: g[k].tolist() for k in g.files if k.startswith("cfg/")}
-    cfg["fc_neurons"] = list(cfg["fc_neurons"])
-    state = {k[6:]: torch.from_numpy(g[k]) for k in g.files if k.startswith("state/")}
-    model = Equiformer_MD17_DeNS(**cfg)
-    res = model.load_state_dict(state, strict=False)
-    assert not res.unexpected_keys and all(k.endswith("tp.output_mask") for k in res.missing_keys), res
-    model = model.eval().to(dtype)
-    t = lambda k: torch.from_numpy(g[k])
-    data = types.SimpleNamespace(z=t("z"), pos=t("pos").to(dtype), batch=t("batch"), force=t("force").to(dtype),
-                                 noise_mask=t("noise_mask"))
-    if dev is not None:
-        model = model.to(dev)
-        for k, v in vars(data).items():
-            setattr(data, k, v.to(dev))
-    return g, model, data
-
-
 def _targets(n_atoms, n_graphs, dtype=torch.float64):
     g = torch.Generator().manual_seed(5)
     return (torch.randn(n_graphs, 1, generator=g, dtype=dtype), torch.randn(n_atoms, 3, generator=g, dtype=dtype),
@@ -160,7 +139,7 @@ def test_forward_edges_equals_forward(which):
     from equiformer_b200.graph import radius_graph
     from equiformer_b200.md17_dens_objective import dens_loss
     from tests._emulation import emulated_kernels
-    _g, model, data = _setup(which)
+    _case, model, data = dens_setup(FIXTURES[which])
     n, G = data.pos.shape[0], int(data.batch.max()) + 1
     y, dy, noise_vec = _targets(n, G)
     loss_of = lambda e, d: dens_loss(e, d, y, dy, noise_vec, data.noise_mask, TASK_MEAN, TASK_STD, STD, 1.0, 80.0, 5.0)
@@ -184,7 +163,7 @@ def test_padding_leaves_real_outputs_unchanged(which):
     from equiformer_b200.graphs import pad_to_bucket
     from equiformer_b200.md17_dens_objective import dens_loss
     from tests._emulation import emulated_kernels
-    _g, model, data = _setup(which)
+    _case, model, data = dens_setup(FIXTURES[which])
     n, G = data.pos.shape[0], int(data.batch.max()) + 1
     y, dy, noise_vec = _targets(n, G)
     edge = radius_graph(data.pos, 5.0, data.batch, max_num_neighbors=1000)
@@ -215,27 +194,26 @@ def test_mirror_dens_l3_matches_reference_model_file():
     """The L3 fixture (``1x3e`` harmonics and force encoding, a ``3e`` block in the feature and the head), kernels
     emulated in float64: energies and outputs to 1e-10, parameter gradients of an energy + output loss to 1e-6."""
     from tests._emulation import emulated_kernels
-    g, model, data = _setup("l3_small")
+    case, model, data = dens_setup(FIXTURES["l3_small"])
     with emulated_kernels():
         energy, dy = model(data)
         (energy.sum() + (dy ** 2).sum()).backward()
-    assert rel_err(energy, torch.from_numpy(g["energy"])) < 1e-10
-    assert rel_err(dy, torch.from_numpy(g["dy"])) < 1e-10
-    for k in g.files:
-        if k.startswith("grad/"):
-            assert rel_err(model.get_parameter(k[5:]).grad, torch.from_numpy(g[k])) < 1e-6, k
+    assert rel_err(energy, case.t("energy")) < 1e-10
+    assert rel_err(dy, case.t("dy")) < 1e-10
+    for k, ref in case.grads.items():
+        assert rel_err(model.get_parameter(k).grad, ref) < 1e-6, k
 
 
 # ------------------------------------------------------------------------------------------------------------- GPU
 
 @pytest.mark.gpu
 def test_cuda_dens_l3_matches_reference_model_file(cuda_device):
-    g, model, data = _setup("l3_small", cuda_device, torch.float32)
+    case, model, data = dens_setup(FIXTURES["l3_small"], cuda_device, torch.float32)
     energy, dy = model(data)
     (energy.sum() + (dy ** 2).sum()).backward()
-    assert rel_err(energy, torch.from_numpy(g["energy"])) < 1e-4
-    assert rel_err(dy, torch.from_numpy(g["dy"])) < 3e-4
-    worst = max(rel_err(model.get_parameter(k[5:]).grad, torch.from_numpy(g[k])) for k in g.files if k.startswith("grad/"))
+    assert rel_err(energy, case.t("energy")) < 1e-4
+    assert rel_err(dy, case.t("dy")) < 3e-4
+    worst = max(rel_err(model.get_parameter(k).grad, ref) for k, ref in case.grads.items())
     assert worst < 2e-3, worst
 
 

@@ -22,24 +22,20 @@ import pytest
 import torch
 
 from tests.helpers import rel_err
+from tests.reference_fixtures import GOLDEN, load, mirror, run_mirror
 
-FIXTURE = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_norms_small.npz")
+FIXTURE = "reference_norms_small.npz"
 NORMS = ("graph", "instance", "fast_layer")
-
-
-@pytest.fixture(scope="module")
-def gold():
-    return np.load(FIXTURE)
 
 
 def _module_names(g):
     return sorted({k.split("/")[1] for k in g.files if k.startswith("mod/")})
 
 
-MODULE_CASES = _module_names(np.load(FIXTURE))
+MODULE_CASES = _module_names(np.load(os.path.join(GOLDEN, FIXTURE)))
 
 
-def _module(name, g):
+def _module(name, case):
     from equiformer_b200.nets.fast_layer_norm import EquivariantLayerNormFast
     from equiformer_b200.nets.graph_norm import EquivariantGraphNorm
     from equiformer_b200.nets.instance_norm import EquivariantInstanceNorm
@@ -50,23 +46,23 @@ def _module(name, g):
     else:
         cls = {"graph": EquivariantGraphNorm, "instance": EquivariantInstanceNorm}[kind]
         m = cls(irreps, eps=1e-5, affine=affine == "affine", reduce=rest[0], normalization=norm)
-    state = {k.split("/")[-1]: torch.from_numpy(g[k]) for k in g.files if k.startswith(f"mod/{name}/state/")}
-    m.load_state_dict(state, strict=True)
+    m.load_state_dict(case.state, strict=True)
     return m.double()
 
 
 # ------------------------------------------------------------------------------------------------ CPU: statements
 @pytest.mark.parametrize("name", MODULE_CASES)
-def test_torch_statement_matches_reference_norm_files(gold, name):
-    m = _module(name, gold)
-    t = lambda k: torch.from_numpy(gold[f"mod/{name}/{k}"])
+def test_torch_statement_matches_reference_norm_files(name):
+    case = load(FIXTURE, f"mod/{name}")
+    m = _module(name, case)
+    t = case.t
     x = t("x").clone().requires_grad_(True)
     y = m(x, batch=t("batch"))
     (y * t("gy")).sum().backward()
     assert rel_err(y.detach(), t("y")) < 1e-10
     assert rel_err(x.grad, t("gx")) < 1e-10
     for k, p in m.named_parameters():
-        assert rel_err(p.grad, t(f"grad/{k}")) < 1e-10, k
+        assert rel_err(p.grad, case.grads[k]) < 1e-10, k
 
 
 def test_get_norm_layer_returns_the_reference_classes():
@@ -137,50 +133,32 @@ def test_fast_layer_norm_equals_layer_norm_v2():
         assert rel_err(a(x), b(x)) < 1e-12
 
 
-def _model_case(g, prefix):
-    cfg = {k[len(prefix) + 5:]: g[k].tolist() for k in g.files if k.startswith(f"{prefix}/cfg/")}
-    cfg["fc_neurons"] = list(cfg["fc_neurons"])
-    state = {k[len(prefix) + 7:]: torch.from_numpy(g[k]) for k in g.files if k.startswith(f"{prefix}/state/")}
-    return cfg, state
-
-
-def _mirror(kind, cfg, state):
+def _mirror(kind, case):
     from equiformer_b200.nets.graph_attention_transformer import GraphAttentionTransformer
     from equiformer_b200.nets.graph_attention_transformer_md17 import GraphAttentionTransformerMD17
-    model = {"qm9": GraphAttentionTransformer, "md17": GraphAttentionTransformerMD17}[kind](**cfg)
-    res = model.load_state_dict(state, strict=False)
-    assert not res.unexpected_keys and all(k.endswith("tp.output_mask") for k in res.missing_keys), res
-    return model.eval()
-
-
-def _run(kind, model, g, prefix, dev=None, dtype=torch.float64):
-    t = lambda k: torch.from_numpy(g[f"{prefix}/{k}"]).to(dev) if dev is not None else torch.from_numpy(g[f"{prefix}/{k}"])
-    pos = t("pos").to(dtype)
-    if kind == "qm9":
-        return model(f_in=None, pos=pos, batch=t("batch"), node_atom=t("z")), None
-    return model(node_atom=t("z"), pos=pos.clone(), batch=t("batch"))
+    return mirror({"qm9": GraphAttentionTransformer, "md17": GraphAttentionTransformerMD17}[kind], case.cfg, case.state)
 
 
 MODEL_CASES = [(kind, norm) for kind in ("qm9", "md17") for norm in NORMS]
 
 
 @pytest.mark.parametrize("kind,norm", MODEL_CASES)
-def test_mirror_loads_reference_state_dict(gold, kind, norm):
-    cfg, state = _model_case(gold, f"{kind}_{norm}")
-    model = _mirror(kind, cfg, state)
-    norm_keys = {k for k in state if ".norm" in k or k.startswith("norm.")}
+def test_mirror_loads_reference_state_dict(kind, norm):
+    case = load(FIXTURE, f"{kind}_{norm}")
+    model = _mirror(kind, case)
+    norm_keys = {k for k in case.state if ".norm" in k or k.startswith("norm.")}
     assert norm_keys and norm_keys <= set(model.state_dict())
     if norm == "graph":
         assert any(k.endswith("mean_shift") for k in norm_keys)
 
 
 @pytest.mark.parametrize("kind,norm", MODEL_CASES)
-def test_no_weight_decay_matches_reference_model_files(gold, kind, norm):
+def test_no_weight_decay_matches_reference_model_files(kind, norm):
     """The parameters left out of weight decay are the reference's: the graph and instance norms' ones among them, the
     fast layer norm's not."""
-    cfg, state = _model_case(gold, f"{kind}_{norm}")
-    model = _mirror(kind, cfg, state)
-    assert model.no_weight_decay() == set(gold[f"{kind}_{norm}/no_weight_decay"].tolist())
+    case = load(FIXTURE, f"{kind}_{norm}")
+    model = _mirror(kind, case)
+    assert model.no_weight_decay() == set(case.arrays["no_weight_decay"].tolist())
 
 
 @pytest.mark.parametrize("family", ["oc20", "oc20_dp", "dens"])
@@ -329,16 +307,15 @@ def test_torch_statement_gradcheck():
 
 
 @pytest.mark.parametrize("kind,norm", MODEL_CASES)
-def test_mirror_with_emulated_kernels_matches_reference_model_files(gold, kind, norm):
+def test_mirror_with_emulated_kernels_matches_reference_model_files(kind, norm):
     from tests._emulation import emulated_kernels
-    prefix = f"{kind}_{norm}"
-    cfg, state = _model_case(gold, prefix)
-    model = _mirror(kind, cfg, state).double()
+    case = load(FIXTURE, f"{kind}_{norm}")
+    model = _mirror(kind, case).double()
     with emulated_kernels(), emulated_norm_kernels():
-        energy, forces = _run(kind, model, gold, prefix)
-    assert rel_err(energy.detach(), torch.from_numpy(gold[f"{prefix}/energy"])) < 1e-10
+        energy, forces = run_mirror(kind, model, case)
+    assert rel_err(energy.detach(), case.t("energy")) < 1e-10
     if forces is not None:
-        assert rel_err(forces.detach(), torch.from_numpy(gold[f"{prefix}/forces"])) < 1e-10
+        assert rel_err(forces.detach(), case.t("forces")) < 1e-10
 
 
 # ------------------------------------------------------------------------------------------------ inventory
@@ -470,18 +447,18 @@ def test_kernels_are_bitwise_repeatable(cuda_device):
 # ------------------------------------------------------------------------------------------------ GPU: models
 @pytest.mark.gpu
 @pytest.mark.parametrize("kind,norm", MODEL_CASES)
-def test_cuda_models_match_reference_model_files(gold, cuda_device, kind, norm):
+def test_cuda_models_match_reference_model_files(cuda_device, kind, norm):
     """The captured step's loss against the fixture's, then the eager energies (and MD17 forces) at 1e-4 (the captured
     step runs first, as in the other capture tests)."""
     from equiformer_b200 import ops
     from equiformer_b200.graphs import GraphedForwardBackward, GraphedStep
     from equiformer_b200.parallel import FlatGradAllReduce
     from oracle import equiformer_ref as R
-    prefix = f"{kind}_{norm}"
-    cfg, state = _model_case(gold, prefix)
-    model = _mirror(kind, cfg, state).to(cuda_device)
-    t = lambda k: torch.from_numpy(gold[f"{prefix}/{k}"]).to(cuda_device)
-    energy_ref = torch.from_numpy(gold[f"{prefix}/energy"]).double()
+    case = load(FIXTURE, f"{kind}_{norm}")
+    cfg = case.cfg
+    model = _mirror(kind, case).to(cuda_device)
+    t = lambda k: case.t(k, cuda_device)
+    energy_ref = case.t("energy")
     pos, batch, z = t("pos"), t("batch"), t("z")
     n_graphs = int(energy_ref.shape[0])
     bucket = FlatGradAllReduce(model.parameters())
@@ -505,25 +482,25 @@ def test_cuda_models_match_reference_model_files(gold, cuda_device, kind, norm):
         for _ in range(2):
             loss = step((int(pos.shape[0]), graph.n_edges), [pos, batch, z, graph.src, graph.dst, graph.row_ptr]).clone()
         assert step.captures == 1
-        ref_loss = energy_ref.sum() + (torch.from_numpy(gold[f"{prefix}/forces"]).double() ** 2).sum()
+        ref_loss = energy_ref.sum() + (case.t("forces") ** 2).sum()
     assert abs(float(loss) - float(ref_loss)) <= 1e-4 * abs(float(ref_loss))
-    energy, forces = _run(kind, model, gold, prefix, cuda_device, torch.float32)
+    energy, forces = run_mirror(kind, model, case, cuda_device, torch.float32)
     assert rel_err(energy.detach(), energy_ref) < 1e-4
     if forces is not None:
-        assert rel_err(forces.detach(), torch.from_numpy(gold[f"{prefix}/forces"])) < 1e-4
+        assert rel_err(forces.detach(), case.t("forces")) < 1e-4
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("norm", ["graph", "instance"])
-def test_bucket_padding_is_its_own_graph(gold, cuda_device, norm):
+def test_bucket_padding_is_its_own_graph(cuda_device, norm):
     """The dummy molecule that pads a batch to its bucket is graph ``n_graphs``: the real molecules' energies and
     gradients with padding equal those without, although the norm statistics are per graph."""
     from equiformer_b200.graph import radius_graph_csr
     from equiformer_b200.graphs import csr_graph, pad_to_bucket
-    prefix = f"qm9_{norm}"
-    cfg, state = _model_case(gold, prefix)
-    model = _mirror("qm9", cfg, state).to(cuda_device)
-    t = lambda k: torch.from_numpy(gold[f"{prefix}/{k}"]).to(cuda_device)
+    case = load(FIXTURE, f"qm9_{norm}")
+    cfg = case.cfg
+    model = _mirror("qm9", case).to(cuda_device)
+    t = lambda k: case.t(k, cuda_device)
     pos, batch, z = t("pos"), t("batch"), t("z")
     G = int(batch.max()) + 1
     edge, row_ptr = radius_graph_csr(pos, cfg["max_radius"], batch, max_num_neighbors=1000)
@@ -539,7 +516,7 @@ def test_bucket_padding_is_its_own_graph(gold, cuda_device, norm):
         (out ** 2).sum().backward()
         runs.append((out.detach(), {k: p.grad.clone() for k, p in model.named_parameters() if p.grad is not None}))
     assert rel_err(runs[1][0], runs[0][0]) < 1e-5
-    assert rel_err(runs[0][0], torch.from_numpy(gold[f"{prefix}/energy"])) < 1e-4
+    assert rel_err(runs[0][0], case.t("energy")) < 1e-4
     # a gradient that vanishes in exact arithmetic (a bias that the next norm's mean subtraction removes) is rounding
     # noise in both runs: errors are taken against 1e-3 of the largest gradient entry of the model at least
     floor = 1e-3 * max(float(g.abs().max()) for g in runs[0][1].values())
@@ -574,12 +551,9 @@ def _family_model(family, norm, dev):
                    fc_neurons=[16, 16], irreps_feature="32x0e", irreps_head="8x0e+4x1e", num_heads=2,
                    irreps_pre_attn="16x0e+8x1e", irreps_mlp_mid="48x0e+24x1e", norm_layer=norm, alpha_drop=0.0)
         return cls(None, None, 1, **cfg).to(dev).eval()
-    from tests.test_md17_dens_train import _setup
-    g, _model, _data = _setup("l2_small")
     from equiformer_b200.nets.equiformer_md17_dens import Equiformer_MD17_DeNS
-    cfg = {k[4:]: g[k].tolist() for k in g.files if k.startswith("cfg/")}
-    cfg["fc_neurons"] = list(cfg["fc_neurons"])
-    return Equiformer_MD17_DeNS(**dict(cfg, norm_layer=norm)).to(dev).eval(), g
+    case = load("reference_model_dens_small.npz")
+    return Equiformer_MD17_DeNS(**dict(case.cfg, norm_layer=norm)).to(dev).eval(), case
 
 
 @pytest.mark.gpu
@@ -591,8 +565,8 @@ def test_model_families_captured_equal_eager(cuda_device, family, norm):
     from equiformer_b200.graphs import DensTrainStep, GraphedStep
     from equiformer_b200.parallel import FlatGradAllReduce
     if family == "dens":
-        model, g = _family_model(family, norm, cuda_device)
-        t = lambda k: torch.from_numpy(g[k]).to(cuda_device)
+        model, case = _family_model(family, norm, cuda_device)
+        t = lambda k: case.t(k, cuda_device)
         pos, batch, z = t("pos").float(), t("batch"), t("z")
         G = int(batch.max()) + 1
         gen = torch.Generator().manual_seed(2)

@@ -9,10 +9,6 @@ routes (generated ``oc20_l1`` DTP kernels, no edge-sized torch GEMM / scatter) a
 """
 from __future__ import annotations
 
-import os
-import types
-
-import numpy as np
 import pytest
 import torch
 
@@ -20,89 +16,51 @@ from oracle import e3nn_ref as e3
 from oracle import equiformer_ref as R
 from tests import oracle_oc20_aux as OA
 from tests.helpers import rel_err
+from tests.reference_fixtures import load, mirror, oc20_data, oracle_config
 
-AUX = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_model_oc20_aux_small.npz")
-OC20_SMALL = os.path.join(os.path.dirname(AUX), "reference_model_oc20_small.npz")
-OC20_STATS = dict(max_atom_type=84, qm9_atom_remap=False, avg_degree=23.395238876342773, avg_num_nodes=77.81317)
+AUX = "reference_model_oc20_aux_small.npz"
 CASES = ["nonlinear", "linear"]
 
 
-@pytest.fixture(scope="module")
-def gold():
-    return np.load(AUX)
-
-
-def _cfg(g, case):
-    cfg = {k[4:]: g[k].tolist() for k in g.files if k.startswith("cfg/")}
-    cfg["fc_neurons"] = list(cfg["fc_neurons"])
-    cfg["nonlinear_message"] = case == "nonlinear"
-    return cfg
-
-
-def _state(g, case):
-    head = f"{case}/state/"
-    return {k[len(head):]: torch.from_numpy(g[k]) for k in g.files if k.startswith(head)}
-
-
-def _grads(g, case):
-    head = f"{case}/grad/"
-    return {k[len(head):]: torch.from_numpy(g[k]) for k in g.files if k.startswith(head)}
+def _load(case):
+    """The run of one case and its constructor arguments: both runs share the file's ``cfg/`` and differ only in
+    ``nonlinear_message``."""
+    run = load(AUX, case)
+    return run, dict(run.cfg, nonlinear_message=case == "nonlinear")
 
 
 def _mirror(cfg, state):
     from equiformer_b200.nets.graph_attention_transformer_oc20 import GraphAttentionTransformerOC20
-    model = GraphAttentionTransformerOC20(None, None, 1, **cfg)
-    res = model.load_state_dict(state, strict=False)
-    assert not res.unexpected_keys and all(k.endswith("tp.output_mask") for k in res.missing_keys), res
-    return model.eval()
-
-
-def _data(g, dev=None, dtype=torch.float64):
-    t = lambda k: torch.from_numpy(g[k])
-    d = types.SimpleNamespace(pos=t("pos").to(dtype), cell=t("cell").to(dtype), batch=t("batch"), atomic_numbers=t("z"),
-                              tags=t("tags"), n_graphs=2)
-    if dev is not None:
-        for k, v in vars(d).items():
-            if isinstance(v, torch.Tensor):
-                setattr(d, k, v.to(dev))
-    return d
-
-
-def _oracle_cfg(cfg):
-    return R.Config(irreps_node_embedding=cfg["irreps_node_embedding"], irreps_sh=cfg["irreps_sh"],
-                    irreps_head=cfg["irreps_head"], irreps_mlp_mid=cfg["irreps_mlp_mid"],
-                    irreps_feature=cfg["irreps_feature"], num_heads=cfg["num_heads"], num_layers=cfg["num_layers"],
-                    max_radius=cfg["max_radius"], number_of_basis=cfg["number_of_basis"],
-                    nonlinear_message=cfg["nonlinear_message"], **OC20_STATS)
+    return mirror(GraphAttentionTransformerOC20, cfg, state, None, None, 1)
 
 
 # ------------------------------------------------------------------------------------------- model construction (CPU)
 
 @pytest.mark.parametrize("case", CASES)
-def test_mirror_loads_reference_aux_state_dict(gold, case):
+def test_mirror_loads_reference_aux_state_dict(case):
     """The reference's ``state_dict`` loads with only ``tp.output_mask`` buffers missing, and the ``auxiliary_head.*``
     parameters have the reference's names and shapes."""
-    state = _state(gold, case)
-    model = _mirror(_cfg(gold, case), state)
+    run, cfg = _load(case)
+    state = run.state
+    model = _mirror(cfg, state)
     ours = {k: tuple(p.shape) for k, p in model.named_parameters() if k.startswith("auxiliary_head.")}
     ref = {k: tuple(v.shape) for k, v in state.items() if k.startswith("auxiliary_head.") and k in dict(model.named_parameters())}
     assert ours and ours == ref
-    assert all(k in ours for k in _grads(gold, case) if k.startswith("auxiliary_head."))
+    assert all(k in ours for k in run.grads if k.startswith("auxiliary_head."))
     assert str(model.auxiliary_head.proj.irreps_out) == "1x1e"        # no 1o block in 32x0e+16x1e
 
 
 def test_aux_off_model_is_unchanged():
     """Without the option there is no ``auxiliary_head`` and the keys are the reference's aux-off keys."""
-    g = np.load(OC20_SMALL)
-    cfg = {k[4:]: g[k].tolist() for k in g.files if k.startswith("cfg/")}
-    cfg["fc_neurons"] = list(cfg["fc_neurons"])
+    small = load("reference_model_oc20_small.npz")
+    cfg = small.cfg
     from equiformer_b200.nets.graph_attention_transformer_oc20 import GraphAttentionTransformerOC20
     off = GraphAttentionTransformerOC20(None, None, 1, **cfg)
     on = GraphAttentionTransformerOC20(None, None, 1, **dict(cfg, use_auxiliary_task=True))
     assert not hasattr(off, "auxiliary_head")
     keys_off = set(off.state_dict())
     assert keys_off == {k for k in on.state_dict() if not k.startswith("auxiliary_head.")}
-    ref = {k[6:] for k in g.files if k.startswith("state/")}
+    ref = set(small.state)
     assert ref <= keys_off and all(k.endswith("tp.output_mask") for k in keys_off - ref)
 
 
@@ -134,40 +92,41 @@ def test_aux_configuration_dicts():
 # ---------------------------------------------------------------------------------------- parity with the reference file
 
 @pytest.mark.parametrize("case", CASES)
-def test_oracle_aux_matches_reference_model_file(gold, case):
-    cfg = _cfg(gold, case)
+def test_oracle_aux_matches_reference_model_file(case):
+    run, cfg = _load(case)
     params = {k: v.requires_grad_(v.is_floating_point() and v.numel() > 0)
-              for k, v in R.cast_params(_state(gold, case), torch.float64).items()}
-    t = lambda k: torch.from_numpy(gold[k])
+              for k, v in R.cast_params(run.state, torch.float64).items()}
+    t = run.t
     edge = t("edge_index")
-    energy, aux = OA.model_forward_oc20_aux(params, _oracle_cfg(cfg), t("pos").double(), t("cell").double(), t("batch"),
-                                            t("z"), t("tags"), 2, edge[0], edge[1], t("cell_offsets"), cfg["irreps_pre_attn"])
-    assert rel_err(energy, t(f"{case}/energy")) < 1e-10
-    assert rel_err(aux, t(f"{case}/aux")) < 1e-10
-    ((t(f"{case}/c").double() * energy).sum() + (t(f"{case}/W").double() * aux).sum()).backward()
-    for k, ref in _grads(gold, case).items():
+    energy, aux = OA.model_forward_oc20_aux(params, oracle_config("oc20", cfg), t("pos").double(), t("cell").double(),
+                                            t("batch"), t("z"), t("tags"), 2, edge[0], edge[1], t("cell_offsets"),
+                                            cfg["irreps_pre_attn"])
+    assert rel_err(energy, t("energy")) < 1e-10
+    assert rel_err(aux, t("aux")) < 1e-10
+    ((t("c").double() * energy).sum() + (t("W").double() * aux).sum()).backward()
+    for k, ref in run.grads.items():
         assert rel_err(params[k].grad, ref) < 1e-6, k
 
 
 @pytest.mark.parametrize("case", CASES)
-def test_mirror_aux_matches_reference_model_file(gold, case):
+def test_mirror_aux_matches_reference_model_file(case):
     """The mirror (own periodic neighbour list, kernels emulated in float64): same edge list as the fixture's, energy and
     aux 1e-10, parameter gradients 1e-6."""
     from equiformer_b200.graph import radius_graph_pbc
     from tests._emulation import emulated_kernels
-    cfg = _cfg(gold, case)
-    model = _mirror(cfg, _state(gold, case)).double()
-    data = _data(gold)
+    run, cfg = _load(case)
+    model = _mirror(cfg, run.state).double()
+    data = oc20_data(run)
     edge, offs, _d2 = radius_graph_pbc(data.pos.float(), data.batch, data.cell.float(), cfg["max_radius"], cfg["max_neighbors"])
-    assert torch.equal(edge, torch.from_numpy(gold["edge_index"]))
-    assert torch.equal(offs.long(), torch.from_numpy(gold["cell_offsets"]).long())
-    t = lambda k: torch.from_numpy(gold[k])
+    assert torch.equal(edge, run.t("edge_index"))
+    assert torch.equal(offs.long(), run.t("cell_offsets").long())
+    t = run.t
     with emulated_kernels():
         energy, aux = model(data)
-        ((t(f"{case}/c").double() * energy).sum() + (t(f"{case}/W").double() * aux).sum()).backward()
-    assert rel_err(energy, t(f"{case}/energy")) < 1e-10
-    assert rel_err(aux, t(f"{case}/aux")) < 1e-10
-    for k, ref in _grads(gold, case).items():
+        ((t("c").double() * energy).sum() + (t("W").double() * aux).sum()).backward()
+    assert rel_err(energy, t("energy")) < 1e-10
+    assert rel_err(aux, t("aux")) < 1e-10
+    for k, ref in run.grads.items():
         assert rel_err(model.get_parameter(k).grad, ref) < 1e-6, k
 
 
@@ -223,19 +182,19 @@ def test_interpolation_is_seeded_moves_only_tagged_atoms_of_drawn_frames():
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("case", CASES)
-def test_cuda_aux_matches_reference_model_file(gold, case, cuda_device):
+def test_cuda_aux_matches_reference_model_file(case, cuda_device):
     from equiformer_b200.graph import radius_graph_pbc
-    cfg = _cfg(gold, case)
-    model = _mirror(cfg, _state(gold, case)).to(cuda_device)
-    data = _data(gold, cuda_device, torch.float32)
+    run, cfg = _load(case)
+    model = _mirror(cfg, run.state).to(cuda_device)
+    data = oc20_data(run, cuda_device, torch.float32)
     edge, offs, _d2 = radius_graph_pbc(data.pos, data.batch, data.cell, cfg["max_radius"], cfg["max_neighbors"])
-    assert torch.equal(edge.cpu(), torch.from_numpy(gold["edge_index"]))
-    t = lambda k: torch.from_numpy(gold[k])
+    assert torch.equal(edge.cpu(), run.t("edge_index"))
+    t = run.t
     energy, aux = model(data)
-    ((t(f"{case}/c").to(cuda_device) * energy).sum() + (t(f"{case}/W").to(cuda_device) * aux).sum()).backward()
-    assert rel_err(energy, t(f"{case}/energy")) < 1e-4
-    assert rel_err(aux, t(f"{case}/aux")) < 1e-4
-    worst = max(rel_err(model.get_parameter(k).grad, ref) for k, ref in _grads(gold, case).items())
+    ((t("c", cuda_device) * energy).sum() + (t("W", cuda_device) * aux).sum()).backward()
+    assert rel_err(energy, t("energy")) < 1e-4
+    assert rel_err(aux, t("aux")) < 1e-4
+    worst = max(rel_err(model.get_parameter(k).grad, ref) for k, ref in run.grads.items())
     assert worst < 1e-3, worst
 
 

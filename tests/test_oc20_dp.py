@@ -17,20 +17,16 @@ from __future__ import annotations
 
 import json
 import os
-import types
 
-import numpy as np
 import pytest
 import torch
 
-from oracle import equiformer_ref as R
 from tests import _emulation as emu
 from tests.helpers import rel_err
+from tests.reference_fixtures import GOLDEN, load, mirror, oc20_data, oracle_config, run_mirror, run_oracle, worst_grad
 
-GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
-FIXTURE = os.path.join(GOLDEN, "reference_model_oc20_dp_small.npz")
+FIXTURE = "reference_model_oc20_dp_small.npz"
 SHAPES = os.path.join(GOLDEN, "reference_state_shapes_oc20_dp.json")
-OC20_STATS = dict(max_atom_type=84, qm9_atom_remap=False, avg_degree=23.395238876342773, avg_num_nodes=77.81317)
 TOL = 2e-5                      # kernel vs the float32 chain
 
 # head layouts (irreps of H heads, sorted and simplified): (H, ds, Cs)
@@ -90,76 +86,32 @@ def test_unsupported_options_raise(option):
 
 
 # ------------------------------------------------------------------------------------------------ reference fixture
-def _fixture():
-    g = np.load(FIXTURE)
-    cfg = {k[4:]: g[k].tolist() for k in g.files if k.startswith("cfg/")}
-    state = {k[6:]: torch.from_numpy(g[k]) for k in g.files if k.startswith("state/")}
-    return g, cfg, state
-
-
-def _mirror(cfg, state):
+def _mirror(case):
     from equiformer_b200.nets.dp_attention_transformer_oc20 import DotProductAttentionTransformerOC20
-    cfg = dict(cfg, fc_neurons=list(cfg["fc_neurons"]))
-    model = DotProductAttentionTransformerOC20(None, None, 1, **cfg)
-    res = model.load_state_dict(state, strict=False)
-    assert not res.unexpected_keys and all(k.endswith("tp.output_mask") for k in res.missing_keys), res
-    return model.eval()
-
-
-def _data(g, dev=None, dtype=torch.float64):
-    t = lambda k: torch.from_numpy(g[k])
-    d = types.SimpleNamespace(pos=t("pos").to(dtype), cell=t("cell").to(dtype), batch=t("batch"), atomic_numbers=t("z"),
-                              tags=t("tags"), n_graphs=2)
-    if dev is not None:
-        for k, v in vars(d).items():
-            if isinstance(v, torch.Tensor):
-                setattr(d, k, v.to(dev))
-    return d
-
-
-def _worst_grad(named_grads: dict, g) -> float:
-    keys = [k[5:] for k in g.files if k.startswith("grad/")]
-    assert len(keys) > 50
-    worst = 0.0
-    for k in keys:
-        ref = torch.from_numpy(g[f"grad/{k}"]).double()
-        got = named_grads[k]
-        assert got is not None, k
-        worst = max(worst, float((got.detach().double().cpu() - ref).abs().max() / ref.abs().max().clamp_min(1e-12)))
-    return worst
+    return mirror(DotProductAttentionTransformerOC20, case.cfg, case.state, None, None, 1)
 
 
 def test_oracle_matches_reference_dp_oc20_model_file():
-    g, cfg, state = _fixture()
-    ocfg = R.Config(irreps_node_embedding=cfg["irreps_node_embedding"], irreps_sh=cfg["irreps_sh"],
-                    irreps_head=cfg["irreps_head"], irreps_mlp_mid=cfg["irreps_mlp_mid"],
-                    irreps_feature=cfg["irreps_feature"], num_heads=cfg["num_heads"], num_layers=cfg["num_layers"],
-                    max_radius=cfg["max_radius"], number_of_basis=cfg["number_of_basis"], nonlinear_message=False,
-                    attention="dot_product", **OC20_STATS)
-    params = {k: v.requires_grad_(v.is_floating_point() and v.numel() > 0) for k, v in R.cast_params(state, torch.float64).items()}
-    t = lambda k: torch.from_numpy(g[k])
-    edge = t("edge_index")
-    energy = R.model_forward_oc20(params, ocfg, t("pos").double(), t("cell").double(), t("batch"), t("z"), t("tags"), 2,
-                                  edge[0], edge[1], t("cell_offsets"))
-    assert rel_err(energy.detach(), t("energy")) < 1e-11
-    (energy ** 2).sum().backward()
-    assert _worst_grad({k: v.grad for k, v in params.items()}, g) < 1e-8
+    case = load(FIXTURE)
+    energy, _forces, params = run_oracle("oc20", case, oracle_config("oc20", case.cfg, attention="dot_product"))
+    assert rel_err(energy.detach(), case.t("energy")) < 1e-11
+    assert worst_grad({k: v.grad for k, v in params.items()}, case.grads, 51) < 1e-8
 
 
 def test_mirror_with_emulated_kernels_matches_reference_dp_oc20_model_file():
     """float64 CPU stand-ins: the predicate of the fused kernel is false, so the existing chain runs."""
     from equiformer_b200.graph import radius_graph_pbc
     from tests._emulation import emulated_kernels
-    g, cfg, state = _fixture()
-    model = _mirror(cfg, state).double()
-    data = _data(g)
-    edge, offs, _d2 = radius_graph_pbc(data.pos.float(), data.batch, data.cell.float(), cfg["max_radius"], cfg["max_neighbors"])
-    assert torch.equal(edge, torch.from_numpy(g["edge_index"]))
+    case = load(FIXTURE)
+    model = _mirror(case).double()
+    data = oc20_data(case)
+    edge, offs, _d2 = radius_graph_pbc(data.pos.float(), data.batch, data.cell.float(), case.cfg["max_radius"],
+                                       case.cfg["max_neighbors"])
+    assert torch.equal(edge, case.t("edge_index"))
     with emulated_kernels():
-        energy = model(data)
-        (energy ** 2).sum().backward()
-    assert rel_err(energy.detach(), torch.from_numpy(g["energy"])) < 1e-10
-    assert _worst_grad({k: p.grad for k, p in model.named_parameters()}, g) < 1e-7
+        energy, _forces = run_mirror("oc20", model, case)
+    assert rel_err(energy.detach(), case.t("energy")) < 1e-10
+    assert worst_grad({k: p.grad for k, p in model.named_parameters()}, case.grads, 51) < 1e-7
 
 
 # ------------------------------------------------------------------------------------------------ host logic (float64)
@@ -327,8 +279,8 @@ def test_double_backward_matches_the_chain(cuda_device, masked):
 @pytest.mark.gpu
 def test_cuda_dp_oc20_model_matches_reference_model_file(cuda_device):
     from equiformer_b200 import ops
-    g, cfg, state = _fixture()
-    model = _mirror(cfg, state).to(cuda_device)
+    case = load(FIXTURE)
+    model = _mirror(case).to(cuda_device)
     calls = []
     orig = ops.dot_softmax_aggregate_raw
 
@@ -338,13 +290,13 @@ def test_cuda_dp_oc20_model_matches_reference_model_file(cuda_device):
 
     ops.dot_softmax_aggregate_raw = counting
     try:
-        energy = model(_data(g, cuda_device, torch.float32))
+        energy = model(oc20_data(case, cuda_device, torch.float32))
     finally:
         ops.dot_softmax_aggregate_raw = orig
-    assert len(calls) == cfg["num_layers"]
-    assert rel_err(energy, torch.from_numpy(g["energy"])) < 5e-5
+    assert len(calls) == case.cfg["num_layers"]
+    assert rel_err(energy, case.t("energy")) < 5e-5
     (energy ** 2).sum().backward()
-    assert _worst_grad({k: p.grad for k, p in model.named_parameters()}, g) < 1e-3
+    assert worst_grad({k: p.grad for k, p in model.named_parameters()}, case.grads, 51) < 1e-3
 
 
 @pytest.mark.gpu

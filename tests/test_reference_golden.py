@@ -20,51 +20,52 @@ import torch
 from oracle import e3nn_ref as e3
 from oracle import equiformer_ref as R
 from tests.helpers import assert_same_grad_presence, rel_err
+from tests.reference_fixtures import (GOLDEN, dens_setup, load, load_state, mirror, oc20_data, oracle_config, run_mirror,
+                                      run_oracle, worst_grad)
 
-FIXTURE = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_modules.npz")
+FIXTURE = "reference_modules.npz"
 LN_CASES = ["qm9_l2", "md17_l3", "oc20_l1", "ffn_mid"]
 
 
 @pytest.fixture(scope="module")
 def gold():
-    return np.load(FIXTURE)
+    return np.load(os.path.join(GOLDEN, FIXTURE))
 
 
-def _state(gold, prefix, dtype=torch.float64):
-    head = f"{prefix}/state/"
-    return {k[len(head):]: torch.from_numpy(gold[k]).to(dtype) for k in gold.files if k.startswith(head)}
+def _state(prefix, dtype=torch.float64):
+    return {k: v.to(dtype) for k, v in load(FIXTURE, prefix).state.items()}
 
 
 def _t(gold, key, dtype=torch.float64):
     return torch.from_numpy(gold[key]).to(dtype)
 
 
-def _params(gold, prefix, name="m"):
-    return {f"{name}.{k}": v for k, v in _state(gold, prefix).items()}
+def _params(prefix, name="m"):
+    return {f"{name}.{k}": v for k, v in _state(prefix).items()}
 
 
 # ------------------------------------------------------------------------------------------------ oracle (CPU, fp64)
 
 def test_oracle_gaussian_rbf_matches_reference(gold):
-    out = R.gaussian_rbf(_params(gold, "gaussian_rbf"), "m", _t(gold, "gaussian_rbf/dist"), float(gold["gaussian_rbf/cutoff"]))
+    out = R.gaussian_rbf(_params("gaussian_rbf"), "m", _t(gold, "gaussian_rbf/dist"), float(gold["gaussian_rbf/cutoff"]))
     assert rel_err(out, _t(gold, "gaussian_rbf/y")) < 1e-12
 
 
 def test_oracle_expnorm_rbf_matches_reference(gold):
-    out = R.expnorm_rbf(_params(gold, "expnorm_rbf"), "m", _t(gold, "expnorm_rbf/dist"), float(gold["expnorm_rbf/cutoff"]))
+    out = R.expnorm_rbf(_params("expnorm_rbf"), "m", _t(gold, "expnorm_rbf/dist"), float(gold["expnorm_rbf/cutoff"]))
     assert rel_err(out, _t(gold, "expnorm_rbf/y")) < 1e-12
 
 
 @pytest.mark.parametrize("tag", ["qm9", "small"])
 def test_oracle_radial_profile_matches_reference(gold, tag):
-    out = R.radial_profile(_params(gold, f"radial_profile_{tag}"), "m", _t(gold, f"radial_profile_{tag}/x"))
+    out = R.radial_profile(_params(f"radial_profile_{tag}"), "m", _t(gold, f"radial_profile_{tag}/x"))
     assert rel_err(out, _t(gold, f"radial_profile_{tag}/y")) < 1e-12
 
 
 @pytest.mark.parametrize("tag", LN_CASES)
 def test_oracle_layer_norm_matches_reference(gold, tag):
     irreps = e3.parse_irreps(str(gold[f"layer_norm_{tag}/irreps"]))
-    out = R.layer_norm_v2(_params(gold, f"layer_norm_{tag}"), "m", irreps, _t(gold, f"layer_norm_{tag}/x"),
+    out = R.layer_norm_v2(_params(f"layer_norm_{tag}"), "m", irreps, _t(gold, f"layer_norm_{tag}/x"),
                           float(gold[f"layer_norm_{tag}/eps"]))
     assert rel_err(out, _t(gold, f"layer_norm_{tag}/y")) < 1e-12
 
@@ -83,7 +84,7 @@ def _mirror(kind, gold, tag=None):
     else:
         prefix = f"layer_norm_{tag}"
         m = layer_norm.EquivariantLayerNormV2(str(gold[f"{prefix}/irreps"]), eps=float(gold[f"{prefix}/eps"]))
-    missing = m.load_state_dict(_state(gold, prefix, torch.float32), strict=True)      # the reference's own keys and shapes
+    missing = m.load_state_dict(_state(prefix, torch.float32), strict=True)      # the reference's own keys and shapes
     assert not missing.missing_keys and not missing.unexpected_keys
     return m, prefix
 
@@ -123,20 +124,8 @@ def test_cuda_path_matches_reference(gold, cuda_device, kind, tag, x_key, tol):
 
 # ------------------------------------------------- the reference's model file end to end (reference_model_small.npz)
 
-SMALL = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_model_small.npz")
-
-
-def _small_case():
-    g = np.load(SMALL)
-    head = "state/"
-    state = {k[len(head):]: torch.from_numpy(g[k]) for k in g.files if k.startswith(head)}
-    cfg = R.Config(irreps_node_embedding=str(g["cfg/irreps_node_embedding"]), irreps_sh=str(g["cfg/irreps_sh"]),
-                   irreps_head=str(g["cfg/irreps_head"]), irreps_mlp_mid=str(g["cfg/irreps_mlp_mid"]),
-                   irreps_feature=str(g["cfg/irreps_feature"]), num_heads=int(g["cfg/num_heads"]),
-                   num_layers=int(g["cfg/num_layers"]), max_radius=float(g["cfg/max_radius"]),
-                   number_of_basis=int(g["cfg/number_of_basis"]), basis_type="gaussian",
-                   nonlinear_message=bool(g["cfg/nonlinear_message"]))
-    return g, state, cfg
+SMALL = "reference_model_small.npz"
+MD17_SMALL = "reference_model_md17_small.npz"
 
 
 def test_oracle_model_matches_reference_model_file():
@@ -144,42 +133,22 @@ def test_oracle_model_matches_reference_model_file():
     radius-graph calls served by the oracle's restatements - see the generator) vs ``oracle.model_forward`` fed the
     reference's ``state_dict``: pins instruction lists, irreps sorting, rescale and bias handling, head reshapes,
     attention wiring, residuals and scale factors of the restatement.  Both sides are float64."""
-    g, state, cfg = _small_case()
-    params = R.cast_params(state, torch.float64)
-    pos, batch, z = torch.from_numpy(g["pos"]).double(), torch.from_numpy(g["batch"]), torch.from_numpy(g["z"])
-    energy = R.model_forward(params, cfg, pos, batch, z, n_graphs=2)
-    assert rel_err(energy, torch.from_numpy(g["energy"])) < 1e-11
+    case = load(SMALL)
+    params = R.cast_params(case.state, torch.float64)
+    pos, batch, z = case.t("pos", dtype=torch.float64), case.t("batch"), case.t("z")
+    energy = R.model_forward(params, oracle_config("qm9", case.cfg), pos, batch, z, n_graphs=2)
+    assert rel_err(energy, case.t("energy")) < 1e-11
 
 
 def test_oracle_md17_model_matches_reference_model_file():
     """The same for ``nets/graph_attention_transformer_md17.py`` (Lmax = 3, exp-normal basis, forces = -dE/dpos by
     autograd through the reference's own forward) vs ``oracle.energy_and_forces``."""
-    g = np.load(os.path.join(os.path.dirname(SMALL), "reference_model_md17_small.npz"))
-    head = "state/"
-    state = {k[len(head):]: torch.from_numpy(g[k]) for k in g.files if k.startswith(head)}
-    cfg = R.Config(irreps_node_embedding=str(g["cfg/irreps_node_embedding"]), irreps_sh=str(g["cfg/irreps_sh"]),
-                   irreps_head=str(g["cfg/irreps_head"]), irreps_mlp_mid=str(g["cfg/irreps_mlp_mid"]),
-                   irreps_feature=str(g["cfg/irreps_feature"]), num_heads=int(g["cfg/num_heads"]),
-                   num_layers=int(g["cfg/num_layers"]), max_radius=float(g["cfg/max_radius"]),
-                   number_of_basis=int(g["cfg/number_of_basis"]), basis_type="exp",
-                   nonlinear_message=bool(g["cfg/nonlinear_message"]), max_atom_type=64, qm9_atom_remap=False)
-    params = R.cast_params(state, torch.float64)
-    pos, batch, z = torch.from_numpy(g["pos"]).double(), torch.from_numpy(g["batch"]), torch.from_numpy(g["z"])
-    energy, forces = R.energy_and_forces(params, cfg, pos, batch, z, n_graphs=1)
-    assert rel_err(energy, torch.from_numpy(g["energy"])) < 1e-11
-    assert rel_err(forces, torch.from_numpy(g["forces"])) < 1e-10
-
-
-def _mirror_model(g, cls, extra=()):
-    cfg = {k[len("cfg/"):]: g[k] for k in g.files if k.startswith("cfg/")}
-    kw = {k: (str(v) if v.dtype.kind in "US" else bool(v) if v.dtype.kind == "b" else
-              [int(c) for c in v] if v.ndim == 1 else int(v) if v.dtype.kind == "i" else float(v)) for k, v in cfg.items()}
-    model = cls(**kw)
-    state = {k[len("state/"):]: torch.from_numpy(g[k]) for k in g.files if k.startswith("state/")}
-    res = model.load_state_dict(state, strict=False)
-    # e3nn's TensorProduct also registers an `output_mask` buffer, which the generator's stub does not carry
-    assert not res.unexpected_keys and all(k.endswith("tp.output_mask") for k in res.missing_keys), (res, extra)
-    return model.eval()
+    case = load(MD17_SMALL)
+    params = R.cast_params(case.state, torch.float64)
+    pos, batch, z = case.t("pos", dtype=torch.float64), case.t("batch"), case.t("z")
+    energy, forces = R.energy_and_forces(params, oracle_config("md17", case.cfg), pos, batch, z, n_graphs=1)
+    assert rel_err(energy, case.t("energy")) < 1e-11
+    assert rel_err(forces, case.t("forces")) < 1e-10
 
 
 def test_mirror_models_take_the_reference_state_dict():
@@ -187,8 +156,9 @@ def test_mirror_models_take_the_reference_state_dict():
     host-side mirrors: the drop-in property of the module API, checked on the CPU."""
     from equiformer_b200.nets.graph_attention_transformer import GraphAttentionTransformer
     from equiformer_b200.nets.graph_attention_transformer_md17 import GraphAttentionTransformerMD17
-    _mirror_model(np.load(SMALL), GraphAttentionTransformer)
-    _mirror_model(np.load(os.path.join(os.path.dirname(SMALL), "reference_model_md17_small.npz")), GraphAttentionTransformerMD17)
+    for name, cls in ((SMALL, GraphAttentionTransformer), (MD17_SMALL, GraphAttentionTransformerMD17)):
+        case = load(name)
+        mirror(cls, case.cfg, case.state)
 
 
 @pytest.mark.gpu
@@ -197,13 +167,13 @@ def test_cuda_model_matches_reference_model_file(cuda_device):
     reference's ``state_dict``, against the energy the reference's own model file produced; float32 vs a float64
     fixture, two blocks deep: 5e-5 of max|E|."""
     from equiformer_b200.nets.graph_attention_transformer import GraphAttentionTransformer
-    g = np.load(SMALL)
-    model = _mirror_model(g, GraphAttentionTransformer).to(cuda_device)
-    pos = torch.from_numpy(g["pos"]).to(cuda_device)
-    batch, z = torch.from_numpy(g["batch"]).to(cuda_device), torch.from_numpy(g["z"]).to(cuda_device)
+    case = load(SMALL)
+    model = mirror(GraphAttentionTransformer, case.cfg, case.state).to(cuda_device)
+    pos = case.t("pos", cuda_device)
+    batch, z = case.t("batch", cuda_device), case.t("z", cuda_device)
     with torch.no_grad():
         energy = model(f_in=None, pos=pos, batch=batch, node_atom=z)
-    assert rel_err(energy, torch.from_numpy(g["energy"])) < 5e-5
+    assert rel_err(energy, case.t("energy")) < 5e-5
 
 
 @pytest.mark.gpu
@@ -211,16 +181,16 @@ def test_cuda_md17_model_matches_reference_model_file(cuda_device):
     """Energy and forces (``-dE/dpos`` through the closed autograd families) of the MD17 mirror on CUDA against the
     reference's own MD17 model file: 5e-5 / 2e-4 relative to the largest component."""
     from equiformer_b200.nets.graph_attention_transformer_md17 import GraphAttentionTransformerMD17
-    g = np.load(os.path.join(os.path.dirname(SMALL), "reference_model_md17_small.npz"))
-    model = _mirror_model(g, GraphAttentionTransformerMD17).to(cuda_device)
-    pos = torch.from_numpy(g["pos"]).to(cuda_device)
-    batch, z = torch.from_numpy(g["batch"]).to(cuda_device), torch.from_numpy(g["z"]).to(cuda_device)
+    case = load(MD17_SMALL)
+    model = mirror(GraphAttentionTransformerMD17, case.cfg, case.state).to(cuda_device)
+    pos = case.t("pos", cuda_device)
+    batch, z = case.t("batch", cuda_device), case.t("z", cuda_device)
     energy, forces = model(node_atom=z, pos=pos, batch=batch)
-    assert rel_err(energy.detach(), torch.from_numpy(g["energy"])) < 5e-5
-    assert rel_err(forces.detach(), torch.from_numpy(g["forces"])) < 2e-4
+    assert rel_err(energy.detach(), case.t("energy")) < 5e-5
+    assert rel_err(forces.detach(), case.t("forces")) < 2e-4
 
 
-SHAPES = os.path.join(os.path.dirname(SMALL), "reference_state_shapes.json")
+SHAPES = os.path.join(GOLDEN, "reference_state_shapes.json")
 
 
 def _shape_table():
@@ -243,25 +213,28 @@ def test_registered_models_have_the_reference_parameters(name):
     assert mine == ref
 
 
-HEADLINE = os.path.join(os.path.dirname(SMALL), "reference_model_headline.npz")
+HEADLINE = "reference_model_headline.npz"
 
 
-def _headline_state():
-    """state_dict of the headline model as the generator set it: small tensors verbatim, large ones from the closed form"""
+def _closed_form_state(g, shapes):
+    """state_dict as the generator set it: small tensors verbatim, large ones from the closed form"""
     from tests.helpers import closed_form_tensor
-    g = np.load(HEADLINE)
-    shapes = _shape_table()["graph_attention_transformer_nonlinear_l2"]
     state = {}
     for k, shape in shapes.items():
-        if f"small/{k}" in g.files:
+        if f"small/{k}" in g:
             state[k] = torch.from_numpy(g[f"small/{k}"])
-        elif f"stat/{k}" in g.files:
+        elif f"stat/{k}" in g:
             mean, std = (float(v) for v in g[f"stat/{k}"])
             state[k] = closed_form_tensor(k, shape, mean, std)
         else:
             state[k] = torch.zeros(shape)          # e3nn's empty `tp.weight` buffers of externally weighted products
             assert state[k].numel() == 0, k
-    return g, state
+    return state
+
+
+def _headline_state():
+    g = load(HEADLINE).arrays
+    return g, _closed_form_state(g, _shape_table()["graph_attention_transformer_nonlinear_l2"])
 
 
 def test_oracle_headline_model_matches_reference_model_file():
@@ -283,9 +256,7 @@ def test_cuda_headline_model_matches_reference_model_file(cuda_device):
     from equiformer_b200.nets import model_entrypoint
     g, state = _headline_state()
     model = model_entrypoint("graph_attention_transformer_nonlinear_l2")(irreps_in="5x0e", radius=5.0, num_basis=128)
-    res = model.load_state_dict(state, strict=False)
-    assert not res.unexpected_keys and all(k.endswith("tp.output_mask") for k in res.missing_keys)
-    model = model.eval().to(cuda_device)
+    model = load_state(model, state).eval().to(cuda_device)
     pos = torch.from_numpy(g["pos"]).to(cuda_device)
     batch, z = torch.from_numpy(g["batch"]).to(cuda_device), torch.from_numpy(g["z"]).to(cuda_device)
     with torch.no_grad():
@@ -313,8 +284,7 @@ def test_cuda_headline_model_matches_reference_through_tcgen05_gemms(cuda_device
     from equiformer_b200.nets import model_entrypoint
     g, state = _headline_state()
     model = model_entrypoint("graph_attention_transformer_nonlinear_l2")(irreps_in="5x0e", radius=5.0, num_basis=128)
-    model.load_state_dict(state, strict=False)
-    model = model.eval().to(cuda_device)
+    model = load_state(model, state).eval().to(cuda_device)
     pos = torch.from_numpy(g["pos"]).to(cuda_device)
     batch, z = torch.from_numpy(g["batch"]).to(cuda_device), torch.from_numpy(g["z"]).to(cuda_device)
     prof = ops.KernelProfile(time_events=False)
@@ -350,27 +320,22 @@ def test_cuda_small_model_gradients_through_tcgen05_gemms_match_oracle(cuda_devi
     ref = R.model_forward(params, R.Config(), pos.double(), batch, z, 5)
     ref.sum().backward()
     assert rel_err(out, ref) < 1e-4
-    errs = []
-    for k, p in model.named_parameters():
-        gref = params[k].grad
-        if not assert_same_grad_presence(k, p.grad, gref):
-            continue
-        errs.append((((p.grad.double().cpu() - gref).abs().max() / gref.abs().max().clamp_min(1e-12)).item(), k))
-    errs.sort(reverse=True)
-    assert errs[0][0] < 1e-3, errs[:5]
+    grads = {k: p.grad for k, p in model.named_parameters()}
+    ref = {k: params[k].grad for k, g in grads.items() if assert_same_grad_presence(k, g, params[k].grad)}
+    assert worst_grad(grads, ref, 1) < 1e-3
 
 
 @pytest.mark.gpu
 def test_cuda_md17_model_matches_reference_through_tcgen05_gemms(cuda_device, tensor_core_gemms_everywhere):
     """Energy and forces of the MD17 fixture (a double-backward-capable path) with the wgmma kernels forced on."""
     from equiformer_b200.nets.graph_attention_transformer_md17 import GraphAttentionTransformerMD17
-    g = np.load(os.path.join(os.path.dirname(SMALL), "reference_model_md17_small.npz"))
-    model = _mirror_model(g, GraphAttentionTransformerMD17).to(cuda_device)
-    pos = torch.from_numpy(g["pos"]).to(cuda_device)
-    batch, z = torch.from_numpy(g["batch"]).to(cuda_device), torch.from_numpy(g["z"]).to(cuda_device)
+    case = load(MD17_SMALL)
+    model = mirror(GraphAttentionTransformerMD17, case.cfg, case.state).to(cuda_device)
+    pos = case.t("pos", cuda_device)
+    batch, z = case.t("batch", cuda_device), case.t("z", cuda_device)
     energy, forces = model(node_atom=z, pos=pos, batch=batch)
-    assert rel_err(energy.detach(), torch.from_numpy(g["energy"])) < 5e-5
-    assert rel_err(forces.detach(), torch.from_numpy(g["forces"])) < 2e-4
+    assert rel_err(energy.detach(), case.t("energy")) < 5e-5
+    assert rel_err(forces.detach(), case.t("forces")) < 2e-4
 
 
 # --------------------------------- host logic of the mirrors (kernels emulated in float64 on the CPU) vs the reference
@@ -383,25 +348,22 @@ def test_mirror_host_logic_matches_reference_model_files():
     from equiformer_b200.nets.graph_attention_transformer_md17 import GraphAttentionTransformerMD17
     from tests._emulation import emulated_kernels
 
-    g = np.load(SMALL)
-    model = _mirror_model(g, GraphAttentionTransformer).double()
+    case = load(SMALL)
+    model = mirror(GraphAttentionTransformer, case.cfg, case.state).double()
     with emulated_kernels(), torch.no_grad():
-        energy = model(f_in=None, pos=torch.from_numpy(g["pos"]).double(), batch=torch.from_numpy(g["batch"]),
-                       node_atom=torch.from_numpy(g["z"]))
-    assert rel_err(energy, torch.from_numpy(g["energy"])) < 1e-10
+        energy = model(f_in=None, pos=case.t("pos", dtype=torch.float64), batch=case.t("batch"), node_atom=case.t("z"))
+    assert rel_err(energy, case.t("energy")) < 1e-10
 
-    g = np.load(os.path.join(os.path.dirname(SMALL), "reference_model_md17_small.npz"))
-    model = _mirror_model(g, GraphAttentionTransformerMD17).double()
+    case = load(MD17_SMALL)
+    model = mirror(GraphAttentionTransformerMD17, case.cfg, case.state).double()
     with emulated_kernels():
-        energy, forces = model(node_atom=torch.from_numpy(g["z"]), pos=torch.from_numpy(g["pos"]).double(),
-                               batch=torch.from_numpy(g["batch"]))
-    assert rel_err(energy.detach(), torch.from_numpy(g["energy"])) < 1e-10
-    assert rel_err(forces.detach(), torch.from_numpy(g["forces"])) < 1e-9
+        energy, forces = model(node_atom=case.t("z"), pos=case.t("pos", dtype=torch.float64), batch=case.t("batch"))
+    assert rel_err(energy.detach(), case.t("energy")) < 1e-10
+    assert rel_err(forces.detach(), case.t("forces")) < 1e-9
 
     g, state = _headline_state()
     model = model_entrypoint("graph_attention_transformer_nonlinear_l2")(irreps_in="5x0e", radius=5.0, num_basis=128)
-    model.load_state_dict(state, strict=False)
-    model = model.eval().double()
+    model = load_state(model, state).eval().double()
     with emulated_kernels(), torch.no_grad():
         energy = model(f_in=None, pos=torch.from_numpy(g["pos"]).double(), batch=torch.from_numpy(g["batch"]),
                        node_atom=torch.from_numpy(g["z"]))
@@ -423,28 +385,16 @@ def test_drop_modules_draw_like_the_reference(gold):
 
 # ------------------------------------------------------------ one block at the OC20 IS2RE l1_256_nonlinear sizes
 
-OC20_BLOCK = os.path.join(os.path.dirname(SMALL), "reference_block_oc20_l1.npz")
+OC20_BLOCK = "reference_block_oc20_l1.npz"
 
 
 def _oc20_block():
     import json
-    from tests.helpers import closed_form_tensor
-    g = np.load(OC20_BLOCK)
-    state = {}
-    for k, shape in json.loads(str(g["shapes"])).items():
-        if f"small/{k}" in g.files:
-            state[k] = torch.from_numpy(g[f"small/{k}"])
-        elif f"stat/{k}" in g.files:
-            mean, std = (float(v) for v in g[f"stat/{k}"])
-            state[k] = closed_form_tensor(k, shape, mean, std)
-        else:
-            state[k] = torch.zeros(shape)
-            assert state[k].numel() == 0, k
-    kw = {k[len("cfg/"):]: (str(g[k]) if g[k].dtype.kind in "US" else bool(g[k]) if g[k].dtype.kind == "b" else
-                            [int(c) for c in g[k]] if g[k].ndim == 1 else int(g[k]) if g[k].dtype.kind == "i" else float(g[k]))
-          for k in g.files if k.startswith("cfg/")}
-    inputs = {k: torch.from_numpy(g[k]) for k in ("x", "edge_src", "edge_dst", "edge_sh", "edge_scalars")}
-    return g, state, kw, inputs
+    block = load(OC20_BLOCK)
+    g = block.arrays
+    state = _closed_form_state(g, json.loads(str(g["shapes"])))
+    inputs = {k: block.t(k) for k in ("x", "edge_src", "edge_dst", "edge_sh", "edge_scalars")}
+    return g, state, block.cfg, inputs
 
 
 def test_oracle_block_matches_reference_at_oc20_sizes():
@@ -465,10 +415,7 @@ def test_mirror_block_host_logic_matches_reference_at_oc20_sizes():
     from equiformer_b200.nets.graph_attention_transformer import TransBlock
     from tests._emulation import emulated_kernels
     g, state, kw, t = _oc20_block()
-    blk = TransBlock(**kw)
-    res = blk.load_state_dict(state, strict=False)
-    assert not res.unexpected_keys and all(k.endswith("tp.output_mask") for k in res.missing_keys)
-    blk = blk.eval().double()
+    blk = mirror(TransBlock, kw, state).double()
     x = t["x"].double()
     with emulated_kernels(), torch.no_grad():
         out = blk(node_input=x, node_attr=torch.ones_like(x[:, :1]), edge_src=t["edge_src"], edge_dst=t["edge_dst"],
@@ -484,9 +431,7 @@ def test_cuda_block_matches_reference_at_oc20_sizes(cuda_device):
     (tests/test_gpu_model.py::test_oc20_l1_layer_vs_oracle).  Written after the round-1 GPU budget ended."""
     from equiformer_b200.nets.graph_attention_transformer import TransBlock
     g, state, kw, t = _oc20_block()
-    blk = TransBlock(**kw)
-    blk.load_state_dict(state, strict=False)
-    blk = blk.eval().to(cuda_device)
+    blk = mirror(TransBlock, kw, state).to(cuda_device)
     d = lambda v: v.to(cuda_device)
     x = d(t["x"])
     with torch.no_grad():
@@ -498,31 +443,18 @@ def test_cuda_block_matches_reference_at_oc20_sizes(cuda_device):
 
 # --------------------------------------------------------------- backward: parameter gradients of the reference's models
 
-def _worst_grad(got: dict, g, n_min: int):
-    keys = [k[len("grad/"):] for k in g.files if k.startswith("grad/")]
-    assert len(keys) >= n_min
-    worst = 0.0
-    for k in keys:
-        ref = torch.from_numpy(g[f"grad/{k}"])
-        assert got[k] is not None, k
-        worst = max(worst, float((got[k].detach().double() - ref).abs().max() / ref.abs().max().clamp_min(1e-12)))
-    return worst
-
-
 def test_parameter_gradients_match_reference_qm9_small():
     """d(sum E^2)/d(parameters) from the reference's own backward through its own forward, vs autograd through the
     oracle and through the mirror (closed autograd families, kernels emulated)."""
     from equiformer_b200.nets.graph_attention_transformer import GraphAttentionTransformer
     from tests._emulation import emulated_kernels
-    g, state, cfg = _small_case()
-    pos, batch, z = torch.from_numpy(g["pos"]).double(), torch.from_numpy(g["batch"]), torch.from_numpy(g["z"])
-    params = {k: v.requires_grad_(v.is_floating_point()) for k, v in R.cast_params(state, torch.float64).items()}
-    (R.model_forward(params, cfg, pos, batch, z, n_graphs=2) ** 2).sum().backward()
-    assert _worst_grad({k: v.grad for k, v in params.items()}, g, 80) < 1e-8
-    model = _mirror_model(g, GraphAttentionTransformer).double()
+    case = load(SMALL)
+    _energy, _forces, params = run_oracle("qm9", case, oracle_config("qm9", case.cfg))
+    assert worst_grad({k: v.grad for k, v in params.items()}, case.grads, 80) < 1e-8
+    model = mirror(GraphAttentionTransformer, case.cfg, case.state).double()
     with emulated_kernels():
-        (model(f_in=None, pos=pos, batch=batch, node_atom=z) ** 2).sum().backward()
-    assert _worst_grad({k: p.grad for k, p in model.named_parameters()}, g, 80) < 1e-7
+        run_mirror("qm9", model, case)
+    assert worst_grad({k: p.grad for k, p in model.named_parameters()}, case.grads, 80) < 1e-7
 
 
 def test_parameter_gradients_match_reference_md17_small():
@@ -530,56 +462,30 @@ def test_parameter_gradients_match_reference_md17_small():
     reference's model file vs the oracle and the mirror."""
     from equiformer_b200.nets.graph_attention_transformer_md17 import GraphAttentionTransformerMD17
     from tests._emulation import emulated_kernels
-    g = np.load(os.path.join(os.path.dirname(SMALL), "reference_model_md17_small.npz"))
-    state = {k[len("state/"):]: torch.from_numpy(g[k]) for k in g.files if k.startswith("state/")}
-    cfg = R.Config(irreps_node_embedding=str(g["cfg/irreps_node_embedding"]), irreps_sh=str(g["cfg/irreps_sh"]),
-                   irreps_head=str(g["cfg/irreps_head"]), irreps_mlp_mid=str(g["cfg/irreps_mlp_mid"]),
-                   irreps_feature=str(g["cfg/irreps_feature"]), num_heads=int(g["cfg/num_heads"]),
-                   num_layers=int(g["cfg/num_layers"]), max_radius=float(g["cfg/max_radius"]),
-                   number_of_basis=int(g["cfg/number_of_basis"]), basis_type="exp",
-                   nonlinear_message=bool(g["cfg/nonlinear_message"]), max_atom_type=64, qm9_atom_remap=False)
-    pos, batch, z = torch.from_numpy(g["pos"]).double(), torch.from_numpy(g["batch"]), torch.from_numpy(g["z"])
-    params = {k: v.requires_grad_(v.is_floating_point()) for k, v in R.cast_params(state, torch.float64).items()}
-    e, f = R.energy_and_forces(params, cfg, pos, batch, z, 1, create_graph=True)
-    (e.sum() + (f ** 2).sum()).backward()
-    assert _worst_grad({k: v.grad for k, v in params.items()}, g, 80) < 1e-8
-    model = _mirror_model(g, GraphAttentionTransformerMD17).double().train()
+    case = load(MD17_SMALL)
+    _energy, _forces, params = run_oracle("md17", case, oracle_config("md17", case.cfg))
+    assert worst_grad({k: v.grad for k, v in params.items()}, case.grads, 80) < 1e-8
+    model = mirror(GraphAttentionTransformerMD17, case.cfg, case.state).double().train()
     for m in model.modules():
         if isinstance(m, torch.nn.Dropout):
             m.p = 0.0
     with emulated_kernels():
-        e, f = model(node_atom=z, pos=pos.clone(), batch=batch)
-        (e.sum() + (f ** 2).sum()).backward()
-    assert _worst_grad({k: p.grad for k, p in model.named_parameters()}, g, 80) < 1e-6
+        run_mirror("md17", model, case)
+    assert worst_grad({k: p.grad for k, p in model.named_parameters()}, case.grads, 80) < 1e-6
 
 
 # ------------------------------------------------------------------ dot-product attention variant (SURVEY.md 8f-4)
 
-DP_SMALL = os.path.join(os.path.dirname(SMALL), "reference_model_dp_small.npz")
-
-
-def _dp_case():
-    g = np.load(DP_SMALL)
-    state = {k[len("state/"):]: torch.from_numpy(g[k]) for k in g.files if k.startswith("state/")}
-    cfg = R.Config(irreps_node_embedding=str(g["cfg/irreps_node_embedding"]), irreps_sh=str(g["cfg/irreps_sh"]),
-                   irreps_head=str(g["cfg/irreps_head"]), irreps_mlp_mid=str(g["cfg/irreps_mlp_mid"]),
-                   irreps_feature=str(g["cfg/irreps_feature"]), num_heads=int(g["cfg/num_heads"]),
-                   num_layers=int(g["cfg/num_layers"]), max_radius=float(g["cfg/max_radius"]),
-                   number_of_basis=int(g["cfg/number_of_basis"]), basis_type="gaussian", nonlinear_message=False,
-                   attention="dot_product")
-    pos, batch, z = torch.from_numpy(g["pos"]).double(), torch.from_numpy(g["batch"]), torch.from_numpy(g["z"])
-    return g, state, cfg, pos, batch, z
+DP_SMALL = "reference_model_dp_small.npz"
 
 
 def test_oracle_dot_product_attention_model_matches_reference_model_file():
     """``nets/dp_attention_transformer.py`` (DotProductAttention / DPTransBlock / DotProductAttentionTransformer) run by
     the reference's code vs the oracle's restatement: energies and parameter gradients of sum E^2."""
-    g, state, cfg, pos, batch, z = _dp_case()
-    params = {k: v.requires_grad_(v.is_floating_point()) for k, v in R.cast_params(state, torch.float64).items()}
-    energy = R.model_forward(params, cfg, pos, batch, z, n_graphs=2)
-    assert rel_err(energy.detach(), torch.from_numpy(g["energy"])) < 1e-11
-    (energy ** 2).sum().backward()
-    assert _worst_grad({k: v.grad for k, v in params.items()}, g, 70) < 1e-8
+    case = load(DP_SMALL)
+    energy, _forces, params = run_oracle("qm9", case, oracle_config("qm9", case.cfg, attention="dot_product"))
+    assert rel_err(energy.detach(), case.t("energy")) < 1e-11
+    assert worst_grad({k: v.grad for k, v in params.items()}, case.grads, 70) < 1e-8
 
 
 def test_mirror_dot_product_attention_matches_reference_model_file():
@@ -587,13 +493,12 @@ def test_mirror_dot_product_attention_matches_reference_model_file():
     loaded with the reference's ``state_dict``: energies and parameter gradients against the reference-run fixture."""
     from equiformer_b200.nets.dp_attention_transformer import DotProductAttentionTransformer
     from tests._emulation import emulated_kernels
-    g, _state, _cfg, pos, batch, z = _dp_case()
-    model = _mirror_model(g, DotProductAttentionTransformer).double()
+    case = load(DP_SMALL)
+    model = mirror(DotProductAttentionTransformer, case.cfg, case.state).double()
     with emulated_kernels():
-        energy = model(f_in=None, pos=pos, batch=batch, node_atom=z)
-        (energy ** 2).sum().backward()
-    assert rel_err(energy.detach(), torch.from_numpy(g["energy"])) < 1e-10
-    assert _worst_grad({k: p.grad for k, p in model.named_parameters()}, g, 70) < 1e-7
+        energy, _forces = run_mirror("qm9", model, case)
+    assert rel_err(energy.detach(), case.t("energy")) < 1e-10
+    assert worst_grad({k: p.grad for k, p in model.named_parameters()}, case.grads, 70) < 1e-7
 
 
 @pytest.mark.gpu
@@ -601,11 +506,12 @@ def test_cuda_dot_product_attention_matches_reference_model_file(cuda_device):
     """The dot-product variant on the CUDA kernels (float32) against the reference-run energies.  Written after the
     round-1 GPU budget ended."""
     from equiformer_b200.nets.dp_attention_transformer import DotProductAttentionTransformer
-    g, _state, _cfg, pos, batch, z = _dp_case()
-    model = _mirror_model(g, DotProductAttentionTransformer).to(cuda_device)
+    case = load(DP_SMALL)
+    model = mirror(DotProductAttentionTransformer, case.cfg, case.state).to(cuda_device)
     with torch.no_grad():
-        energy = model(f_in=None, pos=pos.float().to(cuda_device), batch=batch.to(cuda_device), node_atom=z.to(cuda_device))
-    assert rel_err(energy, torch.from_numpy(g["energy"])) < 5e-5
+        energy = model(f_in=None, pos=case.t("pos", cuda_device, torch.float32), batch=case.t("batch", cuda_device),
+                       node_atom=case.t("z", cuda_device))
+    assert rel_err(energy, case.t("energy")) < 5e-5
 
 
 def test_dot_product_md17_variant_matches_reference_model_file():
@@ -613,83 +519,43 @@ def test_dot_product_md17_variant_matches_reference_model_file():
     code: the oracle and the mirror (emulated kernels) against energy, forces and the gradients of the energy + force loss."""
     from equiformer_b200.nets.dp_attention_transformer import DotProductAttentionTransformerMD17
     from tests._emulation import emulated_kernels
-    g = np.load(os.path.join(os.path.dirname(SMALL), "reference_model_dp_md17_small.npz"))
-    state = {k[len("state/"):]: torch.from_numpy(g[k]) for k in g.files if k.startswith("state/")}
-    cfg = R.Config(irreps_node_embedding=str(g["cfg/irreps_node_embedding"]), irreps_sh=str(g["cfg/irreps_sh"]),
-                   irreps_head=str(g["cfg/irreps_head"]), irreps_mlp_mid=str(g["cfg/irreps_mlp_mid"]),
-                   irreps_feature=str(g["cfg/irreps_feature"]), num_heads=int(g["cfg/num_heads"]),
-                   num_layers=int(g["cfg/num_layers"]), max_radius=float(g["cfg/max_radius"]),
-                   number_of_basis=int(g["cfg/number_of_basis"]), basis_type="exp", nonlinear_message=False,
-                   max_atom_type=64, qm9_atom_remap=False, attention="dot_product")
-    pos, batch, z = torch.from_numpy(g["pos"]).double(), torch.from_numpy(g["batch"]), torch.from_numpy(g["z"])
-    params = {k: v.requires_grad_(v.is_floating_point()) for k, v in R.cast_params(state, torch.float64).items()}
-    e, f = R.energy_and_forces(params, cfg, pos, batch, z, 1, create_graph=True)
-    (e.sum() + (f ** 2).sum()).backward()
-    assert rel_err(e.detach(), torch.from_numpy(g["energy"])) < 1e-11
-    assert rel_err(f.detach(), torch.from_numpy(g["forces"])) < 1e-10
-    assert _worst_grad({k: v.grad for k, v in params.items()}, g, 70) < 1e-8
+    case = load("reference_model_dp_md17_small.npz")
+    e, f, params = run_oracle("md17", case, oracle_config("md17", case.cfg, attention="dot_product"))
+    assert rel_err(e.detach(), case.t("energy")) < 1e-11
+    assert rel_err(f.detach(), case.t("forces")) < 1e-10
+    assert worst_grad({k: v.grad for k, v in params.items()}, case.grads, 70) < 1e-8
 
-    model = _mirror_model(g, DotProductAttentionTransformerMD17).double().train()
+    model = mirror(DotProductAttentionTransformerMD17, case.cfg, case.state).double().train()
     with emulated_kernels():
-        e, f = model(node_atom=z, pos=pos.clone(), batch=batch)
-        (e.sum() + (f ** 2).sum()).backward()
-    assert rel_err(e.detach(), torch.from_numpy(g["energy"])) < 1e-10
-    assert rel_err(f.detach(), torch.from_numpy(g["forces"])) < 1e-9
-    assert _worst_grad({k: p.grad for k, p in model.named_parameters()}, g, 70) < 1e-6
+        e, f = run_mirror("md17", model, case)
+    assert rel_err(e.detach(), case.t("energy")) < 1e-10
+    assert rel_err(f.detach(), case.t("forces")) < 1e-9
+    assert worst_grad({k: p.grad for k, p in model.named_parameters()}, case.grads, 70) < 1e-6
 
 
 # --------------------------------------------------------------- the OC20 model file (periodic boundary conditions, tags)
-OC20_SMALL = os.path.join(os.path.dirname(SMALL), "reference_model_oc20_small.npz")
-OC20_STATS = dict(max_atom_type=84, qm9_atom_remap=False, avg_degree=23.395238876342773, avg_num_nodes=77.81317)
-
-
-def _oc20_fixture():
-    g = np.load(OC20_SMALL)
-    cfg = {k[4:]: g[k].tolist() for k in g.files if k.startswith("cfg/")}
-    state = {k[6:]: torch.from_numpy(g[k]) for k in g.files if k.startswith("state/")}
-    return g, cfg, state
+OC20_SMALL = "reference_model_oc20_small.npz"
 
 
 def test_oracle_oc20_model_matches_reference_model_file():
     """``nets/graph_attention_transformer_oc20.py`` run end to end (tests/golden/make_reference_golden_oc20.py: two
     triclinic periodic frames, tags, 84 atom types) vs ``oracle.model_forward_oc20``: energy and parameter gradients."""
-    g, cfg, state = _oc20_fixture()
-    ocfg = R.Config(irreps_node_embedding=cfg["irreps_node_embedding"], irreps_sh=cfg["irreps_sh"], irreps_head=cfg["irreps_head"],
-                    irreps_mlp_mid=cfg["irreps_mlp_mid"], irreps_feature=cfg["irreps_feature"], num_heads=cfg["num_heads"],
-                    num_layers=cfg["num_layers"], max_radius=cfg["max_radius"], number_of_basis=cfg["number_of_basis"],
-                    nonlinear_message=True, **OC20_STATS)
-    params = {k: v.requires_grad_(v.is_floating_point() and v.numel() > 0) for k, v in R.cast_params(state, torch.float64).items()}
-    t = lambda k: torch.from_numpy(g[k])
+    case = load(OC20_SMALL)
+    ocfg = oracle_config("oc20", case.cfg)
+    params = {k: v.requires_grad_(v.is_floating_point() and v.numel() > 0) for k, v in R.cast_params(case.state, torch.float64).items()}
+    t = case.t
     edge = t("edge_index")
     energy = R.model_forward_oc20(params, ocfg, t("pos").double(), t("cell").double(), t("batch"), t("z"), t("tags"), 2,
                                   edge[0], edge[1], t("cell_offsets"))
     assert rel_err(energy, t("energy")) < 1e-10
     (energy * torch.tensor([[1.0], [-0.7]])).sum().backward()
-    for k in g.files:
-        if k.startswith("grad/"):
-            assert rel_err(params[k[5:]].grad, t(k)) < 1e-6, k
+    for k, ref in case.grads.items():
+        assert rel_err(params[k].grad, ref) < 1e-6, k
 
 
-def _oc20_mirror(cfg, state):
+def _oc20_mirror(case):
     from equiformer_b200.nets.graph_attention_transformer_oc20 import GraphAttentionTransformerOC20
-    cfg = dict(cfg)
-    cfg["fc_neurons"] = list(cfg["fc_neurons"])
-    model = GraphAttentionTransformerOC20(None, None, 1, **cfg)
-    res = model.load_state_dict(state, strict=False)
-    assert not res.unexpected_keys and all(k.endswith("tp.output_mask") for k in res.missing_keys), res
-    return model.eval()
-
-
-def _oc20_data(g, dev=None, dtype=torch.float64):
-    import types
-    t = lambda k: torch.from_numpy(g[k])
-    d = types.SimpleNamespace(pos=t("pos").to(dtype), cell=t("cell").to(dtype), batch=t("batch"), atomic_numbers=t("z"),
-                              tags=t("tags"), n_graphs=2)
-    if dev is not None:
-        for k, v in vars(d).items():
-            if isinstance(v, torch.Tensor):
-                setattr(d, k, v.to(dev))
-    return d
+    return mirror(GraphAttentionTransformerOC20, case.cfg, case.state, None, None, 1)
 
 
 def test_mirror_oc20_model_matches_reference_model_file():
@@ -697,83 +563,62 @@ def test_mirror_oc20_model_matches_reference_model_file():
     ``state_dict``: same edge list as the fixture's, energy 1e-10, parameter gradients 1e-6."""
     from equiformer_b200.graph import radius_graph_pbc
     from tests._emulation import emulated_kernels
-    g, cfg, state = _oc20_fixture()
-    model = _oc20_mirror(cfg, state).double()
-    data = _oc20_data(g)
+    case = load(OC20_SMALL)
+    cfg = case.cfg
+    model = _oc20_mirror(case).double()
+    data = oc20_data(case)
     edge, offs, _d2 = radius_graph_pbc(data.pos.float(), data.batch, data.cell.float(), cfg["max_radius"], cfg["max_neighbors"])
-    assert torch.equal(edge, torch.from_numpy(g["edge_index"])) and torch.equal(offs.long(), torch.from_numpy(g["cell_offsets"]).long())
+    assert torch.equal(edge, case.t("edge_index")) and torch.equal(offs.long(), case.t("cell_offsets").long())
     with emulated_kernels():
         energy = model(data)
         (energy * torch.tensor([[1.0], [-0.7]], dtype=torch.float64)).sum().backward()
-    assert rel_err(energy, torch.from_numpy(g["energy"])) < 1e-10
-    for k in g.files:
-        if k.startswith("grad/"):
-            assert rel_err(model.get_parameter(k[5:]).grad, torch.from_numpy(g[k])) < 1e-6, k
+    assert rel_err(energy, case.t("energy")) < 1e-10
+    for k, ref in case.grads.items():
+        assert rel_err(model.get_parameter(k).grad, ref) < 1e-6, k
 
 
 @pytest.mark.gpu
 def test_cuda_oc20_model_matches_reference_model_file(cuda_device):
     """The OC20 mirror on CUDA (periodic neighbour-list kernels + the edge kernels) against the reference's own output."""
     from equiformer_b200.graph import radius_graph_pbc
-    g, cfg, state = _oc20_fixture()
-    model = _oc20_mirror(cfg, state).to(cuda_device)
-    data = _oc20_data(g, cuda_device, torch.float32)
+    case = load(OC20_SMALL)
+    cfg = case.cfg
+    model = _oc20_mirror(case).to(cuda_device)
+    data = oc20_data(case, cuda_device, torch.float32)
     edge, offs, _d2 = radius_graph_pbc(data.pos, data.batch, data.cell, cfg["max_radius"], cfg["max_neighbors"])
-    assert torch.equal(edge.cpu(), torch.from_numpy(g["edge_index"]))
-    assert torch.equal(offs.cpu().long(), torch.from_numpy(g["cell_offsets"]).long())
+    assert torch.equal(edge.cpu(), case.t("edge_index"))
+    assert torch.equal(offs.cpu().long(), case.t("cell_offsets").long())
     energy = model(data)
     (energy * torch.tensor([[1.0], [-0.7]], device=cuda_device)).sum().backward()
-    assert rel_err(energy, torch.from_numpy(g["energy"])) < 1e-4
-    worst = max(rel_err(model.get_parameter(k[5:]).grad, torch.from_numpy(g[k])) for k in g.files if k.startswith("grad/"))
+    assert rel_err(energy, case.t("energy")) < 1e-4
+    worst = max(rel_err(model.get_parameter(k).grad, ref) for k, ref in case.grads.items())
     assert worst < 1e-3, worst
 
 
 # --------------------------------------------------------------- the DeNS variant (nets/equiformer_md17_dens.py)
-DENS_SMALL = os.path.join(os.path.dirname(SMALL), "reference_model_dens_small.npz")
-
-
-def _dens_setup(dev=None, dtype=torch.float64):
-    import types
-    from equiformer_b200.nets.equiformer_md17_dens import Equiformer_MD17_DeNS
-    g = np.load(DENS_SMALL)
-    cfg = {k[4:]: g[k].tolist() for k in g.files if k.startswith("cfg/")}
-    cfg["fc_neurons"] = list(cfg["fc_neurons"])
-    state = {k[6:]: torch.from_numpy(g[k]) for k in g.files if k.startswith("state/")}
-    model = Equiformer_MD17_DeNS(**cfg)
-    res = model.load_state_dict(state, strict=False)
-    assert not res.unexpected_keys and all(k.endswith("tp.output_mask") for k in res.missing_keys), res
-    model = model.eval().to(dtype)
-    t = lambda k: torch.from_numpy(g[k])
-    data = types.SimpleNamespace(z=t("z"), pos=t("pos").to(dtype), batch=t("batch"), force=t("force").to(dtype),
-                                 noise_mask=t("noise_mask"))
-    if dev is not None:
-        model = model.to(dev)
-        for k, v in vars(data).items():
-            setattr(data, k, v.to(dev))
-    return g, model, data
+DENS_SMALL = "reference_model_dens_small.npz"
 
 
 def test_mirror_dens_model_matches_reference_model_file():
     """``Equiformer_MD17_DeNS`` (force encoding + denoising head on) loaded with the reference's ``state_dict``, kernels
     emulated in float64: energies, the forces / predicted-noise output and the gradients of an energy + output loss."""
     from tests._emulation import emulated_kernels
-    g, model, data = _dens_setup()
+    case, model, data = dens_setup(DENS_SMALL)
     with emulated_kernels():
         energy, dy = model(data)
         (energy.sum() + (dy ** 2).sum()).backward()
-    assert rel_err(energy, torch.from_numpy(g["energy"])) < 1e-10
-    assert rel_err(dy, torch.from_numpy(g["dy"])) < 1e-9
-    for k in g.files:
-        if k.startswith("grad/"):
-            assert rel_err(model.get_parameter(k[5:]).grad, torch.from_numpy(g[k])) < 1e-6, k
+    assert rel_err(energy, case.t("energy")) < 1e-10
+    assert rel_err(dy, case.t("dy")) < 1e-9
+    for k, ref in case.grads.items():
+        assert rel_err(model.get_parameter(k).grad, ref) < 1e-6, k
 
 
 @pytest.mark.gpu
 def test_cuda_dens_model_matches_reference_model_file(cuda_device):
-    g, model, data = _dens_setup(cuda_device, torch.float32)
+    case, model, data = dens_setup(DENS_SMALL, cuda_device, torch.float32)
     energy, dy = model(data)
     (energy.sum() + (dy ** 2).sum()).backward()
-    assert rel_err(energy, torch.from_numpy(g["energy"])) < 1e-4
-    assert rel_err(dy, torch.from_numpy(g["dy"])) < 3e-4
-    worst = max(rel_err(model.get_parameter(k[5:]).grad, torch.from_numpy(g[k])) for k in g.files if k.startswith("grad/"))
+    assert rel_err(energy, case.t("energy")) < 1e-4
+    assert rel_err(dy, case.t("dy")) < 3e-4
+    worst = max(rel_err(model.get_parameter(k).grad, ref) for k, ref in case.grads.items())
     assert worst < 2e-3, worst
