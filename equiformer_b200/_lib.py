@@ -12,7 +12,7 @@ import os
 import shutil
 import subprocess
 import threading
-from ctypes import POINTER, c_char_p, c_float, c_int32, c_int64, c_void_p
+from ctypes import POINTER, c_char_p, c_double, c_float, c_int32, c_int64, c_void_p
 from pathlib import Path
 
 PKG_DIR = Path(__file__).resolve().parent
@@ -28,6 +28,12 @@ L4_SOURCES = ("eqf_abi.cu", "eqf_dtp.cu", "eqf_dtp_vec.cu")
 NORM_LIB_PATH = PKG_DIR / "libeqf_b200_norm.so"
 NORM_SOURCES = ("eqf_norm.cu",)
 EQF_NORM_MAX_ENTRIES = 8      # include/eqf_b200_norm.h: irreps entries per norm layout
+# gradient clipping, AdamW and the model EMA on the flat parameter buffers: their own library and header
+# (include/eqf_b200_optim.h), bound by load_optim()
+OPTIM_LIB_PATH = PKG_DIR / "libeqf_b200_optim.so"
+OPTIM_SOURCES = ("eqf_optim.cu",)
+EQF_OPTIM_THREADS = 256       # include/eqf_b200_optim.h: threads per CTA, 4 elements each per pass
+EQF_OPTIM_MAX_CTAS = 1024     # include/eqf_b200_optim.h: grid cap (and length of the partial-sum scratch)
 SOURCES = ("eqf_abi.cu", "eqf_dtp.cu", "eqf_dtp_vec.cu", "eqf_attn.cu", "eqf_pointwise.cu", "eqf_gemm_tf32x3.cu", "eqf_graph.cu",
            "eqf_fused.cu", "eqf_edge.cu", "eqf_gemm_small.cu")
 
@@ -218,6 +224,17 @@ NORM_SIGNATURES = {
     "eqf_norm_param_reduce": (c_int32, [c_void_p, c_int64, c_int32, c_void_p, c_void_p]),
 }
 
+# every symbol include/eqf_b200_optim.h declares
+OPTIM_SIGNATURES = {
+    "eqf_last_error": (c_char_p, []),
+    "eqf_flat_sqnorm": (c_int32, [c_void_p, c_int64, c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "eqf_flat_adamw": (c_int32, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p,
+                                 c_void_p, c_double, c_double, c_float, c_double, c_void_p, c_void_p]),
+    "eqf_flat_sqnorm_check": (c_int32, [c_void_p, c_int64, c_float, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "eqf_flat_adamw_check": (c_int32, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p,
+                                       c_void_p, c_void_p, c_double, c_double, c_void_p]),
+}
+
 
 class EqfError(RuntimeError):
     pass
@@ -239,19 +256,20 @@ def generate_sources():
 
 
 def needs_build() -> bool:
-    libs = (LIB_PATH, L4_LIB_PATH, NORM_LIB_PATH)
+    libs = (LIB_PATH, L4_LIB_PATH, NORM_LIB_PATH, OPTIM_LIB_PATH)
     if not all(p.exists() for p in libs):
         return True
     mtime = min(p.stat().st_mtime for p in libs)
-    deps = (sources() + [CSRC_DIR / s for s in NORM_SOURCES] + list(CSRC_DIR.glob("*.cuh"))
-            + [INCLUDE_DIR / "eqf_b200.h", INCLUDE_DIR / "eqf_b200_norm.h"])
+    deps = (sources() + [CSRC_DIR / s for s in NORM_SOURCES + OPTIM_SOURCES] + list(CSRC_DIR.glob("*.cuh"))
+            + [INCLUDE_DIR / "eqf_b200.h", INCLUDE_DIR / "eqf_b200_norm.h", INCLUDE_DIR / "eqf_b200_optim.h"])
     return any(p.stat().st_mtime > mtime for p in deps)
 
 
 def build(force: bool = False, verbose: bool = False) -> Path:
     """Compile ``csrc/*.cu`` for sm_90a into ``equiformer_b200/libeqf_b200.so``, ``L4_SOURCES`` with
-    ``-DEQF_MAX_DEGREE=4`` into ``equiformer_b200/libeqf_b200_l4.so`` and ``NORM_SOURCES`` into
-    ``equiformer_b200/libeqf_b200_norm.so`` (in-tree)."""
+    ``-DEQF_MAX_DEGREE=4`` into ``equiformer_b200/libeqf_b200_l4.so``, ``NORM_SOURCES`` into
+    ``equiformer_b200/libeqf_b200_norm.so`` and ``OPTIM_SOURCES`` into ``equiformer_b200/libeqf_b200_optim.so``
+    (in-tree)."""
     generate_sources()
     if not force and not needs_build():
         return LIB_PATH
@@ -265,7 +283,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
     obj_dir.mkdir(parents=True, exist_ok=True)
     compile_flags = [f for f in NVCC_FLAGS if f != "--shared"]
     jobs = ([(src, "", []) for src in sources()] + [(CSRC_DIR / s, "_l4", ["-DEQF_MAX_DEGREE=4"]) for s in L4_SOURCES]
-            + [(CSRC_DIR / s, "_norm", []) for s in NORM_SOURCES])
+            + [(CSRC_DIR / s, "_norm", []) for s in NORM_SOURCES] + [(CSRC_DIR / s, "_optim", []) for s in OPTIM_SOURCES])
 
     def compile_one(job):
         src, suffix, defines = job
@@ -294,6 +312,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
         link(LIB_PATH, [o for o, suffix, _ in results if suffix == ""])
         link(L4_LIB_PATH, [o for o, suffix, _ in results if suffix == "_l4"])
         link(NORM_LIB_PATH, [o for o, suffix, _ in results if suffix == "_norm"])
+        link(OPTIM_LIB_PATH, [o for o, suffix, _ in results if suffix == "_optim"])
     finally:
         shutil.rmtree(obj_dir, ignore_errors=True)
     return LIB_PATH
@@ -332,25 +351,34 @@ def load_l4():
     return _lib_l4
 
 
-_lib_norm = None
+_side_libs = {}
+
+
+def _load_side(path: Path, signatures: dict):
+    """Load a library of its own (every symbol of ``signatures`` required), once."""
+    with _lock:
+        if path not in _side_libs:
+            if not path.exists():
+                raise EqfError(f"{path} is missing: run `python -c 'import __graft_entry__ as g; g.build()'`")
+            lib = ctypes.CDLL(str(path))
+            for name, (restype, argtypes) in signatures.items():
+                try:
+                    fn = getattr(lib, name)
+                except AttributeError as exc:
+                    raise EqfError(f"{path.name} does not export {name}; rebuild it") from exc
+                fn.restype, fn.argtypes = restype, argtypes
+            _side_libs[path] = lib
+    return _side_libs[path]
 
 
 def load_norm():
     """Return the loaded norm library (``include/eqf_b200_norm.h``)."""
-    global _lib_norm
-    with _lock:
-        if _lib_norm is None:
-            if not NORM_LIB_PATH.exists():
-                raise EqfError(f"{NORM_LIB_PATH} is missing: run `python -c 'import __graft_entry__ as g; g.build()'`")
-            lib = ctypes.CDLL(str(NORM_LIB_PATH))
-            for name, (restype, argtypes) in NORM_SIGNATURES.items():
-                try:
-                    fn = getattr(lib, name)
-                except AttributeError as exc:
-                    raise EqfError(f"{NORM_LIB_PATH.name} does not export {name}; rebuild it") from exc
-                fn.restype, fn.argtypes = restype, argtypes
-            _lib_norm = lib
-    return _lib_norm
+    return _load_side(NORM_LIB_PATH, NORM_SIGNATURES)
+
+
+def load_optim():
+    """Return the loaded optimiser library (``include/eqf_b200_optim.h``)."""
+    return _load_side(OPTIM_LIB_PATH, OPTIM_SIGNATURES)
 
 
 def load():

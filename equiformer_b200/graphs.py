@@ -6,12 +6,16 @@ not the GPU, bounds the step.  Everything after neighbour search is free of host
 and replayed: inputs are copied into static buffers, ``graph.replay()`` runs forward, loss and backward, gradients
 land in the flat bucket of :class:`equiformer_b200.parallel.FlatGradAllReduce`.  A new signature triggers a new
 capture (cached), so variable-size batches still work - they just pay the capture when a size is first seen.
-Neighbour search, the gradient all-reduce and the optimiser stay outside the graph.
+Neighbour search and the gradient all-reduce stay outside the graph.  The optimiser does too, unless it is handed to a
+step as ``after_backward``: a callable without arguments (``parallel.CapturableFlatAdamW.step``) that runs inside the
+captured region after the backward, once per replay, and never in the warm-up passes before a capture.  On one process
+that puts clipping, AdamW and the EMA into the graph; across processes the all-reduce must come first, so there the
+optimiser steps eagerly after ``bucket.reduce()``.
 """
 from __future__ import annotations
 
 import gc
-from typing import Callable, Dict, Tuple
+from typing import Callable, Dict, Optional, Tuple
 
 import torch
 
@@ -48,6 +52,14 @@ def pad_to_bucket(pos, batch, z, src, dst, n_graphs: int, atom_quantum: int, edg
     return (pos_p, batch_p, z_p, src_p, dst_p, row_ptr), (Nb, Eb)
 
 
+def _single_process_hook(bucket, after_backward):
+    """An ``after_backward`` optimiser would step on this rank's gradient before the all-reduce: refuse it across ranks."""
+    if after_backward is not None and getattr(bucket, "world", 1) > 1:
+        raise ValueError("after_backward steps before bucket.reduce(): across processes call bucket.reduce() and then "
+                         "the optimiser's step() eagerly")
+    return after_backward
+
+
 def csr_graph(src, dst, row_ptr, n_nodes: int) -> ops.Graph:
     """An ``ops.Graph`` over a destination-sorted edge list and its CSR offsets, built without host synchronisation."""
     csr = ops.Graph.__new__(ops.Graph)
@@ -63,9 +75,11 @@ class _Captured:
 
 class GraphedForwardBackward:
     def __init__(self, model: torch.nn.Module, loss_fn: Callable[[torch.Tensor, torch.Tensor], torch.Tensor],
-                 bucket, max_radius: float, warmup: int = 3, max_cached: int = 8):
+                 bucket, max_radius: float, warmup: int = 3, max_cached: int = 8,
+                 after_backward: Optional[Callable[[], None]] = None):
         self.model, self.loss_fn, self.bucket = model, loss_fn, bucket
         self.max_radius, self.warmup, self.max_cached = max_radius, warmup, max_cached
+        self.after_backward = _single_process_hook(bucket, after_backward)
         self._cache: Dict[Tuple[int, int, int], _Captured] = {}
         self.captures = 0
 
@@ -98,6 +112,8 @@ class GraphedForwardBackward:
         c.graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(c.graph):
             c.loss = self._fwd_bwd(c)
+            if self.after_backward is not None:
+                self.after_backward()
         self.captures += 1
         return c
 
@@ -124,8 +140,10 @@ class GraphedStep:
     together with its backward (gradients stored into the flat bucket) and replayed on refreshed static buffers.  Used by
     ``bench.py`` for the OC20 and periodic-cell workloads, whose neighbour search stays eager."""
 
-    def __init__(self, fn: Callable[..., torch.Tensor], bucket, warmup: int = 3, max_cached: int = 8):
+    def __init__(self, fn: Callable[..., torch.Tensor], bucket, warmup: int = 3, max_cached: int = 8,
+                 after_backward: Optional[Callable[[], None]] = None):
         self.fn, self.bucket, self.warmup, self.max_cached = fn, bucket, warmup, max_cached
+        self.after_backward = _single_process_hook(bucket, after_backward)
         self._cache: Dict[tuple, tuple] = {}
         self.captures = 0
 
@@ -152,6 +170,8 @@ class GraphedStep:
             graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(graph):
                 loss = self._fwd_bwd(static)
+                if self.after_backward is not None:
+                    self.after_backward()
             self.captures += 1
             hit = (graph, static, loss)
             self._cache[key] = hit
@@ -176,13 +196,15 @@ class BucketedForwardBackward:
     connect dummy atoms only (destination-sorted, after every real edge), and its energy - output row ``n_graphs`` - never
     enters the loss.  Real atoms share no edge with it and every per-node / per-graph op of the model is local, so outputs
     and parameter gradients of the real molecules are unchanged (the dummy's cotangent is exactly zero); the price is
-    <= one quantum of extra atoms and edges per step.  One capture per ``(atoms_b, edges_b, graphs)`` bucket.
+    <= one quantum of extra atoms and edges per step.  One capture per ``(atoms_b, edges_b, graphs)`` bucket.  With
+    ``capture=False`` the step runs eagerly, and ``after_backward`` right after its backward.
     """
 
     def __init__(self, model: torch.nn.Module, loss_fn: Callable[[torch.Tensor, torch.Tensor], torch.Tensor], bucket,
                  max_radius: float, atom_quantum: int = 128, edge_quantum: int = 2048, warmup: int = 2, max_cached: int = 16,
-                 capture: bool = True):
+                 capture: bool = True, after_backward: Optional[Callable[[], None]] = None):
         self.model, self.loss_fn, self.bucket = model, loss_fn, bucket
+        self.after_backward = _single_process_hook(bucket, after_backward)
         self.max_radius, self.warmup, self.max_cached = max_radius, warmup, max_cached
         self.aq, self.eq, self.capture = int(atom_quantum), int(edge_quantum), capture
         self._cache: Dict[Tuple[int, int, int], _Captured] = {}
@@ -225,6 +247,8 @@ class BucketedForwardBackward:
             c.graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(c.graph):
                 c.loss = self._fwd_bwd(c)
+                if self.after_backward is not None:
+                    self.after_backward()
             self.captures += 1
         return c
 
@@ -244,7 +268,10 @@ class BucketedForwardBackward:
         if c.graph is not None:
             c.graph.replay()
             return c.loss
-        return self._fwd_bwd(c)
+        loss = self._fwd_bwd(c)
+        if self.after_backward is not None:
+            self.after_backward()
+        return loss
 
 
 class DensTrainStep:
@@ -257,15 +284,17 @@ class DensTrainStep:
     encoding; the dummy molecule's energy row stays out of the loss) and the forward + loss + backward is captured once per
     ``(atoms_b, edges_b, graphs)`` bucket through :class:`GraphedStep`, then replayed.  With ``capture=False`` the same step
     runs eagerly on the unpadded batch.  Noise, neighbour list and padding are eager in both cases.  Gradients land in
-    ``bucket`` (a ``FlatGradAllReduce`` over the model's parameters); the call returns the loss."""
+    ``bucket`` (a ``FlatGradAllReduce`` over the model's parameters); ``after_backward`` runs after the backward, captured
+    with it when the step is captured.  The call returns the loss."""
 
     def __init__(self, model: torch.nn.Module, bucket, task_mean=0.0, task_std=1.0, std: float = 0.05, prob: float = 0.25,
                  corrupt_ratio=0.25, w_e: float = 1.0, w_f: float = 80.0, atom_quantum: int = 32, edge_quantum: int = 512,
-                 capture: bool = True, warmup: int = 2, max_cached: int = 16):
-        self.model, self.bucket = model, bucket
+                 capture: bool = True, warmup: int = 2, max_cached: int = 16,
+                 after_backward: Optional[Callable[[], None]] = None):
+        self.model, self.bucket, self.after_backward = model, bucket, _single_process_hook(bucket, after_backward)
         self.task_mean, self.task_std, self.std, self.prob, self.corrupt_ratio = task_mean, task_std, std, prob, corrupt_ratio
         self.w_e, self.w_f, self.aq, self.eq = w_e, w_f, int(atom_quantum), int(edge_quantum)
-        self.graphed = GraphedStep(self._captured, bucket, warmup, max_cached) if capture else None
+        self.graphed = GraphedStep(self._captured, bucket, warmup, max_cached, after_backward) if capture else None
         self.last_edges = None
 
     @property
@@ -300,6 +329,8 @@ class DensTrainStep:
             loss = self._loss(pos_n, force, y, dy, noise_vec, None, w, noise_mask, batch, z,
                               csr_graph(src, dst, row_ptr, pos.shape[0]), n_graphs)
             loss.backward()
+            if self.after_backward is not None:
+                self.after_backward()
             return loss.detach()
         (pos_p, batch_p, z_p, src_p, dst_p, row_ptr_p), (Nb, Eb) = pad_to_bucket(pos_n, batch, z, src, dst, n_graphs,
                                                                                   self.aq, self.eq)
