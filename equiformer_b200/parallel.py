@@ -122,7 +122,117 @@ def flatten_parameters(named_params, bucket: FlatGradAllReduce, weight_decay: fl
     return [n for n, _ in named], flat, decay
 
 
-class FlatAdamW:
+def _adamw_format():
+    """The group keys (with their defaults, in the order of groups given as ``add_weight_decay`` gives them) and the
+    ``step`` dtype of this torch's ``AdamW.state_dict()``, read from a one-element ``AdamW`` that took one step."""
+    p = torch.nn.Parameter(torch.zeros(1))
+    opt = torch.optim.AdamW([{"params": [p], "weight_decay": 0.0}])
+    p.grad = torch.zeros(1)
+    opt.step()
+    sd = opt.state_dict()
+    return {k: v for k, v in sd["param_groups"][0].items() if k != "params"}, sd["state"][0]["step"].dtype
+
+
+class _AdamWStateDict:
+    """``state_dict`` / ``load_state_dict`` of the flat optimisers in ``torch.optim.AdamW``'s format, with the groups of
+    the reference's ``add_weight_decay`` (``optim_factory.py:27-42``): group 0 the parameters exempt by
+    :func:`is_no_decay` (weight decay 0), group 1 the decayed ones, both in ``named_parameters()`` order, and parameter
+    indices running through group 0 and then group 1.  A torch optimiser built on those groups loads our dict, and we
+    load theirs.  Loading writes into the existing ``m``, ``v`` and ``decay`` (the storage that captured steps read)."""
+
+    def _groups(self):
+        return ([i for i, e in enumerate(self._exempt) if e], [i for i, e in enumerate(self._exempt) if not e])
+
+    def _view(self, buf, i):
+        off, p = self.bucket.offsets[i], self.bucket.params[i]
+        return buf[off:off + p.numel()].view_as(p)
+
+    def state_dict(self) -> dict:
+        """The optimiser state as ``torch.optim.AdamW.state_dict()`` lays it out.  The moments are views of one copy of
+        ``m`` and of ``v`` taken now, so the dict shares no storage with the live state; a step count of 0 gives an empty
+        ``state``, as for a torch optimiser that never stepped."""
+        lr, t = self._lr_and_step()
+        keys, step_dtype = _adamw_format()
+        m, v = (self.m.clone(), self.v.clone()) if t > 0 else (None, None)
+        groups, state, k = [], {}, 0
+        for wd, members in zip(self._group_wd, self._groups()):
+            groups.append(dict(keys, lr=lr, betas=tuple(self.betas), eps=self.eps, weight_decay=wd,
+                               params=list(range(k, k + len(members)))))
+            for i in members:
+                if t > 0:
+                    state[k] = {"step": torch.tensor(float(t), dtype=step_dtype), "exp_avg": self._view(m, i),
+                                "exp_avg_sq": self._view(v, i)}
+                k += 1
+        return {"state": state, "param_groups": groups}
+
+    def load_state_dict(self, state_dict: dict) -> None:
+        """Load a ``torch.optim.AdamW`` state (ours or torch's) in place and adopt its ``lr``, ``betas``, ``eps`` and
+        per-group ``weight_decay``.  Everything is checked before anything is written; a ``ValueError`` names the
+        parameter or key that does not fit: parameter count or shape, decay group, differing per-parameter ``step``
+        (there is one step count), ``amsgrad``, ``maximize``, and groups that differ in ``lr``, ``betas`` or ``eps``.
+        An empty ``state`` means zero moments and step 0."""
+        groups, state = state_dict["param_groups"], state_dict["state"]
+        if len(groups) != 2:
+            raise ValueError(f"param_groups: {len(groups)} groups, expected 2 (no weight decay, weight decay)")
+        for key, bad in (("amsgrad", True), ("maximize", True), ("decoupled_weight_decay", False)):
+            if any(g.get(key, not bad) == bad for g in groups):
+                raise ValueError(f"param_groups: {key}={bad} is not supported by the flat AdamW")
+        hyper = [(float(g["lr"]), tuple(float(b) for b in g["betas"]), float(g["eps"])) for g in groups]
+        for j, key in enumerate(("lr", "betas", "eps")):
+            if hyper[0][j] != hyper[1][j]:
+                raise ValueError(f"param_groups: the groups differ in {key} ({hyper[0][j]} / {hyper[1][j]}); the flat "
+                                 f"AdamW has one {key}")
+        ours = self._groups()
+        order = ours[0] + ours[1]
+        saved = [list(g["params"]) for g in groups]
+        ids = saved[0] + saved[1]
+        if len(ids) != len(order):
+            raise ValueError(f"param_groups: {len(ids)} parameters, the optimiser has {len(order)}")
+        for pos, i in enumerate(order):
+            theirs, here = int(pos >= len(saved[0])), int(pos >= len(ours[0]))
+            if theirs != here:
+                raise ValueError(f"param_groups: index {ids[pos]} is in group {theirs}, but parameter {self._names[i]} "
+                                 f"at that place is in group {here} here (is_no_decay)")
+        unknown = set(state) - set(ids)
+        if unknown:
+            raise ValueError(f"state: indices {sorted(unknown)} belong to no parameter group")
+        pairs = list(zip(ids, order)) if state else []
+        t, first = 0, None
+        for sid, i in pairs:
+            name, p = self._names[i], self.bucket.params[i]
+            s = state.get(sid)
+            if s is None:
+                raise ValueError(f"state: parameter {name} (index {sid}) has no state")
+            for key in ("step", "exp_avg", "exp_avg_sq"):
+                if key not in s:
+                    raise ValueError(f"state[{sid}]: no {key} for parameter {name}")
+                if key != "step" and tuple(s[key].shape) != tuple(p.shape):
+                    raise ValueError(f"state[{sid}]: {key} of shape {tuple(s[key].shape)} for parameter {name} of "
+                                     f"shape {tuple(p.shape)}")
+            step = float(s["step"])
+            if first is None:
+                first, t = (name, step), int(step)
+                if step != t or t < 0:
+                    raise ValueError(f"state[{sid}]: step {step} of parameter {name} is not a step count")
+            elif step != first[1]:
+                raise ValueError(f"state[{sid}]: step {step} of parameter {name} differs from step {first[1]} of "
+                                 f"parameter {first[0]}; the flat AdamW keeps one step count")
+        lr, betas, eps = hyper[0]
+        wd = tuple(float(g["weight_decay"]) for g in groups)
+        self._set_hyper(lr, betas, eps, t)
+        with torch.no_grad():
+            self._group_wd = wd
+            for w, members in zip(wd, ours):
+                for i in members:
+                    self._view(self.decay, i).fill_(w)
+            self.m.zero_()
+            self.v.zero_()
+            for sid, i in pairs:
+                self._view(self.m, i).copy_(state[sid]["exp_avg"])
+                self._view(self.v, i).copy_(state[sid]["exp_avg_sq"])
+
+
+class FlatAdamW(_AdamWStateDict):
     """AdamW over ONE flat parameter buffer (decoupled weight decay, bias correction as torch.optim.AdamW).
 
     The model has ~290 small parameter tensors; a multi-tensor optimiser step costs more GPU time in launch slots
@@ -137,10 +247,18 @@ class FlatAdamW:
     def __init__(self, named_params, bucket: FlatGradAllReduce, lr=5e-4, betas=(0.9, 0.999), eps=1e-8,
                  weight_decay=5e-3, no_decay=()):
         self.bucket, self.lr, self.betas, self.eps = bucket, lr, betas, eps
-        _, self.flat, self.decay = flatten_parameters(named_params, bucket, weight_decay, no_decay)
+        self._names, self.flat, self.decay = flatten_parameters(named_params, bucket, weight_decay, no_decay)
+        self._exempt = [is_no_decay(n, no_decay) for n in self._names]
+        self._group_wd = (0.0, float(weight_decay))
         self.m = torch.zeros_like(self.flat)
         self.v = torch.zeros_like(self.flat)
         self.t = 0
+
+    def _lr_and_step(self):
+        return float(self.lr), int(self.t)
+
+    def _set_hyper(self, lr, betas, eps, t):
+        self.lr, self.betas, self.eps, self.t = lr, betas, eps, t
 
     @torch.no_grad()
     def step(self) -> None:
@@ -154,7 +272,7 @@ class FlatAdamW:
         self.flat.addcdiv_(self.m, denom, value=-self.lr / (1 - b1 ** self.t))
 
 
-class CapturableFlatAdamW:
+class CapturableFlatAdamW(_AdamWStateDict):
     """:class:`FlatAdamW` with gradient-norm clipping and a model EMA, on the fused kernels of ``libeqf_b200_optim.so``.
 
     The learning rate ``lr`` and the step count ``t`` are device tensors, and :meth:`step` reads nothing from the host,
@@ -183,6 +301,8 @@ class CapturableFlatAdamW:
         self.bucket, self.betas, self.eps = bucket, betas, eps
         self.max_grad_norm, self.ema_decay = max_grad_norm, ema_decay
         self._names, self.flat, self.decay = flatten_parameters(named_params, bucket, weight_decay, no_decay)
+        self._exempt = [is_no_decay(n, no_decay) for n in self._names]
+        self._group_wd = (0.0, float(weight_decay))
         dev = self.flat.device
         self.m = torch.zeros_like(self.flat)
         self.v = torch.zeros_like(self.flat)
@@ -212,6 +332,19 @@ class CapturableFlatAdamW:
         """Write the learning rate of the following steps (a device write: no capture is invalidated)."""
         self.lr.fill_(float(value))
 
+    def _lr_and_step(self):
+        return float(self.lr), int(self.t)
+
+    def _set_hyper(self, lr, betas, eps, t):
+        # betas and eps are arguments of the AdamW kernel launch, so a captured step holds the values it was captured
+        # with: adopting other ones would leave the live captures silently stepping with the old ones
+        if tuple(betas) != tuple(float(b) for b in self.betas) or eps != float(self.eps):
+            raise ValueError(f"param_groups: betas {betas} / eps {eps} differ from this optimiser's {tuple(self.betas)} / "
+                             f"{self.eps}; captured steps keep the values they were captured with, so construct "
+                             "CapturableFlatAdamW with the state's betas and eps")
+        self.lr.fill_(lr)
+        self.t.fill_(t)
+
     @torch.no_grad()
     def step(self) -> None:
         from . import optim_kernels
@@ -240,6 +373,20 @@ class CapturableFlatAdamW:
         out.update({k: e for (k, _), e in zip(self._others, self._ema_others)})
         keys = list(self.model.state_dict(keep_vars=True).keys())
         return {k: out[k] for k in keys}
+
+    def load_ema_state_dict(self, state: dict) -> None:
+        """The inverse of :meth:`ema_state_dict`: write a model-keyed EMA (timm's ``ModelEmaV2.module.state_dict()``,
+        a checkpoint's ``state_dict_ema``) into the EMA buffers in place.  Keys are checked as a model load checks them
+        (:func:`equiformer_b200.checkpoint.match_state_dict`)."""
+        from .checkpoint import match_state_dict
+        if self.ema is None:
+            raise RuntimeError("no EMA: construct the optimiser with ema_decay")
+        state = match_state_dict(state, self.model.state_dict(keep_vars=True))
+        with torch.no_grad():
+            for i, name in enumerate(self._names):
+                self._view(self.ema, i).copy_(state[name])
+            for (k, _), e in zip(self._others, self._ema_others):
+                e.copy_(state[k])
 
     @contextlib.contextmanager
     def ema_weights(self):
