@@ -34,6 +34,8 @@ OPTIM_LIB_PATH = PKG_DIR / "libeqf_b200_optim.so"
 OPTIM_SOURCES = ("eqf_optim.cu",)
 EQF_OPTIM_THREADS = 256       # include/eqf_b200_optim.h: threads per CTA, 4 elements each per pass
 EQF_OPTIM_MAX_CTAS = 1024     # include/eqf_b200_optim.h: grid cap (and length of the partial-sum scratch)
+EQF_LR_MAX_MILESTONES = 8     # include/eqf_b200_optim.h: milestones of a multistep schedule
+EQF_LR_KINDS = {"oc20_cosine": 1, "oc20_multistep": 2, "timm_cosine": 3}   # EQF_LR_* of include/eqf_b200_optim.h
 SOURCES = ("eqf_abi.cu", "eqf_dtp.cu", "eqf_dtp_vec.cu", "eqf_attn.cu", "eqf_pointwise.cu", "eqf_gemm_tf32x3.cu", "eqf_graph.cu",
            "eqf_fused.cu", "eqf_edge.cu", "eqf_gemm_small.cu")
 
@@ -108,6 +110,14 @@ class EqfHeadLayout(ctypes.Structure):
         ("d", c_int32 * EQF_MAX_BLOCKS),
         ("C", c_int32 * EQF_MAX_BLOCKS),
         ("n_heads", c_int32),
+    ]
+
+
+class EqfLrSchedule(ctypes.Structure):
+    _fields_ = [
+        ("kind", c_int32), ("n_milestones", c_int32), ("steps_per_unit", c_int64),
+        ("base_lr", c_double), ("warmup", c_double), ("warmup_start", c_double), ("total", c_double),
+        ("min_value", c_double), ("gamma", c_double), ("milestones", c_double * EQF_LR_MAX_MILESTONES),
     ]
 
 
@@ -233,6 +243,11 @@ OPTIM_SIGNATURES = {
     "eqf_flat_sqnorm_check": (c_int32, [c_void_p, c_int64, c_float, c_void_p, c_void_p, c_void_p, c_void_p]),
     "eqf_flat_adamw_check": (c_int32, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p,
                                        c_void_p, c_void_p, c_double, c_double, c_void_p]),
+    "eqf_lr_schedule_check": (c_int32, [POINTER(EqfLrSchedule)]),
+    "eqf_lr_at": (c_int32, [POINTER(EqfLrSchedule), c_int64, POINTER(c_double)]),
+    "eqf_flat_adamw_scheduled": (c_int32, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p,
+                                           c_void_p, c_void_p, c_double, c_double, c_float, c_double, c_void_p,
+                                           POINTER(EqfLrSchedule), c_void_p]),
 }
 
 

@@ -5,8 +5,14 @@
 // whatever the learning rate, the clip coefficient and the step count hold at replay time.  The CTA that finishes last
 // (a completion ticket, the only atomic) finishes the call: eqf_flat_sqnorm sums the per-CTA partials in CTA order,
 // eqf_flat_adamw writes the incremented step count once every CTA has read the old one.
+//
+// A scheduled step (eqf_flat_adamw_scheduled) runs the same kernel instances: the schedule descriptor travels in the
+// kernel arguments, thread 0 of each CTA evaluates lr_at() from the step count instead of reading *lr, and the last CTA
+// also writes the next step's rate.  lr_at() is __host__ __device__, so eqf_lr_at() hands the host the very function the
+// kernel runs.
 #include <cuda_runtime.h>
 
+#include <cmath>
 #include <cstdint>
 #include <string>
 
@@ -102,12 +108,62 @@ struct AdamArgs {
   float* ema;
   int64_t n;
   const float* coef;
-  const float* lr;
+  float* lr;               // read by an unscheduled step, written by a scheduled one
   int64_t* step;
   double b1, b2;
   float eps, ema_w;
   int32_t* tickets;
+  EqfLrSchedule sched;     // kind EQF_LR_NONE: the rate is *lr
 };
+
+// Products and sums rounded one by one: no fused multiply-add, so the device evaluates each schedule expression in the
+// reference's operation order, as Python (and the host compiler, which contracts nothing on x86-64) does.
+__host__ __device__ __forceinline__ double mul_rn(double a, double b) {
+#ifdef __CUDA_ARCH__
+  return __dmul_rn(a, b);
+#else
+  return a * b;
+#endif
+}
+
+__host__ __device__ __forceinline__ double add_rn(double a, double b) {
+#ifdef __CUDA_ARCH__
+  return __dadd_rn(a, b);
+#else
+  return a + b;
+#endif
+}
+
+// The rate of the step whose count before the step is t: include/eqf_b200_optim.h states each kind's expression, and
+// the comments name the reference expression each line copies.
+__host__ __device__ inline double lr_at(const EqfLrSchedule& s, int64_t t) {
+  const double u = (double)(t / s.steps_per_unit);
+  const double pi = 3.141592653589793;   // math.pi
+  if (s.kind == EQF_LR_TIMM_COSINE) {
+    // CosineLRScheduler._get_lr: warmup_lr_init + t * warmup_step, warmup_step = (base - warmup_lr_init) / warmup_t
+    if (u < s.warmup) return add_rn(s.warmup_start, mul_rn(u, (s.base_lr - s.warmup_start) / s.warmup));
+    // lr_min + 0.5 * (lr_max - lr_min) * (1 + math.cos(math.pi * t_curr / t_i)), first and only cycle
+    if (u < s.total)
+      return add_rn(s.min_value, mul_rn(mul_rn(0.5, s.base_lr - s.min_value), 1.0 + cos(mul_rn(pi, u) / s.total)));
+    return s.min_value;
+  }
+  double lambda;
+  if (u <= s.warmup) {
+    // alpha = current_step / float(warmup_epochs); lr_warmup_factor * (1.0 - alpha) + alpha
+    const double a = u / s.warmup;
+    lambda = add_rn(mul_rn(s.warmup_start, 1.0 - a), a);
+  } else if (s.kind == EQF_LR_OC20_MULTISTEP) {
+    int idx = 0;                                           // bisect(lr_decay_epochs, current_step)
+    for (int i = 0; i < s.n_milestones; ++i) idx += s.milestones[i] <= u;
+    lambda = pow(s.gamma, (double)idx);                    // pow(lr_gamma, idx)
+  } else if (u >= s.total) {
+    lambda = s.min_value;
+  } else {
+    // lr_min_factor + 0.5 * (1 - lr_min_factor) * (1 + math.cos(math.pi * (current_step / max_epochs)))
+    lambda = add_rn(s.min_value, mul_rn(mul_rn(0.5, 1.0 - s.min_value), 1.0 + cos(mul_rn(pi, u / s.total))));
+  }
+  return mul_rn(s.base_lr, lambda);                        // base_lr * lmbda(self.last_epoch)
+}
 
 struct AdamScalars {
   float coef, b1, one_m_b1, b2, one_m_b2, neg_lr, neg_step, sqrt_bc2, eps, ema_w;
@@ -139,7 +195,8 @@ __global__ void __launch_bounds__(kThreads) flat_adamw_kernel(AdamArgs a) {
   __shared__ bool last;
   if (threadIdx.x == 0) {
     const int64_t t = *a.step + 1;
-    const double lr = *a.lr;
+    // a scheduled rate is rounded to float as a rate written by set_lr() is
+    const double lr = a.sched.kind == EQF_LR_NONE ? (double)*a.lr : (double)(float)lr_at(a.sched, t - 1);
     sh.t = t;
     sh.coef = *a.coef;
     sh.b1 = (float)a.b1;
@@ -193,6 +250,7 @@ __global__ void __launch_bounds__(kThreads) flat_adamw_kernel(AdamArgs a) {
   __syncthreads();
   if (last && threadIdx.x == 0) {
     *a.step = s.t;
+    if (a.sched.kind != EQF_LR_NONE) *a.lr = (float)lr_at(a.sched, s.t);   // no CTA reads *lr in a scheduled step
     *a.tickets = 0;
   }
 }
@@ -220,6 +278,14 @@ extern "C" int eqf_flat_sqnorm(const float* g, int64_t n, float max_norm, double
   return check_launch("flat_sqnorm_kernel launch");
 }
 
+static int launch_adamw(const AdamArgs& a, void* stream) {
+  if (a.ema)
+    flat_adamw_kernel<true><<<grid_of(a.n), kThreads, 0, (cudaStream_t)stream>>>(a);
+  else
+    flat_adamw_kernel<false><<<grid_of(a.n), kThreads, 0, (cudaStream_t)stream>>>(a);
+  return check_launch("flat_adamw_kernel launch");
+}
+
 extern "C" int eqf_flat_adamw_check(const float* g, const float* p, const float* m, const float* v, const float* decay,
                                     const float* ema, int64_t n, const float* coef, const float* lr, const int64_t* step,
                                     double beta1, double beta2, const int32_t* tickets) {
@@ -236,10 +302,56 @@ extern "C" int eqf_flat_adamw(float* g, float* p, float* m, float* v, const floa
                               double ema_decay, int32_t* tickets, void* stream) {
   const int rc = eqf_flat_adamw_check(g, p, m, v, decay, ema, n, coef, lr, step, beta1, beta2, tickets);
   if (rc) return rc;
-  AdamArgs a{g, p, m, v, decay, ema, n, coef, lr, step, beta1, beta2, eps, (float)(1.0 - ema_decay), tickets};
-  if (ema)
-    flat_adamw_kernel<true><<<grid_of(n), kThreads, 0, (cudaStream_t)stream>>>(a);
-  else
-    flat_adamw_kernel<false><<<grid_of(n), kThreads, 0, (cudaStream_t)stream>>>(a);
-  return check_launch("flat_adamw_kernel launch");
+  AdamArgs a{g, p, m, v, decay, ema, n, coef, const_cast<float*>(lr), step, beta1, beta2, eps,
+             (float)(1.0 - ema_decay), tickets, EqfLrSchedule{}};
+  return launch_adamw(a, stream);
+}
+
+extern "C" int eqf_lr_schedule_check(const EqfLrSchedule* s) {
+  if (!s) return fail("eqf_lr_schedule: null descriptor");
+  const bool timm = s->kind == EQF_LR_TIMM_COSINE, multistep = s->kind == EQF_LR_OC20_MULTISTEP;
+  if (s->kind != EQF_LR_OC20_COSINE && !multistep && !timm) return fail("eqf_lr_schedule: unknown kind");
+  if (!std::isfinite(s->warmup) || (timm ? s->warmup < 0.0 : s->warmup <= 0.0))
+    return fail(timm ? "eqf_lr_schedule: the warm-up length must be finite and >= 0"
+                     : "eqf_lr_schedule: the warm-up length must be finite and positive (the warm-up divides by it)");
+  if (!multistep && !(std::isfinite(s->total) && s->total > 0.0))
+    return fail("eqf_lr_schedule: the total length must be finite and positive");
+  if (s->steps_per_unit < 1) return fail("eqf_lr_schedule: steps_per_unit must be at least 1");
+  if (s->n_milestones < 0 || s->n_milestones > EQF_LR_MAX_MILESTONES)
+    return fail("eqf_lr_schedule: at most EQF_LR_MAX_MILESTONES milestones");
+  for (int i = 0; i < s->n_milestones; ++i) {
+    if (!std::isfinite(s->milestones[i])) return fail("eqf_lr_schedule: milestones must be finite");
+    if (i && s->milestones[i] < s->milestones[i - 1]) return fail("eqf_lr_schedule: milestones must be sorted");
+  }
+  // every rate is base_lr times a value between the warm-up start, 1, the floor and gamma^k (OC20), or lies between
+  // warmup_start, base_lr and min_value (timm): non-negative finite parameters and a finite largest product suffice
+  const double pars[] = {s->base_lr, s->warmup_start, s->min_value, multistep ? s->gamma : 0.0};
+  for (double x : pars)
+    if (!(std::isfinite(x) && x >= 0.0)) return fail("eqf_lr_schedule: a parameter gives a negative or non-finite rate");
+  if (!timm) {
+    double top = s->warmup_start > 1.0 ? s->warmup_start : 1.0;
+    if (s->min_value > top) top = s->min_value;
+    if (multistep && s->gamma > 1.0) top = pow(s->gamma, (double)s->n_milestones);
+    if (!std::isfinite(s->base_lr * top)) return fail("eqf_lr_schedule: a parameter gives a negative or non-finite rate");
+  }
+  return 0;
+}
+
+extern "C" int eqf_lr_at(const EqfLrSchedule* s, int64_t t, double* out) {
+  const int rc = eqf_lr_schedule_check(s);
+  if (rc) return rc;
+  if (t < 0 || !out) return fail("eqf_lr_at: the step count must be >= 0 and out given");
+  *out = lr_at(*s, t);
+  return 0;
+}
+
+extern "C" int eqf_flat_adamw_scheduled(float* g, float* p, float* m, float* v, const float* decay, float* ema, int64_t n,
+                                        const float* coef, float* lr, int64_t* step, double beta1, double beta2,
+                                        float eps, double ema_decay, int32_t* tickets, const EqfLrSchedule* schedule,
+                                        void* stream) {
+  int rc = eqf_flat_adamw_check(g, p, m, v, decay, ema, n, coef, lr, step, beta1, beta2, tickets);
+  if (!rc) rc = eqf_lr_schedule_check(schedule);
+  if (rc) return rc;
+  AdamArgs a{g, p, m, v, decay, ema, n, coef, lr, step, beta1, beta2, eps, (float)(1.0 - ema_decay), tickets, *schedule};
+  return launch_adamw(a, stream);
 }

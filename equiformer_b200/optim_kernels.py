@@ -5,6 +5,7 @@ built on them is ``parallel.CapturableFlatAdamW``.
 """
 from __future__ import annotations
 
+import ctypes
 from typing import Optional
 
 import torch
@@ -43,11 +44,12 @@ def flat_sqnorm_raw(g: torch.Tensor, max_norm: float, partials: torch.Tensor, ti
 
 
 def flat_adamw_raw(g, p, m, v, decay, ema, coef, lr, step, betas, eps: float, ema_decay: Optional[float],
-                   tickets) -> None:
+                   tickets, schedule=None) -> None:
     """One AdamW step on the flat buffers ``g, p, m, v`` (``decay``: per-element weight decay), in place: ``g *= coef``,
     ``step += 1``, and ``ema`` (or None) moved toward the new ``p`` by ``1 - ema_decay``.  ``coef`` / ``lr`` are float32
     ``[1]`` and ``step`` int64 ``[1]`` device tensors, ``tickets`` an int32 ``[1]`` counter as in :func:`flat_sqnorm_raw`;
-    nothing is read from the host."""
+    nothing is read from the host.  With a ``schedule`` (``lr_schedule.LrSchedule``) the rate is the schedule's at the
+    step count before the step, and ``lr`` is left holding the next step's rate (``eqf_flat_adamw_scheduled``)."""
     n = p.numel()
     ptrs = [_flat(t, name, n) for t, name in ((g, "gradient"), (p, "parameters"), (m, "m"), (v, "v"), (decay, "decay"))]
     e = _flat(ema, "ema", n) if ema is not None else None
@@ -55,5 +57,8 @@ def flat_adamw_raw(g, p, m, v, decay, ema, coef, lr, step, betas, eps: float, em
             float(betas[0]), float(betas[1]), float(eps), float(ema_decay if ema is not None else 0.0),
             _flat(tickets, "tickets", 1, torch.int32))
     with torch.cuda.device(p.device), _kernel("flat_adamw", 4 * n * (10 if ema is None else 12)):
-        rc = _lib.load_optim().eqf_flat_adamw(*args, _stream())
-    _check(rc, "eqf_flat_adamw")
+        if schedule is None:
+            rc = _lib.load_optim().eqf_flat_adamw(*args, _stream())
+        else:
+            rc = _lib.load_optim().eqf_flat_adamw_scheduled(*args, ctypes.byref(schedule.descriptor), _stream())
+    _check(rc, "eqf_flat_adamw_scheduled" if schedule is not None else "eqf_flat_adamw")

@@ -276,8 +276,8 @@ class CapturableFlatAdamW(_AdamWStateDict):
     """:class:`FlatAdamW` with gradient-norm clipping and a model EMA, on the fused kernels of ``libeqf_b200_optim.so``.
 
     The learning rate ``lr`` and the step count ``t`` are device tensors, and :meth:`step` reads nothing from the host,
-    so the step can run inside a captured CUDA graph (the ``after_backward`` hook of the steps in ``graphs``) and a
-    schedule computed on the host changes the rate between replays through :meth:`set_lr`.
+    so the step can run inside a captured CUDA graph (the ``after_backward`` hook of the steps in ``graphs``).  The rate
+    follows an attached ``lr_schedule`` on the device, or changes between replays through :meth:`set_lr`.
 
     * ``max_grad_norm``: ``torch.nn.utils.clip_grad_norm_`` over the flat gradient before the update (the OC20 trainer's
       ``clip_grad_norm``, timm's ``dispatch_clip_grad(mode='norm')``).  The clipped gradient is left in the bucket, as
@@ -286,20 +286,28 @@ class CapturableFlatAdamW(_AdamWStateDict):
       parameters (in the AdamW kernel) and the floating-point buffers, a copy for the other buffers.
       :meth:`ema_state_dict` and :meth:`ema_weights` read it.
 
+    * ``lr_schedule``: an ``lr_schedule.LrSchedule``.  The kernel then takes each step's rate from the schedule at the
+      step count ``t`` and leaves the next step's rate in ``lr``, so a captured step follows the schedule replay by
+      replay with no host write; the schedule's base rate replaces ``lr``, and :meth:`set_lr` raises.  A loaded state
+      sets ``t``, and ``lr`` follows from it.  The scheduler state goes through :meth:`lr_schedule_state_dict` and
+      :meth:`load_lr_schedule_state_dict`.
+
     Across processes, call ``bucket.reduce()`` and then :meth:`step` eagerly, so the averaged gradient is clipped, as
     DDP with ``clip_grad_norm_`` does.
     """
 
     def __init__(self, named_params, bucket: FlatGradAllReduce, lr=5e-4, betas=(0.9, 0.999), eps=1e-8,
                  weight_decay=5e-3, no_decay=(), max_grad_norm: Optional[float] = None,
-                 ema_decay: Optional[float] = None, model: Optional[torch.nn.Module] = None):
+                 ema_decay: Optional[float] = None, model: Optional[torch.nn.Module] = None, lr_schedule=None):
         from . import optim_kernels
         if max_grad_norm is not None and not max_grad_norm > 0:
             raise ValueError("max_grad_norm must be positive")
         if ema_decay is not None and not (0.0 <= ema_decay <= 1.0 and model is not None):
             raise ValueError("ema_decay must be in [0, 1] and needs the model whose buffers the EMA follows")
         self.bucket, self.betas, self.eps = bucket, betas, eps
-        self.max_grad_norm, self.ema_decay = max_grad_norm, ema_decay
+        self.max_grad_norm, self.ema_decay, self.lr_schedule = max_grad_norm, ema_decay, lr_schedule
+        if lr_schedule is not None:
+            lr = lr_schedule.lr_at(0)
         self._names, self.flat, self.decay = flatten_parameters(named_params, bucket, weight_decay, no_decay)
         self._exempt = [is_no_decay(n, no_decay) for n in self._names]
         self._group_wd = (0.0, float(weight_decay))
@@ -330,10 +338,39 @@ class CapturableFlatAdamW(_AdamWStateDict):
 
     def set_lr(self, value: float) -> None:
         """Write the learning rate of the following steps (a device write: no capture is invalidated)."""
+        if self.lr_schedule is not None:
+            raise RuntimeError("set_lr: the attached lr_schedule sets the rate of every step")
         self.lr.fill_(float(value))
 
     def _lr_and_step(self):
-        return float(self.lr), int(self.t)
+        t = int(self.t)
+        return (float(self.lr) if self.lr_schedule is None else self.lr_schedule.lr_at(t)), t
+
+    def state_dict(self) -> dict:
+        """:meth:`_AdamWStateDict.state_dict`; with a schedule, the groups also hold the ``initial_lr`` that torch's
+        schedulers add, and ``lr`` is the schedule's rate at ``t`` in double."""
+        sd = super().state_dict()
+        if self.lr_schedule is not None:
+            for g in sd["param_groups"]:
+                g["initial_lr"] = self.lr_schedule.base_lr
+        return sd
+
+    def lr_schedule_state_dict(self) -> dict:
+        """The attached schedule's state at the current step count (``LrSchedule.state_dict``): for the OC20 kinds a
+        ``LambdaLR.state_dict()``, the reference checkpoint's ``scheduler`` entry."""
+        if self.lr_schedule is None:
+            raise RuntimeError("no lr_schedule: construct the optimiser with one")
+        return self.lr_schedule.state_dict(int(self.t))
+
+    def load_lr_schedule_state_dict(self, state: dict) -> None:
+        """Check a scheduler state (ours, or a reference checkpoint's ``scheduler``) against the attached schedule at the
+        loaded step count, after :meth:`load_state_dict`; a ``ValueError`` names the key that differs and nothing is
+        written.  The position is ``t``, so a fitting state leaves ``lr`` at the schedule's rate of step ``t``."""
+        if self.lr_schedule is None:
+            raise RuntimeError("no lr_schedule: construct the optimiser with one")
+        t = int(self.t)
+        self.lr_schedule.check_state_dict(state, t)
+        self.lr.fill_(self.lr_schedule.lr_at(t))
 
     def _set_hyper(self, lr, betas, eps, t):
         # betas and eps are arguments of the AdamW kernel launch, so a captured step holds the values it was captured
@@ -342,7 +379,9 @@ class CapturableFlatAdamW(_AdamWStateDict):
             raise ValueError(f"param_groups: betas {betas} / eps {eps} differ from this optimiser's {tuple(self.betas)} / "
                              f"{self.eps}; captured steps keep the values they were captured with, so construct "
                              "CapturableFlatAdamW with the state's betas and eps")
-        self.lr.fill_(lr)
+        # with a schedule the rate is a function of t: the groups' lr (the rate of step t in a reference checkpoint)
+        # is not adopted
+        self.lr.fill_(lr if self.lr_schedule is None else self.lr_schedule.lr_at(t))
         self.t.fill_(t)
 
     @torch.no_grad()
@@ -356,7 +395,7 @@ class CapturableFlatAdamW(_AdamWStateDict):
             optim_kernels.flat_sqnorm_raw(g, self.max_grad_norm, self._partials, self._tickets[0:1], self.grad_norm,
                                           self.coef)
         optim_kernels.flat_adamw_raw(g, self.flat, self.m, self.v, self.decay, self.ema, self.coef, self.lr, self.t,
-                                     self.betas, self.eps, self.ema_decay, self._tickets[1:2])
+                                     self.betas, self.eps, self.ema_decay, self._tickets[1:2], self.lr_schedule)
         if self.ema is not None:
             if self._lerp[0]:
                 torch._foreach_lerp_(*self._lerp, 1.0 - self.ema_decay)

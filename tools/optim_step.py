@@ -9,7 +9,9 @@ and of the OC20 E(3) model (``OC20_L1_256_E3_NONLINEAR``), seeded gradients:
   a) ``FlatAdamW.step()``;
   b) a) plus ``torch.nn.utils.clip_grad_norm_`` over the flat gradient (one tensor whose ``.grad`` is the bucket) and an
      EMA ``lerp_`` of the flat parameters;
-  c) ``CapturableFlatAdamW.step()`` with clipping and the EMA on (``eqf_flat_sqnorm`` + ``eqf_flat_adamw``).
+  c) ``CapturableFlatAdamW.step()`` with clipping and the EMA on (``eqf_flat_sqnorm`` + ``eqf_flat_adamw``);
+  d) c) with the OC20 cosine schedule of ``l1_256_nonlinear`` attached (``eqf_flat_adamw_scheduled``: the same kernel
+     instances, thread 0 of each CTA evaluating the rate).
 Each is timed with CUDA events over 10 x ``--steps`` eager steps.  ``max_norm`` is half the seeded gradient's norm; b) and
 c) share the gradient, so after the first clip its norm sits at ``max_norm`` and every later step scales it by
 ``max_norm / (norm + 1e-6)`` (the full clip arithmetic, a factor just below 1).
@@ -17,7 +19,8 @@ c) share the gradient, so after the first clip its norm sits at ``max_norm`` and
 Training step, ``bench.py --workload qm9`` batch (128 molecules, radius 5, attention dropout off): neighbour list + replay
 of ``GraphedForwardBackward`` (forward, L1 loss, backward), then
   eager:    ``FlatAdamW.step()`` after the replay;
-  captured: clip (max norm 5) + AdamW + EMA (decay 0.9999) inside the replayed graph (``after_backward``).
+  captured: clip (max norm 5) + AdamW + EMA (decay 0.9999) inside the replayed graph (``after_backward``);
+  captured_scheduled: the same with the OC20 cosine schedule attached (no host write between replays).
 Each step ends in a device synchronise.  The variants alternate for ``--rounds`` rounds in one process and the line reports
 each one's best round, with the card's name, power limit and SM clock read before and after.
 """
@@ -38,6 +41,15 @@ import bench  # noqa: E402
 from lmax4_step import _card, _no_dropout  # noqa: E402
 
 LR, WD, EMA_DECAY = 5e-4, 5e-3, 0.9999
+# the optim block of oc20/configs/is2re/all/graph_attention_transformer/l1_256_nonlinear_g@2_local.yml
+OC20_OPTIM = {"lr_initial": 0.0002, "max_epochs": 20, "scheduler": "LambdaLR",
+              "scheduler_params": {"lambda_type": "cosine", "warmup_factor": 0.2, "warmup_epochs": 2,
+                                   "lr_min_factor": 1.e-2}}
+
+
+def _oc20_schedule():
+    from equiformer_b200.lr_schedule import LrSchedule
+    return LrSchedule.from_oc20_optim(OC20_OPTIM, n_iter_per_epoch=1000)
 
 
 def _model(name, dev):
@@ -75,8 +87,11 @@ def optimiser_variants(name, dev):
 
     fused = CapturableFlatAdamW(model.named_parameters(), bucket, lr=LR, weight_decay=WD, no_decay=skip,
                                 max_grad_norm=max_norm, ema_decay=EMA_DECAY, model=model)
+    scheduled = CapturableFlatAdamW(model.named_parameters(), bucket, weight_decay=WD, no_decay=skip,
+                                    max_grad_norm=max_norm, ema_decay=EMA_DECAY, model=model,
+                                    lr_schedule=_oc20_schedule())
     return bucket.flat.numel(), {"flat_adamw": flat_adamw.step, "flat_adamw_torch_clip_ema": torch_chain,
-                                 "fused_clip_adamw_ema": fused.step}
+                                 "fused_clip_adamw_ema": fused.step, "fused_clip_adamw_ema_scheduled": scheduled.step}
 
 
 def _events(fn, steps, warmup):
@@ -96,7 +111,7 @@ def qm9_steps(dev, inp):
     from equiformer_b200.parallel import CapturableFlatAdamW, FlatAdamW, FlatGradAllReduce
     l1 = lambda out, tgt: (out - tgt).abs().mean()
     steps = {}
-    for variant in ("eager_adamw", "captured_clip_adamw_ema"):
+    for variant in ("eager_adamw", "captured_clip_adamw_ema", "captured_clip_adamw_ema_scheduled"):
         model = _model("qm9", dev)
         bucket = FlatGradAllReduce(model.parameters())
         skip = model.no_weight_decay()
@@ -105,8 +120,9 @@ def qm9_steps(dev, inp):
             gfb = GraphedForwardBackward(model, l1, bucket, max_radius=5.0)
             steps[variant] = lambda gfb=gfb, opt=opt: (gfb(inp["pos"], inp["batch"], inp["z"], inp["target"]), opt.step())
         else:
+            schedule = _oc20_schedule() if variant.endswith("_scheduled") else None
             opt = CapturableFlatAdamW(model.named_parameters(), bucket, lr=LR, weight_decay=WD, no_decay=skip,
-                                      max_grad_norm=5.0, ema_decay=EMA_DECAY, model=model)
+                                      max_grad_norm=5.0, ema_decay=EMA_DECAY, model=model, lr_schedule=schedule)
             gfb = GraphedForwardBackward(model, l1, bucket, max_radius=5.0, after_backward=opt.step)
             steps[variant] = lambda gfb=gfb: gfb(inp["pos"], inp["batch"], inp["z"], inp["target"])
     return steps
