@@ -36,6 +36,16 @@ EQF_OPTIM_THREADS = 256       # include/eqf_b200_optim.h: threads per CTA, 4 ele
 EQF_OPTIM_MAX_CTAS = 1024     # include/eqf_b200_optim.h: grid cap (and length of the partial-sum scratch)
 EQF_LR_MAX_MILESTONES = 8     # include/eqf_b200_optim.h: milestones of a multistep schedule
 EQF_LR_KINDS = {"oc20_cosine": 1, "oc20_multistep": 2, "timm_cosine": 3}   # EQF_LR_* of include/eqf_b200_optim.h
+# the metric terms of the evaluation passes (evaluation.EvalPass): their own library and header (include/eqf_b200_eval.h),
+# bound by load_eval()
+EVAL_LIB_PATH = PKG_DIR / "libeqf_b200_eval.so"
+EVAL_SOURCES = ("eqf_eval.cu",)
+EQF_EVAL_THREADS = 256        # include/eqf_b200_eval.h: threads per CTA, one row each per pass
+EQF_EVAL_MAX_CTAS = 128       # include/eqf_b200_eval.h: grid cap
+EQF_EVAL_SCRATCH = 512        # include/eqf_b200_eval.h: doubles of the partials scratch
+EQF_EVAL_GRAPH_SLOTS = 5      # include/eqf_b200_eval.h: accumulator slots of eqf_eval_graph / _atom / _batch
+EQF_EVAL_ATOM_SLOTS = 3
+EQF_EVAL_BATCH_SLOTS = 2
 SOURCES = ("eqf_abi.cu", "eqf_dtp.cu", "eqf_dtp_vec.cu", "eqf_attn.cu", "eqf_pointwise.cu", "eqf_gemm_tf32x3.cu", "eqf_graph.cu",
            "eqf_fused.cu", "eqf_edge.cu", "eqf_gemm_small.cu")
 
@@ -250,6 +260,18 @@ OPTIM_SIGNATURES = {
                                            POINTER(EqfLrSchedule), c_void_p]),
 }
 
+# every symbol include/eqf_b200_eval.h declares
+EVAL_SIGNATURES = {
+    "eqf_last_error": (c_char_p, []),
+    "eqf_eval_graph": (c_int32, [c_void_p, c_void_p, c_int64, c_float, c_float, c_float, c_void_p, c_void_p, c_void_p,
+                                 c_void_p]),
+    "eqf_eval_atom": (c_int32, [c_void_p, c_void_p, c_int64, c_void_p, c_float, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "eqf_eval_batch": (c_int32, [c_void_p, c_void_p, c_void_p]),
+    "eqf_eval_graph_check": (c_int32, [c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p]),
+    "eqf_eval_atom_check": (c_int32, [c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "eqf_eval_batch_check": (c_int32, [c_void_p, c_void_p]),
+}
+
 
 class EqfError(RuntimeError):
     pass
@@ -271,20 +293,21 @@ def generate_sources():
 
 
 def needs_build() -> bool:
-    libs = (LIB_PATH, L4_LIB_PATH, NORM_LIB_PATH, OPTIM_LIB_PATH)
+    libs = (LIB_PATH, L4_LIB_PATH, NORM_LIB_PATH, OPTIM_LIB_PATH, EVAL_LIB_PATH)
     if not all(p.exists() for p in libs):
         return True
     mtime = min(p.stat().st_mtime for p in libs)
-    deps = (sources() + [CSRC_DIR / s for s in NORM_SOURCES + OPTIM_SOURCES] + list(CSRC_DIR.glob("*.cuh"))
-            + [INCLUDE_DIR / "eqf_b200.h", INCLUDE_DIR / "eqf_b200_norm.h", INCLUDE_DIR / "eqf_b200_optim.h"])
+    deps = (sources() + [CSRC_DIR / s for s in NORM_SOURCES + OPTIM_SOURCES + EVAL_SOURCES] + list(CSRC_DIR.glob("*.cuh"))
+            + [INCLUDE_DIR / "eqf_b200.h", INCLUDE_DIR / "eqf_b200_norm.h", INCLUDE_DIR / "eqf_b200_optim.h",
+               INCLUDE_DIR / "eqf_b200_eval.h"])
     return any(p.stat().st_mtime > mtime for p in deps)
 
 
 def build(force: bool = False, verbose: bool = False) -> Path:
     """Compile ``csrc/*.cu`` for sm_90a into ``equiformer_b200/libeqf_b200.so``, ``L4_SOURCES`` with
     ``-DEQF_MAX_DEGREE=4`` into ``equiformer_b200/libeqf_b200_l4.so``, ``NORM_SOURCES`` into
-    ``equiformer_b200/libeqf_b200_norm.so`` and ``OPTIM_SOURCES`` into ``equiformer_b200/libeqf_b200_optim.so``
-    (in-tree)."""
+    ``equiformer_b200/libeqf_b200_norm.so``, ``OPTIM_SOURCES`` into ``equiformer_b200/libeqf_b200_optim.so`` and
+    ``EVAL_SOURCES`` into ``equiformer_b200/libeqf_b200_eval.so`` (in-tree)."""
     generate_sources()
     if not force and not needs_build():
         return LIB_PATH
@@ -298,7 +321,8 @@ def build(force: bool = False, verbose: bool = False) -> Path:
     obj_dir.mkdir(parents=True, exist_ok=True)
     compile_flags = [f for f in NVCC_FLAGS if f != "--shared"]
     jobs = ([(src, "", []) for src in sources()] + [(CSRC_DIR / s, "_l4", ["-DEQF_MAX_DEGREE=4"]) for s in L4_SOURCES]
-            + [(CSRC_DIR / s, "_norm", []) for s in NORM_SOURCES] + [(CSRC_DIR / s, "_optim", []) for s in OPTIM_SOURCES])
+            + [(CSRC_DIR / s, "_norm", []) for s in NORM_SOURCES] + [(CSRC_DIR / s, "_optim", []) for s in OPTIM_SOURCES]
+            + [(CSRC_DIR / s, "_eval", []) for s in EVAL_SOURCES])
 
     def compile_one(job):
         src, suffix, defines = job
@@ -328,6 +352,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
         link(L4_LIB_PATH, [o for o, suffix, _ in results if suffix == "_l4"])
         link(NORM_LIB_PATH, [o for o, suffix, _ in results if suffix == "_norm"])
         link(OPTIM_LIB_PATH, [o for o, suffix, _ in results if suffix == "_optim"])
+        link(EVAL_LIB_PATH, [o for o, suffix, _ in results if suffix == "_eval"])
     finally:
         shutil.rmtree(obj_dir, ignore_errors=True)
     return LIB_PATH
@@ -394,6 +419,11 @@ def load_norm():
 def load_optim():
     """Return the loaded optimiser library (``include/eqf_b200_optim.h``)."""
     return _load_side(OPTIM_LIB_PATH, OPTIM_SIGNATURES)
+
+
+def load_eval():
+    """Return the loaded evaluation-metric library (``include/eqf_b200_eval.h``)."""
+    return _load_side(EVAL_LIB_PATH, EVAL_SIGNATURES)
 
 
 def load():

@@ -138,7 +138,9 @@ class GraphedForwardBackward:
 class GraphedStep:
     """Generic capture / replay: ``fn(*static_tensors) -> loss`` (forward + loss of any model) is captured once per ``key``
     together with its backward (gradients stored into the flat bucket) and replayed on refreshed static buffers.  Used by
-    ``bench.py`` for the OC20 and periodic-cell workloads, whose neighbour search stays eager."""
+    ``bench.py`` for the OC20 and periodic-cell workloads, whose neighbour search stays eager.  With ``bucket=None`` the
+    step is forward only: ``fn`` is captured without a backward and the call returns what it returned
+    (``evaluation.EvalPass``)."""
 
     def __init__(self, fn: Callable[..., torch.Tensor], bucket, warmup: int = 3, max_cached: int = 8,
                  after_backward: Optional[Callable[[], None]] = None):
@@ -149,6 +151,8 @@ class GraphedStep:
 
     def _fwd_bwd(self, static) -> torch.Tensor:
         loss = self.fn(*static)
+        if self.bucket is None:
+            return loss
         self.bucket.store(torch.autograd.grad(loss, self.bucket.params, allow_unused=True))
         return loss.detach()
 
