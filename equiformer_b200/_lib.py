@@ -46,6 +46,12 @@ EQF_EVAL_SCRATCH = 512        # include/eqf_b200_eval.h: doubles of the partials
 EQF_EVAL_GRAPH_SLOTS = 5      # include/eqf_b200_eval.h: accumulator slots of eqf_eval_graph / _atom / _batch
 EQF_EVAL_ATOM_SLOTS = 3
 EQF_EVAL_BATCH_SLOTS = 2
+# the de-normalised OC20 predictions of a predict pass (evaluation.EvalPass.predict): their own library and header
+# (include/eqf_b200_predict.h), bound by load_predict()
+PREDICT_LIB_PATH = PKG_DIR / "libeqf_b200_predict.so"
+PREDICT_SOURCES = ("eqf_predict.cu",)
+EQF_PREDICT_THREADS = 256     # include/eqf_b200_predict.h: threads per CTA, one row each per pass
+EQF_PREDICT_MAX_CTAS = 128    # include/eqf_b200_predict.h: grid cap
 SOURCES = ("eqf_abi.cu", "eqf_dtp.cu", "eqf_dtp_vec.cu", "eqf_attn.cu", "eqf_pointwise.cu", "eqf_gemm_tf32x3.cu", "eqf_graph.cu",
            "eqf_fused.cu", "eqf_edge.cu", "eqf_gemm_small.cu")
 
@@ -272,6 +278,14 @@ EVAL_SIGNATURES = {
     "eqf_eval_batch_check": (c_int32, [c_void_p, c_void_p]),
 }
 
+# every symbol include/eqf_b200_predict.h declares
+PREDICT_SIGNATURES = {
+    "eqf_last_error": (c_char_p, []),
+    "eqf_predict_is2re": (c_int32, [c_void_p, c_int64, c_float, c_float, c_void_p, c_void_p, c_void_p, c_int64, c_float,
+                                    c_void_p, c_void_p, c_void_p]),
+    "eqf_predict_is2re_check": (c_int32, [c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p]),
+}
+
 
 class EqfError(RuntimeError):
     pass
@@ -293,21 +307,23 @@ def generate_sources():
 
 
 def needs_build() -> bool:
-    libs = (LIB_PATH, L4_LIB_PATH, NORM_LIB_PATH, OPTIM_LIB_PATH, EVAL_LIB_PATH)
+    libs = (LIB_PATH, L4_LIB_PATH, NORM_LIB_PATH, OPTIM_LIB_PATH, EVAL_LIB_PATH, PREDICT_LIB_PATH)
     if not all(p.exists() for p in libs):
         return True
     mtime = min(p.stat().st_mtime for p in libs)
-    deps = (sources() + [CSRC_DIR / s for s in NORM_SOURCES + OPTIM_SOURCES + EVAL_SOURCES] + list(CSRC_DIR.glob("*.cuh"))
+    deps = (sources() + [CSRC_DIR / s for s in NORM_SOURCES + OPTIM_SOURCES + EVAL_SOURCES + PREDICT_SOURCES]
+            + list(CSRC_DIR.glob("*.cuh"))
             + [INCLUDE_DIR / "eqf_b200.h", INCLUDE_DIR / "eqf_b200_norm.h", INCLUDE_DIR / "eqf_b200_optim.h",
-               INCLUDE_DIR / "eqf_b200_eval.h"])
+               INCLUDE_DIR / "eqf_b200_eval.h", INCLUDE_DIR / "eqf_b200_predict.h"])
     return any(p.stat().st_mtime > mtime for p in deps)
 
 
 def build(force: bool = False, verbose: bool = False) -> Path:
     """Compile ``csrc/*.cu`` for sm_90a into ``equiformer_b200/libeqf_b200.so``, ``L4_SOURCES`` with
     ``-DEQF_MAX_DEGREE=4`` into ``equiformer_b200/libeqf_b200_l4.so``, ``NORM_SOURCES`` into
-    ``equiformer_b200/libeqf_b200_norm.so``, ``OPTIM_SOURCES`` into ``equiformer_b200/libeqf_b200_optim.so`` and
-    ``EVAL_SOURCES`` into ``equiformer_b200/libeqf_b200_eval.so`` (in-tree)."""
+    ``equiformer_b200/libeqf_b200_norm.so``, ``OPTIM_SOURCES`` into ``equiformer_b200/libeqf_b200_optim.so``,
+    ``EVAL_SOURCES`` into ``equiformer_b200/libeqf_b200_eval.so`` and ``PREDICT_SOURCES`` into
+    ``equiformer_b200/libeqf_b200_predict.so`` (in-tree)."""
     generate_sources()
     if not force and not needs_build():
         return LIB_PATH
@@ -322,7 +338,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
     compile_flags = [f for f in NVCC_FLAGS if f != "--shared"]
     jobs = ([(src, "", []) for src in sources()] + [(CSRC_DIR / s, "_l4", ["-DEQF_MAX_DEGREE=4"]) for s in L4_SOURCES]
             + [(CSRC_DIR / s, "_norm", []) for s in NORM_SOURCES] + [(CSRC_DIR / s, "_optim", []) for s in OPTIM_SOURCES]
-            + [(CSRC_DIR / s, "_eval", []) for s in EVAL_SOURCES])
+            + [(CSRC_DIR / s, "_eval", []) for s in EVAL_SOURCES] + [(CSRC_DIR / s, "_predict", []) for s in PREDICT_SOURCES])
 
     def compile_one(job):
         src, suffix, defines = job
@@ -353,6 +369,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
         link(NORM_LIB_PATH, [o for o, suffix, _ in results if suffix == "_norm"])
         link(OPTIM_LIB_PATH, [o for o, suffix, _ in results if suffix == "_optim"])
         link(EVAL_LIB_PATH, [o for o, suffix, _ in results if suffix == "_eval"])
+        link(PREDICT_LIB_PATH, [o for o, suffix, _ in results if suffix == "_predict"])
     finally:
         shutil.rmtree(obj_dir, ignore_errors=True)
     return LIB_PATH
@@ -424,6 +441,11 @@ def load_optim():
 def load_eval():
     """Return the loaded evaluation-metric library (``include/eqf_b200_eval.h``)."""
     return _load_side(EVAL_LIB_PATH, EVAL_SIGNATURES)
+
+
+def load_predict():
+    """Return the loaded prediction library (``include/eqf_b200_predict.h``)."""
+    return _load_side(PREDICT_LIB_PATH, PREDICT_SIGNATURES)
 
 
 def load():

@@ -53,6 +53,22 @@ def match_state_dict(state: dict, target: dict) -> dict:
     return {k: renamed[k] for k in target}
 
 
+def atomic_write(path, write) -> None:
+    """Call ``write(f)`` on a binary file opened under a temporary name in ``path``'s directory, fsync it and rename it
+    over ``path``, so an interrupted write leaves the previous file intact.  The temporary file is removed on failure."""
+    path = os.fspath(path)
+    tmp = f"{path}.tmp{os.getpid()}"
+    try:
+        with open(tmp, "wb") as f:
+            write(f)
+            f.flush()
+            os.fsync(f.fileno())
+        os.replace(tmp, path)
+    finally:
+        if os.path.exists(tmp):
+            os.remove(tmp)
+
+
 def _rng_state(generators) -> dict:
     return {"cpu": torch.get_rng_state(),
             "cuda": torch.cuda.get_rng_state() if torch.cuda.is_available() else None,
@@ -83,17 +99,7 @@ def save_training_state(path, model: torch.nn.Module, optimizer, *, epoch: int, 
         if getattr(optimizer, "ema", None) is not None:
             ckpt["state_dict_ema"] = optimizer.ema_state_dict()
         ckpt["rng"] = states
-        path = os.fspath(path)
-        tmp = f"{path}.tmp{os.getpid()}"
-        try:
-            with open(tmp, "wb") as f:
-                torch.save(ckpt, f)
-                f.flush()
-                os.fsync(f.fileno())
-            os.replace(tmp, path)
-        finally:
-            if os.path.exists(tmp):
-                os.remove(tmp)
+        atomic_write(path, lambda f: torch.save(ckpt, f))
     if distributed:
         dist.barrier()
 

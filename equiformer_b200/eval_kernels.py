@@ -12,6 +12,10 @@ The accumulator is a float64 tensor of slots; each launcher adds to the slots it
 
 The kernels are the only implementation the evaluation passes use.  The ``*_torch`` functions state the same terms in
 torch with the same arguments (without the scratch): they are the tests' reference and the accumulator of the CPU tests.
+
+:func:`predict_is2re_raw` launches the one kernel of ``libeqf_b200_predict.so`` (``include/eqf_b200_predict.h``): the
+de-normalised energies and, optionally, predicted positions of a predict pass, stated in torch by
+:func:`predict_is2re_torch`.
 """
 from __future__ import annotations
 
@@ -123,3 +127,54 @@ def eval_batch_torch(loss, acc: torch.Tensor) -> None:
     """:func:`eval_batch_raw` in torch."""
     l = torch.zeros((), dtype=torch.float64) if loss is None else loss.detach().reshape(()).double().cpu()
     acc += torch.stack([l, torch.tensor(1.0, dtype=torch.float64)]).to(acc.device)
+
+
+# ------------------------------------------------------------------------------------------------ predictions
+def predict_is2re_raw(energy: torch.Tensor, n_graphs: int, mean: float, std: float, energy_out: torch.Tensor,
+                      pos: Optional[torch.Tensor] = None, delta: Optional[torch.Tensor] = None,
+                      tags: Optional[torch.Tensor] = None, pos_std: float = 1.0,
+                      pos_out: Optional[torch.Tensor] = None) -> None:
+    """Write ``energy[:n_graphs] * std + mean`` into ``energy_out`` (float32, ``n_graphs`` or more rows of one element
+    each) and, when ``delta`` is given, ``pos + (delta * pos_std + 0)`` on the rows with ``tags > 0`` and ``pos`` on the
+    others into ``pos_out`` (``pos``, ``delta``, ``pos_out`` float32 ``[rows, 3]``, ``tags`` int64 ``[rows]``).  Rows past
+    ``n_graphs`` of ``energy_out`` are left as they are."""
+    n = int(n_graphs)
+    with_pos = delta is not None
+    if with_pos != (pos is not None) or with_pos != (tags is not None) or with_pos != (pos_out is not None):
+        raise _lib.EqfError("pos, delta, tags and pos_out are given together or not at all")
+    rows = 0
+    if with_pos:
+        rows = pos.shape[0] if pos.dim() == 2 else -1
+        for name, t in (("pos", pos), ("delta", delta), ("pos_out", pos_out)):
+            if t.dim() != 2 or t.shape[1] != 3 or t.shape[0] != rows:
+                raise _lib.EqfError(f"pos, delta and pos_out must all be [rows, 3], got {name} {tuple(t.shape)}")
+    args = (_flat(energy, "energy", torch.float32, n, at_least=True), n, float(mean), float(std),
+            _flat(pos, "pos", torch.float32) if with_pos else None,
+            _flat(delta, "delta", torch.float32) if with_pos else None,
+            _flat(tags, "tags", torch.int64, rows) if with_pos else None, rows, float(pos_std),
+            _flat(energy_out, "energy_out", torch.float32, n, at_least=True),
+            _flat(pos_out, "pos_out", torch.float32) if with_pos else None)
+    dev = energy_out.device
+    for name, t in (("energy", energy), ("energy_out", energy_out), ("pos", pos), ("delta", delta), ("tags", tags),
+                    ("pos_out", pos_out)):
+        if t is not None and (not t.is_cuda or t.device != dev):
+            raise _lib.EqfError(f"{name} lives on {t.device}: the prediction kernel is CUDA-only (sm_90a) and takes every "
+                                f"buffer on energy_out's device ({dev})")
+    lib = _lib.load_predict()
+    with torch.cuda.device(dev), _kernel("predict_is2re", 8 * n + 32 * rows):
+        rc = lib.eqf_predict_is2re(*args, _stream())
+    _lib.check(rc, "eqf_predict_is2re", lib)
+
+
+def predict_is2re_torch(energy, n_graphs: int, mean: float, std: float, pos=None, delta=None, tags=None,
+                        pos_std: float = 1.0):
+    """:func:`predict_is2re_raw` in torch, in the reference's operations: ``Normalizer.denorm`` (``tensor * std + mean``)
+    of the energy, the positions normaliser's ``denorm`` (mean 0) of ``delta`` and ``pred_pos[mask] + delta_pos[mask]``
+    over ``tags > 0`` (``energy_trainer_v2.predict``).  Returns the energies ``[n_graphs]`` and the positions (or None)."""
+    e = energy.reshape(-1)[:int(n_graphs)] * std + mean
+    if delta is None:
+        return e, None
+    p = pos.clone()
+    m = tags > 0
+    p[m] = p[m] + (delta * pos_std + 0.0)[m]
+    return e, p

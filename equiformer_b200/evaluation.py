@@ -28,16 +28,25 @@ The captures hold the addresses of the parameters and buffers.  ``CapturableFlat
 ``checkpoint.load_training_state`` write the weights in place, so ``with opt.ema_weights(): ev.run(loader)`` evaluates
 the EMA through the same captures, and a pass after a load evaluates the loaded weights.  Loading a state dict by
 reassigning parameters would leave the captures reading the old storage.
+
+:meth:`EvalPass.predict` is the OC20 trainer's ``predict`` (``energy_trainer_v2.py:134-225``) on the same padding and
+captures: per bucket, the forward and ``eqf_predict_is2re`` of ``libeqf_b200_predict.so``, which de-normalises the energy
+and, with ``write_pos``, adds the auxiliary head's de-normalised displacement to the moving atoms.  The batches need no
+labels.  :func:`save_predictions` and :func:`save_pos_predictions` write the reference's results files.
 """
 from __future__ import annotations
 
+import os
+from collections import defaultdict
 from typing import Dict, Iterable, Optional
 
+import numpy as np
 import torch
 import torch.distributed as dist
 
 from . import _lib
-from .eval_kernels import eval_atom_raw, eval_batch_raw, eval_graph_raw, new_scratch
+from .checkpoint import atomic_write
+from .eval_kernels import eval_atom_raw, eval_batch_raw, eval_graph_raw, new_scratch, predict_is2re_raw
 from .graph import radius_graph_csr, radius_graph_pbc
 from .graphs import GraphedStep, csr_graph, pad_to_bucket
 
@@ -87,7 +96,8 @@ def pad_oc20(pos, batch, atomic_numbers, tags, src, dst, edge_vec, n_graphs: int
 
 
 class EvalPass:
-    """One evaluation pass of ``model`` over a loader: ``run(loader)`` returns the metrics (module docstring).
+    """One evaluation pass of ``model`` over a loader: ``run(loader)`` returns the metrics (module docstring), and for
+    ``oc20_is2re`` ``predict(loader)`` the de-normalised predictions of an unlabelled split.
 
     * ``task``: ``"qm9"`` (``GraphAttentionTransformer``), ``"md17"`` (the MD17 models and ``Equiformer_MD17_DeNS``,
       evaluated on clean data) or ``"oc20_is2re"`` (``GraphAttentionTransformerOC20``, with or without the auxiliary head).
@@ -130,10 +140,16 @@ class EvalPass:
         fn = {"qm9": self._qm9, "md17": self._md17, "oc20_is2re": self._oc20}[task]
         self._fn = fn
         self._graphed = GraphedStep(fn, None, warmup=warmup, max_cached=max_cached) if self.capture else None
+        self._predicting = (GraphedStep(self._oc20_predict, None, warmup=warmup, max_cached=max_cached)
+                            if self.capture and task == "oc20_is2re" else None)
 
     @property
     def captures(self) -> int:
         return 0 if self._graphed is None else self._graphed.captures
+
+    @property
+    def predict_captures(self) -> int:
+        return 0 if self._predicting is None else self._predicting.captures
 
     def set_aux_weight(self, value: float) -> None:
         """The weight of the OC20 auxiliary loss in the following passes (a device write: no capture is invalidated)."""
@@ -154,23 +170,72 @@ class EvalPass:
             reduce_accumulator(self.acc, self.group)
         return metrics_from_accumulator(self.task, self.acc)
 
+    def predict(self, loader: Iterable, write_pos: bool = False) -> dict:
+        """The OC20 trainer's ``predict(loader, per_image=True)``: ``{"id": [str(sid), ...], "energy": [float, ...]}`` in
+        loader order, the energies de-normalised with ``task_mean`` / ``task_std``.  With ``write_pos`` (the auxiliary
+        head only) also ``"pos": {sid: float32 [natoms, 3] CPU tensor}``: the input positions plus the head's
+        displacement times ``positions_std`` on the atoms with ``tags > 0``.
+
+        Batches are read by attribute: ``pos``, ``batch``, ``atomic_numbers``, ``tags``, ``cell``, ``natoms`` and ``sid``;
+        the frame count is ``natoms.numel()``.  The results stay on the device until the end of the pass, which reads
+        them once.  Mode, weights and generator states are left as :meth:`run` leaves them."""
+        if self.task != "oc20_is2re":
+            raise ValueError(f"predict is the OC20 IS2RE trainer's pass; this EvalPass is for {self.task!r}")
+        if write_pos and not self.aux:
+            raise ValueError("write_pos needs the auxiliary head (use_auxiliary_task=True): it predicts the positions")
+        was_training = self.model.training
+        sids, natoms, energies, positions = [], [], [], []
+        self.model.eval()
+        try:
+            with torch.random.fork_rng(devices=[self.device] if self.device.type == "cuda" else []):
+                for batch in loader:
+                    n_atoms = self._get(batch, "natoms").reshape(-1)
+                    G = int(n_atoms.numel())
+                    pos, padded, (Nb, Eb) = self._oc20_inputs(batch, G)
+                    tensors = [*padded, n_atoms]
+                    if write_pos:
+                        tensors.append(torch.cat([pos.float(), pos.new_zeros(Nb - pos.shape[0], 3, dtype=torch.float32)]))
+                    if self._predicting is not None:
+                        energy, pos_out = self._predicting((Nb, Eb, G, write_pos), tensors)
+                    else:
+                        energy, pos_out = self._oc20_predict(*tensors)
+                    energies.append(energy.clone())
+                    if write_pos:
+                        positions.append(pos_out[:pos.shape[0]].clone())
+                        natoms.append(n_atoms)
+                    sids.append(batch.sid)
+        finally:
+            self.model.train(was_training)
+        out = {"id": [str(i) for s in sids for i in torch.as_tensor(s).reshape(-1).tolist()],
+               "energy": torch.cat(energies).tolist() if energies else []}
+        if write_pos:
+            split = torch.split(torch.cat(positions).cpu(), torch.cat(natoms).tolist()) if positions else ()
+            out["pos"] = {sid: p.clone() for sid, p in zip(out["id"], split)}
+        return out
+
     # ------------------------------------------------------------------------------------------ per batch (eager)
     def _get(self, batch, name):
         return getattr(batch, name).to(self.device)
 
+    def _oc20_inputs(self, batch, n_graphs: int):
+        """The eager part of an OC20 batch: the periodic neighbour list, ``edge_vec`` with the image offsets, and
+        :func:`pad_oc20`.  Returns ``(pos, padded, (atoms_b, edges_b))``."""
+        pos, b, cell = self._get(batch, "pos"), self._get(batch, "batch"), self._get(batch, "cell")
+        z, tags = self._get(batch, "atomic_numbers").long(), self._get(batch, "tags").long()
+        edge, offs, _ = radius_graph_pbc(pos, b, cell, self.max_radius, self.max_neighbors)
+        src, dst = edge[0], edge[1]
+        cells = cell.to(pos.dtype).index_select(0, b.index_select(0, dst))
+        edge_vec = (pos.index_select(0, src) - pos.index_select(0, dst)
+                    + torch.bmm(offs.to(pos.dtype).view(-1, 1, 3), cells).view(-1, 3))
+        padded, bucket = pad_oc20(pos, b, z, tags, src, dst, edge_vec, n_graphs, self.aq, self.eq)
+        return pos, padded, bucket
+
     def _update(self, batch) -> None:
         dev = self.device
         if self.task == "oc20_is2re":
-            pos, b, cell = self._get(batch, "pos"), self._get(batch, "batch"), self._get(batch, "cell")
-            z, tags = self._get(batch, "atomic_numbers").long(), self._get(batch, "tags").long()
             y = self._get(batch, "y_relaxed").reshape(-1).float().contiguous()
             G = int(y.shape[0])
-            edge, offs, _ = radius_graph_pbc(pos, b, cell, self.max_radius, self.max_neighbors)
-            src, dst = edge[0], edge[1]
-            cells = cell.to(pos.dtype).index_select(0, b.index_select(0, dst))
-            edge_vec = (pos.index_select(0, src) - pos.index_select(0, dst)
-                        + torch.bmm(offs.to(pos.dtype).view(-1, 1, 3), cells).view(-1, 3))
-            padded, (Nb, Eb) = pad_oc20(pos, b, z, tags, src, dst, edge_vec, G, self.aq, self.eq)
+            pos, padded, (Nb, Eb) = self._oc20_inputs(batch, G)
             tensors = [padded[0], y, *padded[1:]]
             if self.aux:
                 from .oc20_objective import relaxation_target
@@ -236,3 +301,77 @@ class EvalPass:
         acc = self._slots()
         self._graph_terms(energy, y, acc)
         eval_batch_raw(loss.float().reshape(1), acc[_A:])
+
+    def _oc20_predict(self, edge_vec, batch, z, tags, src, dst, row_ptr, n_atoms, *pos):
+        """Captured per bucket: the forward, then the de-normalised energies ``[G]`` and, given the padded positions,
+        the predicted positions ``[atoms_b, 3]`` (the dummy atoms, tag 0, keep their input rows)."""
+        G = n_atoms.shape[0]
+        with torch.no_grad():
+            out = self.model.forward_edges(edge_vec, batch, z, tags, src, dst,
+                                           graph=csr_graph(src, dst, row_ptr, batch.shape[0]), n_graphs=G + 1)
+        energy, aux = out if isinstance(out, tuple) else (out, None)
+        energy_out = torch.empty(G, dtype=torch.float32, device=edge_vec.device)
+        if not pos:
+            predict_is2re_raw(energy.reshape(-1), G, self.mean, self.std, energy_out)
+            return energy_out, None
+        pos_out = torch.empty_like(pos[0])
+        predict_is2re_raw(energy.reshape(-1), G, self.mean, self.std, energy_out, pos[0], aux.contiguous(), tags,
+                          self.positions_std, pos_out)
+        return energy_out, pos_out
+
+
+# ------------------------------------------------------------------------------------------------ results files
+def _rank_world():
+    distributed = dist.is_initialized() and dist.get_world_size() > 1
+    return (dist.get_rank(), dist.get_world_size(), True) if distributed else (0, 1, False)
+
+
+def save_predictions(predictions: dict, results_dir, results_file: str = "predictions", name: str = "is2re") -> str:
+    """The OC20 trainer's ``save_results(predictions, results_file, keys=["energy"])`` (``base_trainer_oc20.py:707-757``).
+
+    Every process writes its ``{name}_{results_file}_{rank}.npz`` (``ids`` as a numpy string array, ``energy`` as the
+    float64 array numpy makes of the floats), then waits for the others.  Rank 0 reads the files in rank order, removes
+    them, keeps each id once with ``np.unique(ids, return_index=True)`` (so the ids come out sorted as strings; a
+    ``DistributedSampler`` repeats samples to even out the ranks) and writes ``{name}_{results_file}.npz``.  Every
+    process returns its path once it is written.  Files are written under a temporary name and renamed."""
+    rank, world, distributed = _rank_world()
+    path_of = lambda suffix: os.path.join(os.fspath(results_dir), f"{name}_{results_file}{suffix}.npz")
+    atomic_write(path_of(f"_{rank}"), lambda f: np.savez_compressed(f, ids=predictions["id"],
+                                                                    energy=predictions["energy"]))
+    if distributed:
+        dist.barrier()
+    if rank == 0:
+        gathered = defaultdict(list)
+        for i in range(world):
+            with np.load(path_of(f"_{i}"), allow_pickle=True) as r:
+                gathered["ids"].extend(r["ids"])
+                gathered["energy"].extend(r["energy"])
+            os.remove(path_of(f"_{i}"))
+        _, idx = np.unique(gathered["ids"], return_index=True)
+        result = {k: np.array(v)[idx] for k, v in gathered.items()}
+        atomic_write(path_of(""), lambda f: np.savez_compressed(f, **result))
+    if distributed:
+        dist.barrier()
+    return path_of("")
+
+
+def save_pos_predictions(pos: dict, run_dir) -> str:
+    """The ``write_pos`` files of the OC20 trainer's ``predict`` (``energy_trainer_v2.py:208-222``): every process writes
+    ``pos_pred_{rank}.pt`` (``{sid: [natoms, 3] tensor}``, kept afterwards), then rank 0 gathers them in rank order into
+    ``pos_pred.pt``, the first occurrence of an id winning.  Every process returns its path once it is written."""
+    rank, world, distributed = _rank_world()
+    run_dir = os.fspath(run_dir)
+    atomic_write(os.path.join(run_dir, f"pos_pred_{rank}.pt"), lambda f: torch.save(pos, f))
+    if distributed:
+        dist.barrier()
+    full = os.path.join(run_dir, "pos_pred.pt")
+    if rank == 0:
+        gathered = {}
+        for i in range(world):
+            for k, v in torch.load(os.path.join(run_dir, f"pos_pred_{i}.pt")).items():
+                if k not in gathered:
+                    gathered[k] = v
+        atomic_write(full, lambda f: torch.save(gathered, f))
+    if distributed:
+        dist.barrier()
+    return full
